@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- learner env-frames/sec of the V-trace hot path on B200.
+"""bench.py -- learner env-frames/sec of the V-trace hot path on H100.
 
   python bench.py --gpus N --steps K --warmup W            (this framework, CUDA)
   python bench.py --impl reference --gpus N --steps K ...  (the reference's algorithm on
@@ -26,7 +26,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = 'env-frames/sec (learner, device-timed) on synthetic 84x84x4 T=20 unrolls @1/2/4/8 B200'
+METRIC = 'env-frames/sec (learner, device-timed) on synthetic 84x84x4 T=20 unrolls @1/2/4/8 H100'
 UNIT = 'env-frames/s'
 A = 18
 OBS = (84, 84, 4)
@@ -47,12 +47,18 @@ def parse_args():
   p.add_argument('--cpu-batch', type=int, default=0,
                  help='unrolls per CPU-baseline step (0 = the same batch as the GPU arm)')
   p.add_argument('--conv', default='tc3p', choices=['simt', 'tc', 'tc3', 'tc3p'],
-                 help="contraction path of the convs and dense layers: fp32 SIMT, tcgen05 bf16, "
-                      "tcgen05 bf16x3 (fp32-faithful split operands), or tc3p = bf16x3 on HBM-resident "
+                 help="contraction path of the convs and dense layers: fp32 SIMT, wgmma bf16, "
+                      "wgmma bf16x3 (fp32-faithful split operands), or tc3p = bf16x3 on HBM-resident "
                       "operand planes with TMA-fed warp-specialised kernels (deep net; the default)")
   p.add_argument('--no-extras', action='store_true',
                  help='skip the profiling pass, the loss-kernel sweep and the CPU baseline')
+  p.add_argument('--dump-outputs', metavar='DIR', default=None,
+                 help='after the timed steps, write what the last timed step computed (loss, loss terms, '
+                      'gradients, updated parameters) as DIR/<name>.npy; the inputs are seeded, so two builds '
+                      'can be compared output for output')
   a = p.parse_args()
+  if a.dump_outputs and a.impl == 'reference':
+    p.error('--dump-outputs writes what the CUDA path computed; it does not apply to --impl reference')
   if a.net == 'shallow' and a.conv == 'tc3p':
     a.conv = 'tc3'
   if a.cpu_batch <= 0:
@@ -129,7 +135,7 @@ def workload_config(args, n):
       'optimizer': 'Adam lr=4.8e-4 beta1=0 eps=3.125e-7 (dmlab/vtrace_main.py:46-51)',
       'loss': 'gamma=0.99 lambda=1 baseline_cost=0.5 entropy_cost=2.5e-4 kl_cost=0',
       'grad_reduce': 'sum', 'parallelism': 'dp%d' % n,
-      'l2': 'per-step inputs (37.9 MB uint8 frames) + activations (>2 GB) exceed the 126 MB L2; '
+      'l2': 'per-step inputs (37.9 MB uint8 frames) + activations (>2 GB) exceed the 50 MB L2; '
             'no explicit flush'}
 
 
@@ -340,7 +346,7 @@ def inference_path_bench(agent, iters=200, warmup=30, N=64, num_envs=256, T=20, 
       'training_batches_assembled': len(stop),
       'bound': 'latency: 64 frames x 0.11 GFLOP = 7 GFLOP and 1.8 MB of frames per batch are ~10 us of '
                'tensor / HBM time; the step is a chain of ~40 dependent small kernels (each pays its launch + '
-               'setup: TMEM allocation, weights into shared memory) + 1.8 MB H2D + host bookkeeping; replaying it '
+               'setup: weights into shared memory) + 1.8 MB H2D + host bookkeeping; replaying it '
                'as a CUDA graph removes the CPU issue cost but not the dependent-kernel chain (measured: same '
                'p50), so throughput scales with the inference batch size instead',
   }
@@ -441,7 +447,7 @@ def r2d2_cpu_throughput(B, steps, warmup, burn_in=40, unroll=100):
 
 
 def run_r2d2(args):
-  """BASELINE configs[4]: R2D2 LSTM agent, synthetic replay, n-step targets, 1 x B200.  A step =
+  """BASELINE configs[4]: R2D2 LSTM agent, synthetic replay, n-step targets, 1 x H100.  A step =
   insert `batch/replay_ratio` new unrolls into the prioritized replay -> sample `batch` unrolls by
   priority (+ importance weights) -> burn-in + suffix unrolls of the online and target networks ->
   n-step double-DQN loss -> backward -> global-norm clip -> Adam -> priority write-back
@@ -500,12 +506,15 @@ def run_r2d2(args):
   while not feeder.ready() or replay.num_inserted < st.replay_buffer_size:
     feeder.insert(dev_new)
 
+  last_out = [None]
+
   def one_step(from_host):
     new = utils.map_structure(lambda t: t.cuda(non_blocking=True), host_new) if from_host else dev_new
     feeder.insert(new)
     sampled = feeder.sample()
     loss, priorities, indices, norm = step.minimize(sampled)
     feeder.update_priorities(indices, priorities)
+    last_out[0] = (loss, priorities, indices, norm)
     return loss
 
   def timed(fn, k):
@@ -526,6 +535,10 @@ def run_r2d2(args):
   launches = (_lib.launch_count() - n0) // args.steps
   agent.check_errors()
   clocks = sampler.stop()
+  if args.dump_outputs:
+    loss, priorities, indices, norm = last_out[0]
+    dump_outputs(args.dump_outputs, {'loss': loss, 'priorities': priorities, 'indices': indices,
+                                     'grad_norm': norm, 'parameters': agent.params})
   ms_e2e = timed(lambda: float(one_step(True)), args.steps)
   frames = B * st.unroll_length
   line = {'metric': R2D2_METRIC, 'value': frames / (ms * 1e-3), 'unit': UNIT, 'n_gpus': 1, 'steps': args.steps,
@@ -547,8 +560,8 @@ def run_r2d2(args):
     _lib.check(L.seedrl_profile_end(ms_c, n_c))
     line['kernel_time_ms_per_step'] = {L.seedrl_profile_category_name(i).decode(): round(ms_c[i], 4) for i in range(ncat)}
     line['kernel_time_note'] = ('conv3x3_fwd = im2col, conv3x3_dgrad = col2im, sgemm = every GEMM incl. the three '
-                                'convolutions (tcgen05 bf16x3), lstm_pointwise = the persistent LSTM(512) recurrences')
-    # roofline of the dominant family: the tcgen05 GEMMs, against the dense bf16 peak x 1/3 (bf16x3)
+                                'convolutions (wgmma bf16x3), lstm_pointwise = the persistent LSTM(512) recurrences')
+    # roofline of the dominant family: the wgmma GEMMs, against the dense bf16 peak x 1/3 (bf16x3)
     peaks = {}
     try:
       peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
@@ -556,7 +569,7 @@ def run_r2d2(args):
       pass
     fl = r2d2_gemm_flops(T, B, st.burn_in)
     tf = fl * 3 / (ms_c[[L.seedrl_profile_category_name(i).decode() for i in range(ncat)].index('sgemm')] * 1e-3) / 1e12
-    peak = float(peaks.get('bf16_tflops_sustained', 1465.2))
+    peak = float(peaks.get('bf16_tflops_sustained', 989.0))     # fallback: H100 SXM data sheet, dense bf16
     line['roofline'] = {'kernel': 'gemm_tc_kernel (all contractions of the step, bf16x3: 3 MMAs per fp32 product)',
                         'bound': 'tensor', 'achieved': tf, 'peak': peak, 'unit': 'TFLOP/s', 'frac': tf / peak,
                         'traffic': None, 'fp32_equivalent_flops_per_step': fl}
@@ -567,7 +580,7 @@ def run_r2d2(args):
 
 
 R2D2_METRIC = ('learner env-frames/sec (R2D2 learner step, device-timed; frames = batch_size x unroll_length) on '
-               'synthetic prioritized replay @1 B200')
+               'synthetic prioritized replay @1 H100')
 
 
 def r2d2_config(args):
@@ -576,7 +589,7 @@ def r2d2_config(args):
                       'n_steps 5, gamma 0.997, clip_norm 40, Adam lr 4.8e-4 eps 1e-3 (agents/r2d2/learner.py:43-92, '
                       'atari/r2d2_main.py:36-51)' % args.batch,
           'batch_size': args.batch, 'unroll_length': 100, 'burn_in': 40, 'num_actions': A, 'parallelism': 'dp1',
-          'l2': 'per-step activations (>10 GB) exceed the 126 MB L2; no explicit flush'}
+          'l2': 'per-step activations (>10 GB) exceed the 50 MB L2; no explicit flush'}
 
 
 def r2d2_gemm_flops(T, B, burn_in):
@@ -590,6 +603,25 @@ def r2d2_gemm_flops(T, B, burn_in):
 
 
 _JSON_FD = None
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(outdir, arrays):
+  """Writes {name: tensor or array} as float32 / float64 .npy files, at most DUMP_LIMIT_BYTES in all;
+  over the limit nothing is written."""
+  import numpy as np
+  out = {}
+  for name, t in arrays.items():
+    a = np.asarray(t.detach().cpu().numpy() if hasattr(t, 'detach') else t)
+    out[name] = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+  total = sum(a.nbytes for a in out.values())
+  if total > DUMP_LIMIT_BYTES:
+    raise SystemExit('bench.py: --dump-outputs would write %d bytes, more than %d' % (total, DUMP_LIMIT_BYTES))
+  os.makedirs(outdir, exist_ok=True)
+  for name, a in out.items():
+    np.save(os.path.join(outdir, name + '.npy'), a)
 
 
 def emit(line):
@@ -700,10 +732,17 @@ def main():
     sampler.ready()
     sampler.begin()
   n0 = _lib.launch_count()
-  ms_step = timed(lambda: step.minimize(unroll), args.steps)
+  last_out = [None]
+
+  def timed_step():
+    last_out[0] = step.minimize(unroll)
+  ms_step = timed(timed_step, args.steps)
   launches = (_lib.launch_count() - n0) // args.steps
   ms_step_median = last_median[0]
   agent.check_errors()      # raises if any kernel of the timed steps timed out on a barrier
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, {'loss': last_out[0][0], 'loss_terms': step.last_loss_terms,
+                                     'gradients': agent.grads, 'parameters': agent.params})
   clocks = sampler.stop() if sampler else None
   value = world * B * T / (ms_step * 1e-3)
 
@@ -775,8 +814,8 @@ def main():
     peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
   except Exception:
     pass
-  hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-  peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s'
+  hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+  peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet 3.35 TB/s'
 
   if not args.no_extras:
     # ---- profiling pass (separate from the timed regions) --------------------------------
@@ -835,7 +874,7 @@ def main():
           learner.vtrace_loss_fwd_bwd(st, ll, lb, bl, act, rew, dn, ecp)
         times = []
         for _ in range(10):
-          flush.zero_()          # evict L2 (256 MB > 126 MB)
+          flush.zero_()          # evict L2 (256 MB > 50 MB)
           e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
           e0.record()
           learner.vtrace_loss_fwd_bwd(st, ll, lb, bl, act, rew, dn, ecp)
@@ -854,16 +893,16 @@ def main():
         msk = e0.elapsed_time(e1) / 20
         ws = 3 * T1 * Bs * A * 4
         sweep.append({'B': Bs, 'ms_single_launch_l2_flushed': ms, 'ms_back_to_back': msk,
-                      'working_set_bytes': ws, 'exceeds_l2': ws > (126 << 20),
+                      'working_set_bytes': ws, 'exceeds_l2': ws > (50 << 20),
                       'algorithmic_bytes': nb, 'GBps': nb / (msk * 1e-3) / 1e9,
                       'frac_of_hbm_peak': nb / (msk * 1e-3) / 1e9 / hbm_peak,
                       'GBps_single_launch': nb / (ms * 1e-3) / 1e9})
         del ll, lb, bl, act, rew, dn, flush
       line['roofline_vtrace_loss'] = {
           'bound': 'hbm', 'peak': hbm_peak, 'unit': 'GB/s', 'peak_source': peak_src,
-          'kernel': 'vtrace_loss_stream_kernel (B >= 148 tiles) / vtrace_loss_kernel (small B)',
+          'kernel': 'vtrace_loss_stream_kernel (B >= 132 tiles) / vtrace_loss_kernel (small B)',
           'timing': 'GBps = algorithmic bytes / mean of 20 back-to-back launches (inputs + outputs of the '
-                    'B=65536 case are 297 MB > 126 MB L2; the smaller cases are L2-resident and '
+                    'B=65536 case are 297 MB > 50 MB L2; the smaller cases are L2-resident and '
                     'host-launch-bound, reported for latency only); ms_single_launch_l2_flushed = median of '
                     '10 single launches after an L2 flush, including the Python wrapper',
           'sweep': sweep}
@@ -919,7 +958,7 @@ def main():
           nb = int(L.seedrl_debug_planes_bytes(Nf, Hh, Hh, Cc))
           xin = torch.empty(nb, dtype=torch.uint8, device='cuda'); ok = torch.empty(nb, dtype=torch.uint8, device='cuda')
           _lib.check(L.seedrl_debug_to_planes(Nf, Hh, Hh, Cc, 1, _lib.ptr(xk), _lib.ptr(xin), _lib.stream_ptr()))
-          kname = 'convp_kernel<16,16,4> (TMA + tcgen05 bf16x3, plane tensors in/out) N=%d 42x42' % Nf
+          kname = 'convp_kernel<16,16,4> (TMA + wgmma bf16x3, plane tensors in/out) N=%d 42x42' % Nf
 
           def conv_once():
             _lib.check(L.seedrl_debug_convp(Cc, Cc, Nf, Hh, Hh, _lib.ptr(xin), _lib.ptr(wk), _lib.ptr(bk), None, None,
@@ -938,31 +977,12 @@ def main():
           conv_once()
         ms_k = timed(conv_once, 10)
         alg = 2.0 * Nf * Hh * Hh * Cc * 4
-        # DRAM traffic of this kernel from the committed `ncu --set full` capture of the same source
-        # (profiles/r02_ncu_traffic.json, tools/ncu_traffic.py), scaled by the frame count
-        traffic, tc_busy, tsrc = None, None, None
-        try:
-          tj = json.load(open(os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')))
-          for kn, rec in tj.items():
-            if 'convp_kernel<16, 16, 4>' in kn and args.conv == 'tc3p':
-              traffic = (rec['dram_read_bytes'] + rec['dram_write_bytes']) * Nf / rec['frames']
-              tc_busy, tsrc = rec['tensor_pipe_active_pct'], 'profiles/' + rec['report'].replace('.ncu-rep', '.txt')
-        except Exception:
-          pass
         line['roofline_dominant_kernel'] = {
             'kernel': kname + ' (+ its 3 us weight-pack launch)',
             'bound': 'hbm', 'algorithmic_bytes_per_launch': alg, 'avg_launch_ms': ms_k,
             'achieved': alg / (ms_k * 1e-3) / 1e9, 'peak': hbm_peak, 'unit': 'GB/s',
-            'frac': alg / (ms_k * 1e-3) / 1e9 / hbm_peak, 'traffic': traffic,
-            'traffic_source': tsrc, 'tensor_pipe_busy_pct_ncu': tc_busy,
-            'second_bound': 'tensor pipe: small-N tcgen05.mma is limited by its 4 KB A-tile read from shared '
-                            'memory (~39 clk per 128xNx16 whatever N); ncu shows the pipe ~80 % busy at ~50 % of '
-                            'HBM peak, i.e. the kernel sits at the instruction-rate limit of bf16x3 at N = 16..64',
+            'frac': alg / (ms_k * 1e-3) / 1e9 / hbm_peak, 'traffic': None,
             'launches_per_step': 8, 'ok': int(errk.item()) == 0}
-        if traffic and 'roofline' in line:
-          line['roofline']['traffic'] = traffic * line['roofline']['algorithmic_bytes_per_launch'] / alg
-          line['roofline']['traffic_note'] = ('DRAM bytes of the dominant conv instance (ncu) scaled by the '
-                                              "family's algorithmic bytes per launch")
         del xk, ok
       except Exception as exc:        # pylint: disable=broad-except
         line['roofline_dominant_kernel'] = {'unavailable': repr(exc)[:200]}

@@ -1,4 +1,4 @@
-/* seedrl_b200.h -- C-ABI of libseedrl_b200.so: the B200 (sm_100a) hot path of a
+/* seedrl_b200.h -- C-ABI of libseedrl_b200.so: the H100 (sm_90a) hot path of a
  * SEED-RL V-trace learner.  Plain C, no torch / C++ types in any signature.
  *
  * Conventions (all entry points):
@@ -173,10 +173,10 @@ size_t seedrl_net_num_params(const seedrl_net* net);          /* excl. entropy p
 size_t seedrl_net_arena_floats(const seedrl_net* net);
 /* Contraction path of every 3x3 convolution (forward, data and weight gradient) and of the
  * Dense / LSTM-projection / head GEMMs:
- * 0 = fp32 SIMT (bit-reproducible fp32 reference path), 1 = tcgen05 tensor cores, bf16
- * operands with fp32 accumulation, 2 = tcgen05 with bf16x3 split operands (hi*hi + lo*hi +
+ * 0 = fp32 SIMT (bit-reproducible fp32 reference path), 1 = wgmma tensor cores, bf16
+ * operands with fp32 accumulation, 2 = wgmma with bf16x3 split operands (hi*hi + lo*hi +
  * hi*lo: fp32-faithful to ~2^-16 relative), 3 = the same bf16x3 arithmetic with the 16/32-channel
- * activations and gradients kept in HBM as bf16 hi/lo channel-group planes (the UMMA operand
+ * activations and gradients kept in HBM as bf16 hi/lo channel-group planes (the wgmma operand
  * format): TMA-fed, warp-specialised conv kernels (csrc/conv_planes.cu; deep net only). */
 int seedrl_net_set_conv_mode(seedrl_net* net, int mode);
 /* LSTM recurrence: 2 (default) = one persistent kernel for all T steps each way with CTA = (batch
@@ -222,7 +222,7 @@ int seedrl_net_backward_overlap(const seedrl_net* net, const float* params, int 
                                 float* grads, void* workspace, size_t workspace_bytes,
                                 void* head_ready_event, seedrl_stream_t stream);
 size_t seedrl_net_grad_split(const seedrl_net* net);
-/* The tcgen05 / persistent kernels never spin forever: a barrier wait that expires sets an
+/* The wgmma / persistent kernels never spin forever: a barrier wait that expires sets an
  * error flag in the workspace and the kernel bails out (its results are then garbage).
  * seedrl_net_forward clears the flag; this call copies it back (synchronising `stream`) and
  * returns SEEDRL_ERR_INTERNAL if any kernel of the last forward/backward on this workspace
@@ -344,7 +344,7 @@ int seedrl_profile_end(double* ms_per_category, uint64_t* launches_per_category)
  *   [T,B,H,W,C] ALREADY STACKED (C = stack_size; seedrl_r2d2_stack_frames), h0/c0 [B,512] ->
  *   q_values [T,B,A], action int32 [T,B] (argmax, first maximum; may be NULL), h_out/c_out.
  *   backward: dq [T,B,A] -> grads (arena layout, overwritten); must follow the forward of the same
- *   (T,B) on the same workspace.  mode: 0 fp32 SIMT GEMMs, 2 (default) tcgen05 bf16x3.
+ *   (T,B) on the same workspace.  mode: 0 fp32 SIMT GEMMs, 2 (default) wgmma bf16x3.
  *   Errors: SEEDRL_ERR_INVALID_ARGUMENT for null / undersized buffers (the reference raises from
  *   TF shape checks); seedrl_r2d2_net_check_error as seedrl_net_check_error. */
 typedef struct seedrl_r2d2_net seedrl_r2d2_net;
@@ -423,7 +423,8 @@ int seedrl_debug_conv_pixels(int N, int H, int W, int which, int start, int coun
  * TMA-streamed vtrace_loss_stream_kernel.  Lets the tests run both on the same inputs. */
 int seedrl_debug_set_loss_stream(int enabled);
 /* K positions per pipeline stage of the tensor-core weight-gradient kernel: the largest of 512 / 256 / 128
- * not above `kc` whose stages fit shared memory is used (default 512). */
+ * not above `kc` that the input width allows (512: 8-channel uint8 frames only; 256: up to 16
+ * channels) and whose stages fit shared memory is used (default 256). */
 int seedrl_debug_set_wgrad_chunk(int kc);
 /* Output positions per tile of the tensor-core forward / data-gradient kernel: the largest
  * of 512 / 256 / 128 not above `mt` that keeps two CTAs per SM is used (default 512). */
@@ -443,24 +444,24 @@ int seedrl_debug_conv3x3_wgrad(int cin, int cout, int in_mode, int N, int H, int
                                const void* x, const float* dy, float* dw, float* db,
                                float* partial, size_t partial_bytes,
                                seedrl_stream_t stream);
-/* tcgen05 (tensor-core, bf16 x bf16 -> fp32) 3x3 convolution: packs fp32 HWIO weights
+/* wgmma (tensor-core, bf16 x bf16 -> fp32) 3x3 convolution: packs fp32 HWIO weights
  * (flip != 0: flipped + transposed, i.e. the data-gradient; split != 0: bf16x3 hi/lo
  * operands, fp32-faithful) into wq_scratch (>= 2*9*max(cin,16)*cout*2 bytes) and runs the implicit-GEMM kernel.  variant bit0/bit1 swap the
- * LBO/SBO fields of the A/B shared-memory descriptors (bring-up aid); *error_flag becomes 1
- * if the kernel's bounded mbarrier wait expires. */
+ * LBO/SBO fields of the A/B shared-memory descriptors (bring-up aid).  The kernel has no
+ * bounded waits: *error_flag is left unchanged. */
 int seedrl_debug_conv3x3_tc(int cin, int cout, int in_mode, int split, int N, int H, int W,
                             const void* in, const float* w, const float* bias,
                             const float* mask, const float* res, float* out, int flip,
                             int variant, void* wq_scratch, int* error_flag,
                             seedrl_stream_t stream);
-/* tcgen05 weight gradient (MN-major operands, one TMEM accumulator per tap). */
+/* wgmma weight gradient (MN-major operands, register accumulators). */
 int seedrl_debug_conv3x3_wgrad_tc(int cin, int cout, int in_mode, int split, int N, int H, int W,
                                   const void* x, const float* dy, float* dw, float* db,
                                   float* partial, size_t partial_bytes, int* error_flag,
                                   seedrl_stream_t stream);
 int seedrl_debug_maxpool(int backward, int N, int H, int W, int C, const float* x_or_dy,
                          float* y_or_dx, uint8_t* idx, seedrl_stream_t stream);
-/* C[M,N] (=|+=) op(A) op(B) on the tensor cores (tcgen05, bf16 or bf16x3 operands, fp32
+/* C[M,N] (=|+=) op(A) op(B) on the tensor cores (wgmma, bf16 or bf16x3 operands, fp32
  * accumulate): ta: A stored [K,M]; tb: B stored [N,K]; epilogue bias / relu / mask / accumulate
  * as seedrl_debug_sgemm.  ws (may be NULL) takes split-K partials. */
 int seedrl_debug_gemm_tc(int ta, int tb, int split, int M, int N, int K, const float* A, int lda,

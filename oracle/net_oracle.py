@@ -84,7 +84,7 @@ def param_specs(net, num_actions, obs_shape):
 
 # When set to torch.bfloat16, the 3x3 convolutions with >= 16 input channels round their
 # OPERANDS (activations, weights, and -- in the backward -- the incoming gradient) to bf16
-# and accumulate in fp32: the arithmetic contract of the tcgen05 tensor-core path
+# and accumulate in fp32: the arithmetic contract of the wgmma tensor-core path
 # (seed_rl_b200 conv_mode='tc').  The fp32 reference semantics are CONV_OPERAND_DTYPE=None.
 CONV_OPERAND_DTYPE = None
 

@@ -1,4 +1,4 @@
-"""seed_rl_b200: B200-native (sm_100a) hot path of a SEED-RL V-trace learner.
+"""seed_rl_b200: H100-native (sm_90a) hot path of a SEED-RL V-trace learner.
 
 Mirrors the reference's module layout for the path it replaces:
   common.vtrace, common.parametric_distribution, common.utils,

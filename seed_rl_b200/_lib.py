@@ -224,7 +224,7 @@ def require_cuda(t, dtype, name):
   if not isinstance(t, torch.Tensor):
     t = torch.as_tensor(t)
   if not torch.cuda.is_available():
-    raise RuntimeError('seed_rl_b200 needs a CUDA device (B200); there is no CPU path '
+    raise RuntimeError('seed_rl_b200 needs a CUDA device (H100); there is no CPU path '
                        '(argument %r).' % name)
   if t.device.type != 'cuda':
     t = t.cuda()

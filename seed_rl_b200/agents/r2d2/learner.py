@@ -43,7 +43,7 @@ _define(flags.DEFINE_float, 'replay_ratio', 1.5, 'Average number of times each o
         'used for training.')
 _define(flags.DEFINE_integer, 'inference_batch_size', -1, 'Batch size for inference, -1 for auto-tune.')
 _define(flags.DEFINE_integer, 'unroll_length', 100, 'Unroll length in agent steps.')
-_define(flags.DEFINE_integer, 'num_training_tpus', 1, 'Unused on B200 (kept for flag compatibility).')
+_define(flags.DEFINE_integer, 'num_training_tpus', 1, 'Unused: there are no TPUs (kept for flag compatibility).')
 _define(flags.DEFINE_integer, 'update_target_every_n_step', 2500,
         'Update the target network at this frequency (expressed in number of training steps)')
 _define(flags.DEFINE_integer, 'replay_buffer_size', 100, 'Size of the replay buffer (in number of unrolls stored).')

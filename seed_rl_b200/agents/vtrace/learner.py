@@ -28,7 +28,7 @@ common_flags.define_once(flags.DEFINE_integer, 'total_environment_frames', int(1
 common_flags.define_once(flags.DEFINE_integer, 'batch_size', 32, 'Batch size for training.')
 common_flags.define_once(flags.DEFINE_integer, 'inference_batch_size', -1, 'Batch size for inference, -1 for auto-tune.')
 common_flags.define_once(flags.DEFINE_integer, 'unroll_length', 100, 'Unroll length in agent steps.')
-common_flags.define_once(flags.DEFINE_integer, 'num_training_tpus', 1, 'Unused on B200 (kept for flag compatibility).')
+common_flags.define_once(flags.DEFINE_integer, 'num_training_tpus', 1, 'Unused: there are no TPUs (kept for flag compatibility).')
 common_flags.define_once(flags.DEFINE_string, 'init_checkpoint', None,
                     'Path to the checkpoint used to initialize the agent.')
 # Loss settings.
@@ -48,7 +48,7 @@ common_flags.define_once(flags.DEFINE_integer, 'log_batch_frequency', 100, 'We a
                      'before logging batch statistics like entropy.')
 common_flags.define_once(flags.DEFINE_integer, 'log_episode_frequency', 1, 'We average that many episodes'
                      ' before logging average episode return and length.')
-# B200 additions
+# flags of this implementation (not in the reference)
 common_flags.define_once(flags.DEFINE_enum, 'grad_reduce', 'sum', ['sum', 'mean'],
                   'Cross-replica gradient reduction. The reference SUMs '
                   '(tests/utils_test.py:609-650).')

@@ -76,7 +76,7 @@ class DuelingLSTMDQNNet(object):
   (Keras layouts, tf.Module variable order)."""
 
   def __init__(self, num_actions, observation_shape, stack_size=1, seed=0, device=None, gemm_mode='tc3'):
-    """gemm_mode: 'tc3' = tcgen05 bf16x3 (fp32-faithful) for every contraction (convolutions as
+    """gemm_mode: 'tc3' = wgmma bf16x3 (fp32-faithful) for every contraction (convolutions as
     im2col GEMMs, Dense, LSTM projection, heads); 'simt' = fp32 CUDA cores."""
     L = _lib.lib()
     self._num_actions = int(num_actions)

@@ -103,6 +103,6 @@ def get_parametric_distribution_for_action_space(action_space, continuous_config
   if hasattr(action_space, 'n') and not hasattr(action_space, 'nvec'):
     return categorical_distribution(int(action_space.n),
                                     dtype=getattr(action_space, 'dtype', 'int64'))
-  raise ValueError('Only Discrete action spaces are on the B200 hot path; got %r '
+  raise ValueError('Only Discrete action spaces are on the GPU hot path; got %r '
                    '(continuous / multi-discrete / tuple spaces are out of scope).' %
                    (action_space,))

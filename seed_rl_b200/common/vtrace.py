@@ -2,7 +2,7 @@
 (from_importance_weights, VTraceReturns; reference common/vtrace.py:31-148).
 
 Same name, argument meaning and error behaviour; tensors are torch CUDA tensors
-and the arithmetic is ONE sm_100a kernel behind the C-ABI
+and the arithmetic is ONE sm_90a kernel behind the C-ABI
 (seedrl_vtrace_from_importance_weights).  No CPU fallback.
 """
 import collections

@@ -3,7 +3,7 @@
 // `Computation`): many callers each contribute k rows of a fixed-size batch; when the
 // batch is full one computation runs; outputs fan back out to the callers.
 //
-// B200-first differences (same observable behaviour, pinned by
+// H100-first differences (same observable behaviour, pinned by
 // grpc/python/ops_test.py's batching tests):
 //   * callers write their payload DIRECTLY into a pinned host slab at their claimed
 //     row offset (no TensorProto -> tensor -> batch-tensor double copy,

@@ -1,4 +1,4 @@
-// Shared helpers for libseedrl_b200 (sm_100a only).
+// Shared helpers for libseedrl_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -60,7 +60,7 @@ inline void count_launch(int cat = PC_MISC, cudaStream_t st = 0) {
   if (g_prof_on) prof_mark_(cat, st);
 }
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline size_t ceil_div_sz(size_t a, size_t b) { return (a + b - 1) / b; }

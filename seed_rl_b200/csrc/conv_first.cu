@@ -4,7 +4,7 @@
 // The gradient that reaches the convolution output is the max-pool's scatter of the pooled gradient
 // g: at most one position per (pooled pixel, channel) is non-zero.  Materialising that full-
 // resolution tensor (607 MB fp32 at 1 344 frames) and running a dense weight-gradient convolution over
-// it was 0.69 ms of the 5.5 ms step (pool backward 0.30 + weight gradient 0.39).  Here each
+// it costs a full-resolution write, two full-resolution reads and the dense MACs.  Here each
 // (pooled pixel q, channel co) adds  g[q][co] * x[argmax(q, co) + tap]  to dW[tap][:][co] directly:
 //     dW[kh][kw][ci][co] = sum_{n,q} g[n,q,co] * x[n][p(q,co) + (kh-1, kw-1)][ci] / 255,
 //     db[co]            = sum_{n,q} g[n,q,co],
@@ -190,24 +190,24 @@ int first_wgrad_pooled(int N, int H, int W, const uint8_t* frames, const void* g
 // =================================================================================================
 // First layer, forward, fused: Conv2D(16, 3, 'same') on the uint8 frames + bias + MaxPool 3x3/2
 // 'same' (dmlab/networks.py:31-37,47-48) -> the pooled activation as plane tensors (raw and ReLU'd)
-// + the arg-max taps.  The full-resolution conv output (607 MB fp32 at 1 344 frames, written once and
-// read once by a separate pool kernel: 0.53 ms of the step) never leaves the SM.
+// + the arg-max taps.  The full-resolution conv output (607 MB fp32 at 1 344 frames, which a separate
+// pool kernel would write once and read once) never leaves the SM.
 //
 // Work unit = (frame, band of kCpRows pooled rows).  Per unit:
 //   1. the band's frame rows -> shared memory as a PAIR array: entry e = [pixel e, pixel e+1] of the
 //      zero-bordered band (row pitch SW = W + 2), 4 channels each, bf16 (exact for 0..255) = 16 bytes.
-//      That array IS a K-major UMMA operand whose row p reads, for kernel row kh, the 16 bytes at
+//      That array IS a K-major wgmma operand whose row p reads, for kernel row kh, the 16 bytes at
 //      e = p + kh*SW (taps kw = 0, 1) and at e + 2 (taps kw = 2 and a 4th, zero-weight, tap): the two
 //      K-groups of one K = 16 instruction are the same array 32 bytes apart (LBO = 32 B).  A whole
-//      kernel row per MMA: 3 MMAs of 128 x 32 x 16 per 128 positions, no im2col pass.
-//   2. one elected thread issues them: D[128, 0:16] = A hi(W), D[128, 16:32] = A lo(W)
-//      (frames are exact in bf16, so two products make the fp32-faithful result);
-//   3. epilogue: TMEM -> (hi + lo) / 255 + bias -> fp32 tile in shared memory;
+//      kernel row per MMA: 3 MMAs of 64 x 32 x 16 per 64 positions, no im2col pass.
+//   2. warpgroup wg issues them for position blocks wg, wg + 2, ...: D[64, 0:16] = A hi(W),
+//      D[64, 16:32] = A lo(W) (frames are exact in bf16, so two products make the fp32-faithful result);
+//   3. epilogue: accumulator registers -> (hi + lo) / 255 + bias -> fp32 tile in shared memory;
 //   4. pooling from shared memory, TF-SAME windows, first maximum wins; hi/lo split; coalesced
 //      16-byte plane stores; padding positions of the plane tensors written as zeros.
-// 2 CTAs / SM (TMEM 2 x 256 columns): the phases of one CTA overlap the other's.
-// kCpRows pooled rows per unit (template parameter: 3 -> up to 6 blocks of 128 positions, TMEM 256 columns,
-// 2 CTAs / SM; 2 -> up to 4 blocks, TMEM 128 columns, 3 CTAs / SM).
+// 2 CTAs / SM: the phases of one CTA overlap the other's.
+// kCpRows pooled rows per unit (template parameter: 3 -> up to 6 blocks of 128 positions, 2 CTAs / SM;
+// 2 -> up to 4 blocks, 3 CTAs / SM).
 constexpr int kCpThreadsF = 256;
 constexpr int kCpOutStride = 20;    // floats per position in the fp32 tile (16 + 4: pool reads 2-way conflict)
 
@@ -241,9 +241,8 @@ template <int kCpRows>
 __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_kernel(const __grid_constant__ CUtensorMap tm_frames,
                                                                     const Conv0PoolArgs a) {
   constexpr int kCpMaxBlocks = kCpRows == 2 ? 4 : 6;
-  constexpr uint32_t kTmemCols = kCpRows == 2 ? 128u : 256u;
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const int W = a.W, H = a.H, SW = W + 2;
   const int npair = kCpMaxBlocks * 128 + 2 * SW + 8;          // pair entries an MMA may touch
   uint4* s_p = reinterpret_cast<uint4*>(smem_raw);            // pair array, 16 B per entry
@@ -251,16 +250,14 @@ __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_k
   uint8_t* s_bq = reinterpret_cast<uint8_t*>(s_out + (size_t)kCpMaxBlocks * 128 * kCpOutStride);
   s_bq = reinterpret_cast<uint8_t*>(((uintptr_t)s_bq + 127) & ~(uintptr_t)127);     // B: 48 x 32 bf16 = 3 KB
   float* s_bias = reinterpret_cast<float*>(s_bq + 48 * 32 * 2);
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_bias + 16);
-  uint64_t* s_full = s_bar + 1;                               // [2] TMA stage filled
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_full + 2);
+  uint64_t* s_full = reinterpret_cast<uint64_t*>(s_bias + 16);   // [2] TMA stage filled
   constexpr int kRawRows = 2 * kCpRows + 3;                   // frame rows per tile (incl. the halo rows)
-  uint32_t* s_raw = reinterpret_cast<uint32_t*>(((uintptr_t)(s_tmem + 4) + 127) & ~(uintptr_t)127);   // [2][kRawRows][W]
+  uint32_t* s_raw = reinterpret_cast<uint32_t*>(((uintptr_t)(s_full + 4) + 127) & ~(uintptr_t)127);   // [2][kRawRows][W]
   const uint32_t raw_bytes = (uint32_t)(kRawRows * W) * 4u;
   const uint32_t raw_stride = (raw_bytes + 127u) & ~127u;     // stage pitch (TMA destinations are 128-byte aligned)
 
   // ---- one-time setup: B operand (K-major, [N = 32][K = 48]: hi(w) | lo(w); k = kh*16 + kw*4 + ci,
-  //      the 4th tap of a row has zero weights), bias, barrier, TMEM -------------------------------
+  //      the 4th tap of a row has zero weights), bias, barriers ----------------------------------
   for (int i = tid; i < 48 * 32; i += kCpThreadsF) {
     const int k = i / 32, nn = i - k * 32;
     const int kh = k >> 4, kw = (k >> 2) & 3, ci = k & 3;
@@ -276,27 +273,17 @@ __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_k
   if (tid < 16) s_bias[tid] = __ldg(a.bias + tid);
   for (int i = tid; i < npair; i += kCpThreadsF) s_p[i] = make_uint4(0u, 0u, 0u, 0u);
   if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_full)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_full + 1)));
+    mbar_init(s_full, 1);
+    mbar_init(s_full + 1, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_frames)) : "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-  constexpr uint32_t idesc = umma_idesc(128, 32);
   const uint32_t a_base = smem_u32(s_p), b_base = smem_u32(s_bq);
 
   const int bands = (a.Ho + kCpRows - 1) / kCpRows;
   const int units = a.N * bands;
-  uint32_t phase = 0;
   bool timed_out = false;
   auto unit_geom = [&](int u, int* n, int* r0, int* r1, int* cr0, int* cr1) {
     *n = u / bands;
@@ -339,42 +326,38 @@ __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_k
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    // ---- 2. MMAs: one per kernel row and 128-position block -------------------------------------
-    if (warp == 0 && elect_one()) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int m = 0; m < nblk; ++m) {
+    // ---- 2. MMAs: one per kernel row and 64-position block; 3. epilogue: accumulators -> fp32 tile
+    //      [position o = lr*SW + c][16 (+4 pad)] -------------------------------------------------------
+    for (int m = wg; m < 2 * nblk; m += kCpThreadsF / 128) {
+      float acc[16];
 #pragma unroll
-        for (int kh = 0; kh < 3; ++kh) {
-          const uint64_t da = umma_desc(a_base + (uint32_t)(m * 128 + kh * SW) * 16u, 32u, 128u);
-          const uint64_t db = umma_desc(b_base + (uint32_t)(2 * kh) * 512u, 512u, 128u);
-          umma_f16(tmem_base + (uint32_t)(m * 32), da, db, idesc, kh > 0 ? 1u : 0u);
-        }
+      for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+      wgmma_fence_acc<16>(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int kh = 0; kh < 3; ++kh) {
+        const uint64_t da = gmma_desc(a_base + (uint32_t)(m * 64 + kh * SW) * 16u, 32u, 128u);
+        const uint64_t db = gmma_desc(b_base + (uint32_t)(2 * kh) * 512u, 512u, 128u);
+        Wgmma<32>::mma<0, 0>(acc, da, db, 1u);
       }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(s_bar))
-                   : "memory");
-    }
-    if (!mbar_wait_bounded(s_bar, phase)) timed_out = true;
-    phase ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- 3. epilogue: accumulators -> fp32 tile [position o = lr*SW + c][16 (+4 pad)] --------------
-    for (int m = warp >> 2; m < nblk; m += 2) {
-      const int q = warp & 3;
-      const int o = m * 128 + q * 32 + lane;
-      float v[32];
-      tmem_ld<32>(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * 32), v);
-      if (o < npos) {
-        float4* dst = reinterpret_cast<float4*>(s_out + (size_t)o * kCpOutStride);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc<16>(acc);
+      // a thread holds channels c, c+1 of two positions; columns 16.. are the lo(W) products
 #pragma unroll
-        for (int c4 = 0; c4 < 4; ++c4) {
-          const float4 bq = reinterpret_cast<const float4*>(s_bias)[c4];
-          dst[c4] = make_float4(fmaf(v[c4 * 4 + 0] + v[16 + c4 * 4 + 0], 1.0f / 255.0f, bq.x),
-                                fmaf(v[c4 * 4 + 1] + v[16 + c4 * 4 + 1], 1.0f / 255.0f, bq.y),
-                                fmaf(v[c4 * 4 + 2] + v[16 + c4 * 4 + 2], 1.0f / 255.0f, bq.z),
-                                fmaf(v[c4 * 4 + 3] + v[16 + c4 * 4 + 3], 1.0f / 255.0f, bq.w));
+      for (int h = 0; h < 2; ++h) {
+        const int o = m * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+        if (o < npos) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(s_out + (size_t)o * kCpOutStride + c) =
+                make_float2(fmaf(acc[4 * j + 2 * h] + acc[4 * (j + 2) + 2 * h], 1.0f / 255.0f, s_bias[c]),
+                            fmaf(acc[4 * j + 2 * h + 1] + acc[4 * (j + 2) + 2 * h + 1], 1.0f / 255.0f, s_bias[c + 1]));
+          }
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     // ---- 4. max-pool 3x3 / 2 from the tile; thread = (pooled pixel, 8-channel group) ----------------
     const int nout = (r1 - r0) * a.Wo * 2;
@@ -448,11 +431,6 @@ __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_k
     __syncthreads();      // s_out and the pair array are rewritten by the next unit
   }
   if (timed_out && a.err) atomicExch(a.err, 1);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-  }
 }
 
 static int g_c0_rows = getenv("SEEDRL_C0_ROWS") ? (atoi(getenv("SEEDRL_C0_ROWS")) == 2 ? 2 : 3) : 3;

@@ -1,7 +1,7 @@
 // "Planes" convolution path (conv_mode 3, 'tc3p'): activations and gradients of the 16/32-channel
 // layers of dmlab/networks.py:26-60 live in HBM in the tensor core's own operand format, so that
 // every 3x3 convolution (forward, data gradient, weight gradient) is
-//      TMA tile (cp.async.bulk.tensor)  ->  tcgen05.mma  ->  epilogue
+//      TMA tile (cp.async.bulk.tensor)  ->  wgmma  ->  epilogue
 // with no thread ever touching an input element.
 //
 // HBM format of a [N, H, W, C] activation ("plane tensor"):
@@ -12,7 +12,7 @@
 //   planes (bf16(v)), then the C/8 "lo" planes (bf16(v - hi)) -- v = hi + lo to ~2^-17 relative,
 //   the bf16x3 operand split of the 'tc3' mode, done ONCE by the producing kernel's epilogue
 //   instead of by every consumer.  Padding positions hold zeros.
-//   One plane is exactly the canonical no-swizzle UMMA layout (core matrix = 8 positions x 16 B):
+//   One plane is exactly the canonical no-swizzle wgmma layout (core matrix = 8 positions x 16 B):
 //   K-major A operand of the forward / data-gradient GEMM (M = positions, K = channels: LBO = plane
 //   stride, SBO = 128 B) and MN-major operand of the weight-gradient GEMM (K = positions: LBO =
 //   128 B, SBO = plane stride); a filter tap (kh, kw) is the descriptor start address moved by
@@ -20,16 +20,17 @@
 //
 // Kernels (all persistent, 1 CTA / SM, warp-specialised, mbarrier pipelines, bounded waits):
 //   convp_kernel<CIN, COUT, NSUB>   forward / data gradient.  warp 0 = TMA producer (one
-//       cp.async.bulk.tensor.3d per tile: box = 16-position chunks x (2 * CIN/8 planes), two
-//       smem stages), warp 1 = MMA issuer (NSUB*9*CIN/16*3 tcgen05.mma kind::f16 128 x COUT x 16
-//       per tile into one of TWO TMEM accumulator sets, tcgen05.commit -> stage-empty and
-//       accumulator-full barriers), warps 4..11 = epilogue (tcgen05.ld -> bias / ReLU-mask /
-//       residual -> hi/lo split -> coalesced 16-byte plane stores; optionally a second, ReLU'd
-//       copy for the next conv, or fp32 NHWC for the max-pool / Dense consumers).
+//       cp.async.bulk.tensor.3d per tile: box = chunks of positions x (2 * CIN/8 planes), two
+//       smem stages), warps 4..11 = two warpgroups that each take every other 64-position block
+//       of a tile: 9*CIN/16*2 wgmma 64 x {2 COUT, COUT} x 16 into registers, release the stage
+//       on its empty barrier, then the epilogue (accumulators -> per-warpgroup fp32 scratch ->
+//       bias / ReLU-mask / residual -> hi/lo split -> coalesced 16-byte plane stores; optionally
+//       a second, ReLU'd copy for the next conv, or fp32 NHWC for the max-pool / Dense consumers).
 //   wgradp_kernel<CP, COUT, KC>     weight + bias gradient: M = (kw, ci) rows from three
 //       kw-shifted TMA copies of the x planes (+ a constant ones row whose accumulator is the bias
-//       gradient), N = c_out from the dy planes, K = positions, one TMEM accumulator per kernel
-//       row kh; per-CTA partials reduced in fixed order by the deferred reduce of conv_tc_kernels.cu.
+//       gradient), N = (kh, c_out) from three kh-shifted copies of the dy planes, K = positions; one
+//       warpgroup per 64 rows holds its accumulator in registers; per-CTA partials reduced in
+//       fixed order by the deferred reduce of conv_tc_kernels.cu.
 //   poolp_fwd / poolp_bwd / to_planes / from_planes: elementwise format kernels.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -74,8 +75,7 @@ static EncodeTiledFn encode_tiled_fn() {
 }
 
 // Positions per TMA box row.  The TMA engine pays a fixed cost per box row, so rows are as long as
-// the 256-element box limit allows: 128 positions x 16 B = 256 x uint64 (measured: 16-position rows
-// made the conv kernels TMA-issue-bound at ~40 cycles per row).  Tiles start on multiples of it.
+// the 256-element box limit allows: 128 positions x 16 B = 256 x uint64.  Tiles start on multiples of it.
 static int g_chunk = 0;
 int planes_chunk() {
   if (g_chunk == 0) {
@@ -111,13 +111,6 @@ static int make_plane_map(CUtensorMap* tm, const void* base, long long Lp, int p
   return SEEDRL_OK;
 }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
@@ -129,10 +122,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
           "r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
       : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
 }
 __device__ __forceinline__ float bf16lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
@@ -163,24 +152,17 @@ __global__ void __launch_bounds__(kCpThreads, 1)
 convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
   constexpr int G = CIN / 8, GO = COUT / 8, NS = CIN / 16;
   constexpr int MT = NSUB * kCpM;
-  // one accumulator set: per M block 2*COUT columns [a*hi(w) + lo(a)*hi(w) | hi(a)*lo(w)]
-  constexpr int ACC_COLS = NSUB * 2 * COUT;
-  constexpr int TCOLS = 2 * ACC_COLS <= 32 ? 32 : (2 * ACC_COLS <= 64 ? 64 : (2 * ACC_COLS <= 128 ? 128
-                        : (2 * ACC_COLS <= 256 ? 256 : 512)));
-  static_assert(2 * ACC_COLS <= 512, "TMEM has 512 columns");
-  constexpr int NEPI = NSUB >= 2 ? 8 : 4;                // epilogue warps that own an M block
+  constexpr int SLD = COUT + 4;                          // scratch row pitch (floats)
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int PW = a.g.PW;
   const uint32_t P = (uint32_t)(a.nch * a.chunk) * 16u;  // plane stride in a stage (bytes)
   const uint32_t stage_bytes = 2u * G * P;
   uint8_t* s_stage = smem_raw;                           // [2][hi G planes | lo G planes]
   uint4* s_b = reinterpret_cast<uint4*>(smem_raw + 2 * (size_t)stage_bytes);   // 2 * 9*CIN*COUT bf16
-  float* s_bias = reinterpret_cast<float*>(s_b + 2 * 9 * CIN * COUT / 8);
+  float* s_scr = reinterpret_cast<float*>(s_b + 2 * 9 * CIN * COUT / 8);      // [2 warpgroups][64][SLD]
+  float* s_bias = s_scr + 2 * 64 * SLD;
   uint64_t* s_full = reinterpret_cast<uint64_t*>(s_bias + COUT);
   uint64_t* s_empty = s_full + 2;
-  uint64_t* s_tfull = s_empty + 2;
-  uint64_t* s_tempty = s_tfull + 2;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_tempty + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   for (int i = tid; i < 2 * 9 * CIN * COUT / 8; i += kCpThreads) s_b[i] = __ldg(a.wq + i);
@@ -188,23 +170,13 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
       mbar_init(s_full + i, 1);
-      mbar_init(s_empty + i, 1);
-      mbar_init(s_tfull + i, 1);
-      mbar_init(s_tempty + i, NEPI);
+      mbar_init(s_empty + i, 8);                       // the 8 consumer warps
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_in)) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // weights: generic -> async proxy
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
 
   const int my_tiles = ((int)blockIdx.x < a.ntiles) ? (a.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   bool timed_out = false;
@@ -221,56 +193,17 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ================================ MMA issuer ==============================================
-    // The tensor core reads its A tile (128 positions x 16 channels = 4 KB) from shared memory
-    // at ~128 B/clk for EVERY instruction -- that, not the FLOP rate, bounds small-N MMAs (measured:
-    // 39 clk per 128x16x16).  So the bf16x3 product is issued as TWO reads of the activations per
-    // (tap, slab): hi(a) x [hi(w) | lo(w)] as one N = 2*COUT instruction, lo(a) x hi(w) accumulated
-    // onto its first half; the epilogue adds the halves.
-    constexpr uint32_t idesc2 = umma_idesc(kCpM, 2 * COUT), idesc1 = umma_idesc(kCpM, COUT);
-    const uint32_t b_base = smem_u32(s_b);
-    for (int it = 0; it < my_tiles; ++it) {
-      const int s = it & 1;
-      if (!mbar_wait_bounded(s_full + s, (uint32_t)((it >> 1) & 1))) { timed_out = true; break; }
-      if (it >= 2 && !mbar_wait_bounded(s_tempty + s, (uint32_t)(((it >> 1) - 1) & 1))) { timed_out = true; break; }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t a_base = smem_u32(s_stage + (size_t)s * stage_bytes);
-        const uint32_t d_base = tmem_base + (uint32_t)(s * ACC_COLS);
-        // descriptors are advanced by adding to their address field (16-byte units)
-        const uint64_t da0 = umma_desc(a_base, P, 128u);
-        const uint64_t db0 = umma_desc(b_base, (uint32_t)(2 * GO) * 128u, 128u);
-        const uint64_t lo_off = (uint64_t)((G * P) >> 4), slab_off = (uint64_t)((2 * P) >> 4);
-#pragma unroll 1
-        for (int m = 0; m < NSUB; ++m) {
-          uint32_t acc = 0;
-          const uint32_t d = d_base + (uint32_t)(m * 2 * COUT);
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            const uint64_t off = (uint64_t)(m * kCpM + (tap / 3) * PW + (tap % 3));
-#pragma unroll
-            for (int sl = 0; sl < NS; ++sl) {
-              const uint64_t da = da0 + off + (uint64_t)sl * slab_off;
-              const uint64_t db = db0 + (uint64_t)((tap * NS + sl) * (COUT * 64 / 16));
-              umma_f16(d, da, db, idesc2, acc);
-              umma_f16(d, da + lo_off, db, idesc1, 1u);
-              acc = 1;
-            }
-          }
-        }
-        umma_commit(s_empty + s);       // this stage's smem may be refilled once these MMAs retire
-        umma_commit(s_tfull + s);       // ... and the accumulator set is complete
-      }
-      __syncwarp();
-    }
   } else if (warp >= 4) {
-    // ================================ epilogue ================================================
-    const int q = warp & 3;                       // TMEM lane quadrant this warp may read
-    const int half = (warp - 4) >> 2;             // 0 / 1: which M blocks of a tile
+    // ============================ MMA + epilogue warpgroups ===================================
+    // The tensor core reads the A tile (positions x 16 channels) from shared memory for EVERY
+    // instruction -- that, not the FLOP rate, bounds small-N MMAs.  So the bf16x3 product is issued
+    // as TWO reads of the activations per (tap, slab): hi(a) x [hi(w) | lo(w)] as one N = 2*COUT
+    // instruction, lo(a) x hi(w) accumulated onto its first half; the epilogue adds the halves.
+    const int cw = (warp - 4) >> 2;               // consumer warpgroup 0 / 1
+    const int et = tid - 128;                     // 0 .. 255
+    float* scr = s_scr + cw * 64 * SLD;
     const size_t plane_u = (size_t)a.Lp;          // plane stride in 16-byte units (global)
     if (blockIdx.x == 0) {                        // head margin s in [0, PW + 1): zeros
-      const int et = tid - 128;
       const uint4 z = make_uint4(0u, 0u, 0u, 0u);
       for (int i = et; i < (PW + 1) * 2 * GO; i += kCpThreads - 128) {
         const int pl = i / (PW + 1), s = i - pl * (PW + 1);
@@ -278,64 +211,74 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
         if (a.out_relu) a.out_relu[(size_t)pl * plane_u + s] = z;
       }
     }
-    const bool active = NSUB >= 2 || half == 0;
-    for (int it = 0; it < my_tiles && active; ++it) {
-      const int as = it & 1;
+    const uint32_t b_base = smem_u32(s_b);
+    const uint64_t db0 = gmma_desc(b_base, (uint32_t)(2 * GO) * 128u, 128u);
+    for (int it = 0; it < my_tiles; ++it) {
+      const int s = it & 1;
       const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-      if (!mbar_wait_bounded(s_tfull + as, (uint32_t)((it >> 1) & 1))) { timed_out = true; break; }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      constexpr int NB = NSUB >= 2 ? NSUB / 2 : 1;     // M blocks per warp
+      if (!mbar_wait_bounded(s_full + s, (uint32_t)((it >> 1) & 1))) { timed_out = true; break; }
+      const uint32_t a_base = smem_u32(s_stage + (size_t)s * stage_bytes);
+      // descriptors are advanced by adding to their address field (16-byte units)
+      const uint64_t da0 = gmma_desc(a_base, P, 128u);
+      const uint64_t lo_off = (uint64_t)((G * P) >> 4), slab_off = (uint64_t)((2 * P) >> 4);
 #pragma unroll 1
-      for (int bi = 0; bi < NB; ++bi) {
-        const int m = NSUB >= 2 ? half + 2 * bi : 0;
-        const int p = tile * MT + m * kCpM + q * 32 + lane;
-        const int s = p + PW + 1;
-        const int pix = out_pixel(a.g, p);
-        const bool in_store = s < a.Lp;
-        // residual / mask operands of this position (issued before the TMEM read)
-        uint4 rh[GO], rl[GO], mk[GO];
+      for (int m = cw; m < 2 * NSUB; m += 2) {
+        float acc[COUT];                          // 64 x 2*COUT: [a*hi(w) + lo(a)*hi(w) | hi(a)*lo(w)]
 #pragma unroll
-        for (int go = 0; go < GO; ++go) {
-          rh[go] = make_uint4(0u, 0u, 0u, 0u); rl[go] = rh[go]; mk[go] = rh[go];
-          if (pix >= 0) {
-            if (a.res) {
-              rh[go] = __ldg(a.res + (size_t)go * plane_u + s);
-              rl[go] = __ldg(a.res + (size_t)(GO + go) * plane_u + s);
-            }
-            if (a.mask) mk[go] = __ldg(a.mask + (size_t)go * plane_u + s);
+        for (int i = 0; i < COUT; ++i) acc[i] = 0.f;
+        wgmma_fence_acc<COUT>(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint64_t off = (uint64_t)(m * 64 + (tap / 3) * PW + (tap % 3));
+#pragma unroll
+          for (int sl = 0; sl < NS; ++sl) {
+            const uint64_t da = da0 + off + (uint64_t)sl * slab_off;
+            const uint64_t db = db0 + (uint64_t)((tap * NS + sl) * (COUT * 64 / 16));
+            Wgmma<2 * COUT>::template mma<0, 0>(acc, da, db, 1u);
+            Wgmma<COUT>::template mma<0, 0>(acc, da + lo_off, db, 1u);
           }
         }
-        float v[COUT];
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc<COUT>(acc);
+        // this warpgroup's last block of the tile: its MMAs no longer read the stage
+        if (m + 2 >= 2 * NSUB && lane == 0) mbar_arrive(s_empty + s);
+        {
+          const int w = warp & 3, r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-        for (int hc = 0; hc < COUT / 16; ++hc) {
-          float v2[16];
-          const uint32_t col = (uint32_t)(as * ACC_COLS + m * 2 * COUT + hc * 16);
-          tmem_ld<16>(tmem_base + ((uint32_t)(q * 32) << 16) + col, v + hc * 16);
-          tmem_ld<16>(tmem_base + ((uint32_t)(q * 32) << 16) + col + COUT, v2);
+          for (int j = 0; j < COUT / 8; ++j)
 #pragma unroll
-          for (int e = 0; e < 16; ++e) v[hc * 16 + e] += v2[e];
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<float2*>(scr + (r0 + 8 * h) * SLD + 8 * j + c0) =
+                  make_float2(acc[4 * j + 2 * h] + acc[4 * (j + COUT / 8) + 2 * h],
+                              acc[4 * j + 2 * h + 1] + acc[4 * (j + COUT / 8) + 2 * h + 1]);
         }
-        if (bi == NB - 1) {          // accumulator set drained: hand it back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(s_tempty + as);
-        }
+        warpgroup_sync(cw);
+        // thread = (position row, every other channel group): bias / mask / residual -> stores
+        const int row = (tid & 127) & 63;
+        const int p = tile * MT + m * 64 + row;
+        const int sp = p + PW + 1;
+        const int pix = out_pixel(a.g, p);
+        const bool in_store = sp < a.Lp;
 #pragma unroll
-        for (int go = 0; go < GO; ++go) {
+        for (int go = (tid & 127) >> 6; go < GO; go += 2) {
           float x[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) x[e] = v[go * 8 + e] + s_bias[go * 8 + e];
-          if (a.mask) {
-            const uint32_t mw[4] = {mk[go].x, mk[go].y, mk[go].z, mk[go].w};
+          for (int e = 0; e < 8; ++e) x[e] = scr[row * SLD + go * 8 + e] + s_bias[go * 8 + e];
+          if (pix >= 0 && a.mask) {
+            const uint4 mk = __ldg(a.mask + (size_t)go * plane_u + sp);
+            const uint32_t mw[4] = {mk.x, mk.y, mk.z, mk.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               x[2 * e] = bf16lo(mw[e]) > 0.f ? x[2 * e] : 0.f;
               x[2 * e + 1] = bf16hi(mw[e]) > 0.f ? x[2 * e + 1] : 0.f;
             }
           }
-          if (a.res) {
-            const uint32_t hw[4] = {rh[go].x, rh[go].y, rh[go].z, rh[go].w};
-            const uint32_t lw[4] = {rl[go].x, rl[go].y, rl[go].z, rl[go].w};
+          if (pix >= 0 && a.res) {
+            const uint4 rh = __ldg(a.res + (size_t)go * plane_u + sp), rl = __ldg(a.res + (size_t)(GO + go) * plane_u + sp);
+            const uint32_t hw[4] = {rh.x, rh.y, rh.z, rh.w};
+            const uint32_t lw[4] = {rl.x, rl.y, rl.z, rl.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               x[2 * e] += bf16lo(hw[e]) + bf16lo(lw[e]);
@@ -348,29 +291,25 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
           }
           const float4 xa = make_float4(x[0], x[1], x[2], x[3]), xb = make_float4(x[4], x[5], x[6], x[7]);
           if (a.out_raw && in_store) {
-            a.out_raw[(size_t)go * plane_u + s] = pack8_bf16(xa, xb);
-            a.out_raw[(size_t)(GO + go) * plane_u + s] = pack8_bf16(bf16_resid4(xa), bf16_resid4(xb));
+            a.out_raw[(size_t)go * plane_u + sp] = pack8_bf16(xa, xb);
+            a.out_raw[(size_t)(GO + go) * plane_u + sp] = pack8_bf16(bf16_resid4(xa), bf16_resid4(xb));
           }
           if (a.out_relu && in_store) {
             const float4 ra = make_float4(fmaxf(xa.x, 0.f), fmaxf(xa.y, 0.f), fmaxf(xa.z, 0.f), fmaxf(xa.w, 0.f));
             const float4 rb = make_float4(fmaxf(xb.x, 0.f), fmaxf(xb.y, 0.f), fmaxf(xb.z, 0.f), fmaxf(xb.w, 0.f));
-            a.out_relu[(size_t)go * plane_u + s] = pack8_bf16(ra, rb);
-            a.out_relu[(size_t)(GO + go) * plane_u + s] = pack8_bf16(bf16_resid4(ra), bf16_resid4(rb));
+            a.out_relu[(size_t)go * plane_u + sp] = pack8_bf16(ra, rb);
+            a.out_relu[(size_t)(GO + go) * plane_u + sp] = pack8_bf16(bf16_resid4(ra), bf16_resid4(rb));
           }
           if (a.out_nhwc && pix >= 0) {
             float4* o = reinterpret_cast<float4*>(a.out_nhwc + (size_t)pix * COUT + go * 8);
             o[0] = xa; o[1] = xb;
           }
         }
+        warpgroup_sync(cw);                       // the scratch is rewritten by the next block
       }
     }
   }
   if (timed_out && a.err) atomicExch(a.err, 1);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TCOLS));
-  }
 }
 
 template <int CIN, int COUT, int NSUB>
@@ -384,7 +323,7 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
   const int CH = planes_chunk();
   const int nch = (L + CH - 1) / CH;
   const size_t stage = (size_t)2 * (CIN / 8) * nch * CH * 16;
-  const size_t smem = 2 * stage + (size_t)2 * 9 * CIN * COUT * 2 + COUT * 4 + 8 * 8 + 16;
+  const size_t smem = 2 * stage + (size_t)2 * 9 * CIN * COUT * 2 + (size_t)2 * 64 * (COUT + 4) * 4 + COUT * 4 + 4 * 8;
   if (smem > 227 * 1024) return kPlanesTryNext;
   CUtensorMap tm;
   SEEDRL_TRY_RC(make_plane_map(&tm, c.in, Lp, 2 * (CIN / 8), 0, CH, nch, 2 * (CIN / 8)));
@@ -442,13 +381,14 @@ int convp_forward(int cin, int cout, const PlaneConv& c, cudaStream_t st) {
 //   A  = three kw-shifted TMA copies of the x planes (no halo) + one constant plane whose first
 //        channel is 1 (its accumulator row is the bias gradient);  MN-major, 128 rows
 //   B  = three kh-shifted TMA copies of the dy planes; MN-major, hi planes then lo planes
-// so the activation tile -- the operand whose shared-memory read (4 KB per instruction at
-// ~128 B/clk) bounds small-N MMAs -- is read TWICE per 16 positions:
+// so the activation tile -- the operand whose shared-memory read bounds small-N MMAs -- is read
+// TWICE per 16 positions:
 //   hi(x) x [hi(dy) kh=0..2 | lo(dy) kh=0..2]   N = 6*COUT   -> D[:, 0 : 6*COUT]
 //   lo(x) x  hi(dy) kh=0..2                     N = 3*COUT   -> accumulated onto D[:, 0 : 3*COUT]
-// (the first version kept kh as a start-address offset of the x planes: three accumulators, nine
-// instructions and nine reads of the x tile per 16 positions -- the tensor pipe was 92 % busy at 19 %
-// of HBM bandwidth).  Terms with j < 0 pair the zero row above the first image with dy and vanish.
+// Terms with j < 0 pair the zero row above the first image with dy and vanish.  Warp 0 issues the
+// TMA copies; warpgroup c (warps 4 + 4c ..) multiplies rows [64 c, 64 c + 64) of M (one warpgroup for
+// 16-channel inputs: 3*16 + 1 rows, two for 32-channel inputs) and keeps the 64 x 6*COUT accumulator
+// in registers across all chunks of the CTA.
 struct WgradpArgs {
   int PW, nchx, nchunks, nb;            // TMA chunks per box (x and dy alike); K chunks; stages
   int chunk;                            // positions per TMA chunk
@@ -456,20 +396,20 @@ struct WgradpArgs {
   int* err;
 };
 
-constexpr int kWpThreads = 192;
 constexpr int kWpMaxStages = 4;
+__host__ __device__ constexpr int wgradp_mrows(int CP) { return 3 * (CP / 8) + 1 <= 8 ? 64 : 128; }
+__host__ __device__ constexpr int wgradp_threads(int CP) { return 128 + 2 * wgradp_mrows(CP); }
 
 struct WgradMaps { CUtensorMap x[3], dy[3]; };
 
 template <int CP, int COUT, int KC>
-__global__ void __launch_bounds__(kWpThreads, 1)
+__global__ void __launch_bounds__(wgradp_threads(CP), 1)
 wgradp_kernel(const __grid_constant__ WgradMaps tm, const WgradpArgs a) {
   constexpr int G = CP / 8, GO = COUT / 8;
   constexpr int XG = 3 * G + 1;                          // M groups per half: (kw, g) planes + ones/zeros plane
-  // 16-channel inputs fill only 49 of an M = 128 instruction's rows; M = 64 (8 row groups >= XG = 7)
-  // reads half the A tile per instruction -- the small-N MMA is bound by that read
-  constexpr int MROWS = XG <= 8 ? 64 : 128;
-  constexpr int TCOLS = 6 * COUT <= 128 ? 128 : 256;
+  constexpr int MROWS = wgradp_mrows(CP);                // 64: the 16-channel case fills 49 rows of one warpgroup
+  constexpr int NCW = MROWS / 64;                        // MMA warpgroups
+  constexpr int THREADS = wgradp_threads(CP);
   constexpr int NW = 9 * CP * COUT + COUT;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int nb = a.nb;
@@ -479,13 +419,11 @@ wgradp_kernel(const __grid_constant__ WgradMaps tm, const WgradpArgs a) {
   const uint32_t stage_bytes = 2u * xh_bytes + 2u * dh_bytes;   // [x hi | x lo | dy hi (kh,go) | dy lo (kh,go)]
   uint64_t* s_full = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* s_empty = s_full + kWpMaxStages;
-  uint64_t* s_done = s_empty + kWpMaxStages;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_done + 1);
   uint8_t* s_stage = smem_raw + 128;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   // the constant planes of every stage: ones (x hi, channel 0 of each position) and zeros (x lo)
-  for (int i = tid; i < nb * (int)(Pk / 16); i += kWpThreads) {
+  for (int i = tid; i < nb * (int)(Pk / 16); i += THREADS) {
     const int sg = i / (int)(Pk / 16), k = i - sg * (int)(Pk / 16);
     uint4* xh = reinterpret_cast<uint4*>(s_stage + (size_t)sg * stage_bytes + (size_t)(XG - 1) * Pk);
     uint4* xl = reinterpret_cast<uint4*>(s_stage + (size_t)sg * stage_bytes + xh_bytes + (size_t)(XG - 1) * Pk);
@@ -493,20 +431,11 @@ wgradp_kernel(const __grid_constant__ WgradMaps tm, const WgradpArgs a) {
     xl[k] = make_uint4(0u, 0u, 0u, 0u);
   }
   if (tid == 0) {
-    for (int i = 0; i < kWpMaxStages; ++i) { mbar_init(s_full + i, 1); mbar_init(s_empty + i, 1); }
-    mbar_init(s_done, 1);
+    for (int i = 0; i < kWpMaxStages; ++i) { mbar_init(s_full + i, 1); mbar_init(s_empty + i, 4 * NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
 
   const int my_chunks = ((int)blockIdx.x < a.nchunks) ? (a.nchunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   bool timed_out = false;
@@ -530,72 +459,54 @@ wgradp_kernel(const __grid_constant__ WgradMaps tm, const WgradpArgs a) {
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
+  } else if (warp >= 4) {
     // both operands MN-major
-    constexpr uint32_t idesc6 = umma_idesc(MROWS, 6 * COUT) | (1u << 15) | (1u << 16);
-    constexpr uint32_t idesc3 = umma_idesc(MROWS, 3 * COUT) | (1u << 15) | (1u << 16);
+    const int cw = (warp - 4) >> 2;
+    float acc[3 * COUT];                          // 64 x 6*COUT: [x * hi(dy) kh=0..2 | hi(x) * lo(dy) kh=0..2]
+#pragma unroll
+    for (int i = 0; i < 3 * COUT; ++i) acc[i] = 0.f;
+    wgmma_fence_acc<3 * COUT>(acc);
+    // descriptors with start address 0 (the address field counts 16-byte units)
+    const uint64_t d0 = gmma_desc(0u, 128u, Pk);
     for (int it = 0; it < my_chunks; ++it) {
       const int s = it % nb;
       if (!mbar_wait_bounded(s_full + s, (uint32_t)((it / nb) & 1))) { timed_out = true; break; }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t xb = smem_u32(s_stage + (size_t)s * stage_bytes);
-        const uint32_t db = xb + 2u * xh_bytes;
-        // descriptors with start address 0 (the address field counts 16-byte units)
-        const uint64_t d0 = umma_desc(0u, 128u, Pk);
-        const uint64_t xh = d0 + (xb >> 4), xl = xh + (xh_bytes >> 4);
-        const uint64_t dh = d0 + (db >> 4);
-        const uint32_t acc0 = it > 0 ? 1u : 0u;
+      const uint32_t xb = smem_u32(s_stage + (size_t)s * stage_bytes);
+      const uint32_t db = xb + 2u * xh_bytes;
+      const uint64_t xh = d0 + (xb >> 4) + (uint64_t)cw * ((8u * Pk) >> 4), xl = xh + (xh_bytes >> 4);
+      const uint64_t dh = d0 + (db >> 4);
+      wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < KC / 16; ++ks) {
-          const uint32_t ko = (uint32_t)(ks * 16);
-          umma_f16(tmem_base, xh + ko, dh + ko, idesc6, (ks > 0) ? 1u : acc0);
-          umma_f16(tmem_base, xl + ko, dh + ko, idesc3, 1u);
-        }
-        umma_commit(s_empty + s);
+      for (int ks = 0; ks < KC / 16; ++ks) {
+        const uint32_t ko = (uint32_t)(ks * 16);
+        Wgmma<6 * COUT>::template mma<1, 1>(acc, xh + ko, dh + ko, 1u);
+        Wgmma<3 * COUT>::template mma<1, 1>(acc, xl + ko, dh + ko, 1u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();                            // the previous chunk's MMAs have read their stage
+      if (it > 0 && lane == 0) mbar_arrive(s_empty + (it - 1) % nb);
     }
-    if (elect_one()) umma_commit(s_done);
-    __syncwarp();
-  }
-  // ---- drain, then rows (kw, ci) of the accumulator -> this CTA's partial ------------------------
-  if (my_chunks > 0 && !timed_out) {
-    if (!mbar_wait_bounded(s_done, 0u)) timed_out = true;
+    wgmma_wait<0>();
+    wgmma_fence_acc<3 * COUT>(acc);
+    // ---- rows (kw, ci) of the accumulator -> this CTA's partial ------------------------------------
+    float* dst = a.partial + (size_t)blockIdx.x * NW;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = 64 * cw + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+      const int kw = row / CP, ci = row - kw * CP;
+#pragma unroll
+      for (int j = 0; j < 3 * COUT / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int n = 8 * j + 2 * (lane & 3) + e, kh = n / COUT, co = n - kh * COUT;
+          const float v = acc[4 * j + 2 * h + e] + acc[4 * (j + 3 * COUT / 8) + 2 * h + e];
+          if (row < 3 * CP) dst[((size_t)(kh * 3 + kw) * CP + ci) * COUT + co] = v;
+          else if (row == 3 * CP && kh == 1) dst[9 * CP * COUT + co] = v;   // ones row x the unshifted dy copy
+        }
+      }
+    }
   }
   if (timed_out && a.err) atomicExch(a.err, 1);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  __syncthreads();
-  float* dst = a.partial + (size_t)blockIdx.x * NW;
-  if (warp >= 2) {
-    // TMEM lane -> accumulator row: M = 128: lane = row; M = 64 (cute tmem_frg_1sm, M_MMA == 64): row m
-    // lives in lane (m % 16) + 32 * (m / 16), i.e. 16 rows per 32-lane sub-partition
-    const int row = MROWS == 128 ? (warp & 3) * 32 + lane : (lane < 16 ? (warp & 3) * 16 + lane : 1 << 20);
-    const int kw = row / CP, ci = row - kw * CP;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-#pragma unroll 1
-    for (int kh = 0; kh < 3; ++kh) {
-#pragma unroll
-      for (int hc = 0; hc < COUT / 16; ++hc) {
-        float v[16], v2[16];
-        tmem_ld<16>(lane_addr + (uint32_t)(kh * COUT + hc * 16), v);                 // x * hi(dy)
-        tmem_ld<16>(lane_addr + (uint32_t)(3 * COUT + kh * COUT + hc * 16), v2);     // hi(x) * lo(dy)
-        if (row < 3 * CP) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e)
-            dst[((size_t)(kh * 3 + kw) * CP + ci) * COUT + hc * 16 + e] = my_chunks > 0 ? v[e] + v2[e] : 0.f;
-        } else if (row == 3 * CP && kh == 1) {           // ones row x the unshifted-by-rows dy copy
-#pragma unroll
-          for (int e = 0; e < 16; ++e) dst[9 * CP * COUT + hc * 16 + e] = my_chunks > 0 ? v[e] + v2[e] : 0.f;
-        }
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TCOLS));
-  }
 }
 
 template <int CP, int COUT, int KC>
@@ -609,9 +520,9 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
   const int nchx = KC / CH;
   const size_t Pk = (size_t)KC * 16;
   const size_t stage = 2 * XG * Pk + 2 * 3 * GO * Pk;
-  // the M = 128 MMA reads 16 row groups from each x half: groups past XG are junk rows (never
+  // the MMAs read 8 * (M / 64) row groups from each x half: groups past XG are junk rows (never
   // read back) whose addresses stay inside the stage (x lo is followed by the dy planes)
-  const long long over = (long long)(16 - XG) * (long long)Pk - (long long)(6 * GO) * (long long)Pk;
+  const long long over = (long long)(wgradp_mrows(CP) / 8 - XG) * (long long)Pk - (long long)(6 * GO) * (long long)Pk;
   const size_t tail = (over > 0 ? (size_t)over : 0) + 256;
   int nb = kWpMaxStages;
   while (nb > 1 && 128 + nb * stage + tail > 227 * 1024) --nb;
@@ -639,7 +550,7 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgradp: partial buffer too small");
   a.partial = batch->buf + batch->used;
   batch->used += (size_t)grid * NW;
-  wgradp_kernel<CP, COUT, KC><<<grid, kWpThreads, smem, st>>>(tm, a);
+  wgradp_kernel<CP, COUT, KC><<<grid, wgradp_threads(CP), smem, st>>>(tm, a);
   count_launch(PC_CONV_WGRAD, st);
   SEEDRL_CHECK_LAUNCH();
   batch->jobs[batch->n++] = ReduceJob{a.partial, dw, db, grid, 9 * CP * COUT, COUT};

@@ -1,23 +1,23 @@
-// conv3x3 'same' on the 5th-gen tensor cores (tcgen05 + TMEM), bf16 (or bf16x3) operands,
+// conv3x3 'same' on the Hopper tensor cores (wgmma), bf16 (or bf16x3) operands,
 // fp32 accumulation -- forward, data-gradient and weight-gradient of every convolution of
 // dmlab/networks.py:26-60, the uint8 4->16 first layer included.
 //
 // Implicit GEMM on the "tall image" (see conv_kernels.cu): a CTA owns tiles of MT = 128..512
-// consecutive flattened output positions (MT / 128 UMMA row blocks).  Activations are staged in shared memory as
+// consecutive flattened output positions (MT / 64 wgmma row blocks).  Activations are staged in shared memory as
 // channel-group planes [CIN/8][positions][8 ch] bf16 (16 B per position per plane), which
-// IS the canonical no-swizzle K-major UMMA layout:
+// IS the canonical no-swizzle K-major wgmma layout:
 //     8 consecutive positions x 8 channels  = one 128-byte core matrix
 //     SBO (next 8 rows)            = 128 B
 //     LBO (next 8 K-elements)      = plane stride
 // and filter tap (kh,kw) is nothing but the descriptor START ADDRESS moved by
 // (kh*PW + kw) * 16 bytes.  So the 3x3 conv is 9 * CIN/16 back-to-back
-// tcgen05.mma.kind::f16 (128 x COUT x 16) issued by one thread into one TMEM
-// accumulator -- no im2col, no per-tap data movement.
+// wgmma.mma_async (64 x COUT x 16) per row block into one register accumulator -- no im2col,
+// no per-tap data movement.
 // Weights are pre-packed (prep kernel) to the K-major core-matrix layout
 // [tap][slab][kchunk][COUT/8][8 co][8 ci] bf16; the data-gradient uses the same kernel
 // with flipped/transposed packing.
-// Epilogue: tcgen05.ld 32x32b (thread = one output position, COUT fp32 columns) ->
-// bias / ReLU-mask / residual -> fp32 NHWC.
+// Epilogue straight from the accumulator registers (a thread holds 2 adjacent channels of 2
+// positions per 8-channel group) -> bias / ReLU-mask / residual -> fp32 NHWC.
 #include <cuda_bf16.h>
 
 #include <cstdio>
@@ -63,8 +63,7 @@ __global__ void pack_w_tc_kernel(int CIN, int COUT, int cin_src, int flip, int s
   if (split) wq[9 * CIN * COUT + i] = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
-// All layers' weights packed by ONE launch (blockIdx.y = job): the per-conv pack launches were
-// ~27 launches of ~3 us per learner step.
+// All layers' weights packed by ONE launch (blockIdx.y = job) instead of one small launch per conv.
 __global__ void pack_w_tc_batch_kernel(const __grid_constant__ PackTable t, int split) {
   const PackJob j = t.jobs[blockIdx.y];
   const int CIN = j.ck, COUT = j.cout;
@@ -115,12 +114,12 @@ constexpr int kTcM = 128;
 #define SEEDRL_TC_MIN_BLOCKS 4
 #endif
 constexpr int kTcMinBlocks = SEEDRL_TC_MIN_BLOCKS;   // resident CTAs per SM the register budget targets
-                                                     // (one fewer for 32 input channels: measured)
+                                                     // (one fewer for 32 input channels)
 
-// One tile = MT consecutive output positions (MT / 128 UMMA row blocks, one TMEM accumulator
-// each); the staged input covers MT + 2*PW + 2 positions, so the halo re-read and the
-// per-tile barriers shrink with MT.  8 warps: all stage; warp 0's elected lane issues the
-// MMAs; warp w reads TMEM lanes 32*(w%4).. of row blocks w/4, w/4+2, ...
+// One tile = MT consecutive output positions (MT / 64 wgmma row blocks); the staged input covers
+// MT + 2*PW + 2 positions, so the halo re-read and the per-tile barriers shrink with MT.
+// 8 warps: all stage; warpgroup wg multiplies row blocks wg, wg + 2, ... one at a time and
+// stores each from its registers.
 // SPLIT = bf16x3: activations and weights are split v = hi + lo (two bf16 planes / two packed
 // weight sets) and each K-step issues hi*hi + lo*hi + hi*lo -- an fp32-faithful (~2^-16
 // relative) contraction on the tensor cores; SPLIT = false is plain bf16 operands.
@@ -131,15 +130,13 @@ template <int CIN, int COUT, int IN_MODE, bool SPLIT, int MT>
 __global__ void __launch_bounds__(kTcThreads, CIN >= 32 ? kTcMinBlocks - 1 : kTcMinBlocks)
 conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restrict__ wq,
                   const float* __restrict__ bias, const float* __restrict__ mask,
-                  const float* __restrict__ res, float* __restrict__ out, int variant,
-                  int* __restrict__ error_flag) {
+                  const float* __restrict__ res, float* __restrict__ out, int variant) {
   constexpr int CK = CIN < 16 ? 16 : CIN;   // channels the MMAs contract over
   constexpr int G = CIN < 8 ? 1 : CIN / 8;  // staged channel-group planes
   constexpr int NS = CK / 16;               // K slabs per tap
   constexpr bool ASPLIT = SPLIT && IN_MODE != IN_U8;
   constexpr int SA = ASPLIT ? 2 : 1, SB = SPLIT ? 2 : 1;
-  constexpr int NSUB = MT / kTcM;
-  constexpr int TCOLS = NSUB * COUT <= 32 ? 32 : (NSUB * COUT <= 64 ? 64 : 128);
+  constexpr int NBLK = MT / 64;
   constexpr int IT = IN_MODE == IN_U8 ? SEEDRL_TC_ITEMS_U8 : (G == 2 ? SEEDRL_TC_ITEMS_G2 : 4);
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int PW = g.PW;
@@ -147,30 +144,15 @@ conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restr
   const int LPl = L | 1;              // plane stride in 16-byte units (odd: conflict-free stores)
   uint4* s_a = reinterpret_cast<uint4*>(smem_raw);                       // [SA][G][LPl] x 16 B
   uint4* s_b = s_a + (size_t)SA * G * LPl;                               // [SB] 9*CK*COUT bf16
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_b + SB * 9 * CK * COUT / 8);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_bar + 1);
-  float* s_bias = reinterpret_cast<float*>(s_bar + 2);                   // [COUT], 16-byte aligned
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  float* s_bias = reinterpret_cast<float*>(s_b + SB * 9 * CK * COUT / 8); // [COUT]
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const float* inf = reinterpret_cast<const float*>(in_);
   const uint32_t* inu = reinterpret_cast<const uint32_t*>(in_);          // IN_U8: 4 channels = one word
 
-  // ---- one-time setup: weights -> smem, mbarrier, TMEM allocation --------------------
+  // ---- one-time setup: weights -> smem ------------------------------------------------
   for (int i = tid; i < SB * 9 * CK * COUT / 8; i += kTcThreads) s_b[i] = __ldg(wq + i);
   if (tid < COUT) s_bias[tid] = bias ? __ldg(bias + tid) : 0.f;
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-  constexpr uint32_t idesc = umma_idesc(kTcM, COUT);
   const uint32_t a_base = smem_u32(s_a), b_base = smem_u32(s_b);
   const uint32_t plane_b = CIN < 16 ? 0u : (uint32_t)LPl * 16u;   // K-group stride of A
   const uint32_t a_lbo = (variant & 1) ? 128u : plane_b;
@@ -179,14 +161,12 @@ conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restr
   const uint32_t b_sbo = (variant & 2) ? (uint32_t)(COUT / 8) * 128u : 128u;
   const float oscale = IN_MODE == IN_U8 ? (1.0f / 255.0f) : 1.0f;
 
-  uint32_t phase = 0;
   const int nchunks = (int)((g.Q + MT - 1) / MT);
   for (int ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
     const int q0 = ch * MT;
     // ---- stage the input tile: NHWC -> bf16 channel-group planes ---------------------------
-    // IT items per thread per round: all loads of a round are issued before any is consumed
-    // (measured: 3, 4, 5 or 8 items per round give the same time -- with 3-4 CTAs per SM the
-    // round latency is hidden by the other CTAs)
+    // IT items per thread per round: all loads of a round are issued before any is consumed;
+    // with several CTAs per SM the round latency is hidden by the other CTAs
     for (int i0 = tid; i0 < L * G; i0 += IT * kTcThreads) {
       float4 va[IN_MODE == IN_U8 ? 1 : IT], vb[IN_MODE == IN_U8 ? 1 : IT];
       uint32_t vw[IN_MODE == IN_U8 ? IT : 1];
@@ -239,89 +219,57 @@ conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restr
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
 
-    // ---- one elected lane of warp 0 issues the NSUB * 9 * NS MMAs, then commits ------------
-    if (warp == 0 && elect_one()) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    // ---- warpgroup wg: row blocks wg, wg + 2, ...: 9 * NS (x3 when SPLIT) MMAs, then the epilogue
 #pragma unroll 1
-      for (int m = 0; m < NSUB; ++m) {
-        uint32_t acc = 0;
+    for (int m = wg; m < NBLK; m += kTcThreads / 128) {
+      float acc[COUT / 2];
 #pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-          const int off = m * kTcM + (tap / 3) * PW + (tap % 3);
+      for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
+      wgmma_fence_acc<COUT / 2>(acc);
+      wgmma_fence();
 #pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            const uint64_t da = umma_desc(a_base + ((uint32_t)(sl * 2) * LPl + off) * 16u, a_lbo, a_sbo);
-            const uint64_t db = umma_desc(b_base + (uint32_t)(tap * NS + sl) * (COUT * 32u), b_lbo, b_sbo);
-            umma_f16(tmem_base + (uint32_t)(m * COUT), da, db, idesc, acc);
-            acc = 1;
-            if (SPLIT) {   // + lo(a)*hi(b) + hi(a)*lo(b); the address field counts 16-byte units
-              if (ASPLIT) umma_f16(tmem_base + (uint32_t)(m * COUT), da + (uint64_t)(G * LPl), db, idesc, 1u);
-              umma_f16(tmem_base + (uint32_t)(m * COUT), da, db + (uint64_t)(9 * CK * COUT / 8), idesc, 1u);
-            }
+      for (int tap = 0; tap < 9; ++tap) {
+        const int off = m * 64 + (tap / 3) * PW + (tap % 3);
+#pragma unroll
+        for (int sl = 0; sl < NS; ++sl) {
+          const uint64_t da = gmma_desc(a_base + ((uint32_t)(sl * 2) * LPl + off) * 16u, a_lbo, a_sbo);
+          const uint64_t db = gmma_desc(b_base + (uint32_t)(tap * NS + sl) * (COUT * 32u), b_lbo, b_sbo);
+          Wgmma<COUT>::template mma<0, 0>(acc, da, db, 1u);
+          if (SPLIT) {   // + lo(a)*hi(b) + hi(a)*lo(b); the address field counts 16-byte units
+            if (ASPLIT) Wgmma<COUT>::template mma<0, 0>(acc, da + (uint64_t)(G * LPl), db, 1u);
+            Wgmma<COUT>::template mma<0, 0>(acc, da, db + (uint64_t)(9 * CK * COUT / 8), 1u);
           }
         }
       }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                       smem_u32(s_bar))
-                   : "memory");
-    }
-    // ---- everyone waits for the accumulators (bounded spin: never hang the GPU) ------------
-    {
-      uint32_t done = 0;
-      int spins = 0;
-      while (!done) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}\n"
-            : "=r"(done)
-            : "r"(smem_u32(s_bar)), "r"(phase)
-            : "memory");
-        if (!done && ++spins > (1 << 22)) {
-          if (error_flag) atomicExch(error_flag, 1);
-          break;
-        }
-      }
-      phase ^= 1;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-
-    // ---- epilogue: TMEM lane (= position) -> registers -> fp32 NHWC, 16 channels at a time ---
-    for (int m = warp >> 2; m < NSUB; m += kTcThreads / 128) {
-      const int q = warp & 3;
-      const int pix = out_pixel(g, q0 + m * kTcM + q * 32 + lane);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc<COUT / 2>(acc);
+      // ---- epilogue: (position, 2 channels) pairs of the accumulator -> fp32 NHWC ---------------
 #pragma unroll
-      for (int hc = 0; hc < COUT / 16; ++hc) {
-        float acc[16];
-        tmem_ld<16>(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * COUT + hc * 16), acc);
+      for (int h = 0; h < 2; ++h) {
+        const int pix = out_pixel(g, q0 + m * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * h);
         if (pix >= 0) {
-          const size_t o = (size_t)pix * COUT + hc * 16;
 #pragma unroll
-          for (int c4 = 0; c4 < 4; ++c4) {
-            const float4 bq = reinterpret_cast<const float4*>(s_bias)[hc * 4 + c4];     // broadcast read
-            float4 v = make_float4(fmaf(acc[c4 * 4 + 0], oscale, bq.x), fmaf(acc[c4 * 4 + 1], oscale, bq.y),
-                                   fmaf(acc[c4 * 4 + 2], oscale, bq.z), fmaf(acc[c4 * 4 + 3], oscale, bq.w));
+          for (int j = 0; j < COUT / 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const size_t o = (size_t)pix * COUT + c;
+            float2 v = make_float2(fmaf(acc[4 * j + 2 * h], oscale, s_bias[c]),
+                                   fmaf(acc[4 * j + 2 * h + 1], oscale, s_bias[c + 1]));
             if (mask) {
-              const float4 mk = __ldg(reinterpret_cast<const float4*>(mask + o) + c4);
+              const float2 mk = __ldg(reinterpret_cast<const float2*>(mask + o));
               v.x = mk.x > 0.f ? v.x : 0.f; v.y = mk.y > 0.f ? v.y : 0.f;
-              v.z = mk.z > 0.f ? v.z : 0.f; v.w = mk.w > 0.f ? v.w : 0.f;
             }
             if (res) {
-              const float4 r = __ldg(reinterpret_cast<const float4*>(res + o) + c4);
-              v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+              const float2 r = __ldg(reinterpret_cast<const float2*>(res + o));
+              v.x += r.x; v.y += r.y;
             }
-            reinterpret_cast<float4*>(out + o)[c4] = v;
+            *reinterpret_cast<float2*>(out + o) = v;
           }
         }
       }
     }
-    // TMEM reads and smem reads of this tile are done before the next tile overwrites them
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    // every MMA of this tile has read the staged input before the next tile overwrites it
     __syncthreads();
-  }
-
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TCOLS));
   }
 }
 
@@ -338,8 +286,6 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
   constexpr int CK = CIN < 16 ? 16 : CIN;
   constexpr int G = CIN < 8 ? 1 : CIN / 8;
   constexpr int SA = (SPLIT && IN_MODE != IN_U8) ? 2 : 1, SB = SPLIT ? 2 : 1;
-  constexpr int NSUB = MT / kTcM;
-  constexpr int TCOLS = NSUB * COUT <= 32 ? 32 : (NSUB * COUT <= 64 ? 64 : 128);
   const size_t smem = SA * (size_t)G * (L | 1) * 16 + SB * (size_t)9 * CK * COUT * 2 + 16 + COUT * 4 + 64;
   if (smem > 200 * 1024) {
     if (MT > kTcM) return kTcTryNext;
@@ -352,7 +298,7 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
     attr = true;
   }
   // resident CTAs per SM: registers (64K, allocated in units of 8 per thread), shared memory
-  // (228 KB, 1 KB reserved per CTA), threads, TMEM columns
+  // (228 KB, 1 KB reserved per CTA), threads
   static int regs = 0, static_smem = 0;
   if (regs == 0) {
     cudaFuncAttributes fa;
@@ -364,7 +310,6 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
   const int by_smem = (int)((size_t)(228 * 1024) / (smem + (size_t)static_smem + 1024));
   if (per_sm > by_smem) per_sm = by_smem;
   if (per_sm > 2048 / kTcThreads) per_sm = 2048 / kTcThreads;
-  if (per_sm > 512 / TCOLS) per_sm = 512 / TCOLS;
   if (per_sm > 6) per_sm = 6;
   if (per_sm < 2 && MT > kTcM) return kTcTryNext;          // a smaller tile keeps >= 2 CTAs / SM
   if (per_sm < 1) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3_tc: image too wide");
@@ -375,10 +320,10 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
   if (grid > nchunks) grid = nchunks;
   static const bool dbg = getenv("SEEDRL_DEBUG_LAUNCH") != nullptr;
   if (dbg)
-    fprintf(stderr, "conv3x3_tc<%d,%d,%d,%d> MT=%d per_sm=%d grid=%lld smem=%zu tcols=%d\n", CIN, COUT, IN_MODE,
-            (int)SPLIT, MT, per_sm, grid, smem, TCOLS);
+    fprintf(stderr, "conv3x3_tc<%d,%d,%d,%d> MT=%d per_sm=%d grid=%lld smem=%zu\n", CIN, COUT, IN_MODE,
+            (int)SPLIT, MT, per_sm, grid, smem);
   conv3x3_tc_kernel<CIN, COUT, IN_MODE, SPLIT, MT><<<(unsigned)grid, kTcThreads, smem, st>>>(
-      g, in, wq, bias, mask, res, out, variant, err);
+      g, in, wq, bias, mask, res, out, variant);
   count_launch(g_conv_cat, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
@@ -395,49 +340,39 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
 //     MN-group stride (SBO) = plane stride.
 // A = dy planes [COUT/8][128].  B = x planes [3][CP/8][Lk]: plane (kw, g) holds x shifted by kw
 // positions (the producers store every x unit three times), so that the three taps of a
-// kernel row are consecutive N-groups of ONE MMA (N = 3*CP instead of three N = COUT
-// MMAs: the tensor pipe's per-instruction floor, not its FLOP rate, is what small-N MMAs
-// pay); kh is a descriptor start-address offset of kh*PW positions.  UMMA M is 64, rows
-// >= COUT of the accumulators are junk (they read whatever follows the dy planes in shared
-// memory) and are never read back.  The 3 accumulators (3 * 3*CP TMEM columns) live across
-// ALL chunks of a persistent CTA (1 CTA / SM).  Warp-specialised pipeline over `nb` stages:
-//     warps 1..15  producers: global -> registers (prefetched two chunks ahead) ->
-//                  bf16 planes in smem -> fence.proxy.async -> arrive on full[stage]
-//     warp 0       waits full[stage]; one elected lane issues the 24 (x3 when SPLIT) MMAs by
-//                  bumping the descriptor start-address field, commits to empty[stage]
+// kernel row are consecutive N-groups of ONE MMA (N = 3*CP instead of three N = CP MMAs);
+// kh is a descriptor start-address offset of kh*PW positions.  wgmma M is 64, rows >= COUT of
+// the accumulators are junk (they read whatever follows the dy planes in shared memory) and are
+// never stored.  Warpgroup kh (warps 4kh .. 4kh+3) owns kernel row kh: its 64 x 3*CP accumulator
+// lives in registers across ALL chunks of a persistent CTA (1 CTA / SM).  Pipeline over `nb` stages:
+//     warps 12..19 producers: global -> registers (prefetched two chunks ahead when registers
+//                  allow) -> bf16 planes in smem -> fence.proxy.async -> arrive on full[stage]
+//     warps 0..11  wait full[stage], issue KC/16 (x3 when SPLIT) MMAs, keep one chunk in flight
+//                  (wgmma.wait_group 1) and release the previous chunk's stage on empty[stage]
 // SPLIT = bf16x3: operands are split v = hi + lo (two bf16 planes) and the product is
 // hi*hi + lo*hi + hi*lo, i.e. fp32-faithful (~2^-16 relative) contraction on tensor cores.
 // uint8 frames (first conv, CIN = 4 padded to one 8-channel group) are exact in bf16: no lo
 // plane; the 1/255 scale is applied to the accumulators.
 // Per-CTA partial dW/db are reduced in fixed order by wgrad_reduce (deterministic).
-__host__ __device__ constexpr uint32_t umma_idesc_mn(int M, int N) {
-  return umma_idesc(M, N) | (1u << 15) | (1u << 16);
-}
 
-// x items per producer per chunk (compile-time bound on ceil(L * G / producers))
+// x items per producer per chunk (compile-time bound on ceil(L * G / producers); L = KC + 2*PW + 2
+// with PW <= 86 for 8-channel, <= 44 for 16-channel and <= 23 for 32-channel inputs)
 __host__ __device__ constexpr int wg_ix(int G, int KC) {
-  return KC <= 128 ? 2 : (KC <= 256 ? (G == 1 ? 1 : (G == 2 ? 2 : 3)) : (G == 1 ? 2 : (G == 2 ? 3 : 5)));
+  return KC <= 128 ? (G == 4 ? 3 : 2) : (KC <= 256 ? (G == 1 ? 2 : (G == 2 ? 3 : 5)) : 3);
 }
-static int g_wgrad_kc = 512;   // K positions per pipeline stage to try first (bench/debug knob)
+// Longest chunk per input width: beyond it the producers' prefetch registers spill under the
+// 640-thread launch bound.
+__host__ __device__ constexpr int wg_max_chunk(int CP) { return CP == 8 ? 512 : (CP == 16 ? 256 : 128); }
+static int g_wgrad_kc = 256;   // K positions per pipeline stage to try first (bench/debug knob)
 void conv3x3_wgrad_tc_set_chunk(int kc) { g_wgrad_kc = kc; }
 
-constexpr int kWgThreads = 512;
-constexpr int kWgProducers = kWgThreads - 32;
+constexpr int kWgMmaThreads = 3 * 128;          // one warpgroup per kernel row
+constexpr int kWgProducers = 256;
+constexpr int kWgThreads = kWgMmaThreads + kWgProducers;
 constexpr int kWgMaxBufs = 3;
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, bool* timed_out) {
-  uint32_t done = 0;
-  int spins = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1 << 22)) { *timed_out = true; return; }
-  }
+  if (!mbar_wait_bounded(bar, parity)) *timed_out = true;
 }
 
 template <int CIN, int COUT, int IN_MODE, bool SPLIT, int KC>
@@ -448,8 +383,7 @@ conv3x3_wgrad_tc_kernel(ConvGeom g, const void* __restrict__ x_, const float* __
   constexpr int G = CP / 8, GO = COUT / 8;
   constexpr bool XSPLIT = SPLIT && IN_MODE != IN_U8;
   constexpr int SX = XSPLIT ? 2 : 1, SD = SPLIT ? 2 : 1;
-  constexpr int NN = 3 * CP;                              // UMMA N: (kw, ci)
-  constexpr int TCOLS = 3 * NN <= 128 ? 128 : (3 * NN <= 256 ? 256 : 512);
+  constexpr int NN = 3 * CP;                              // wgmma N: (kw, ci)
   constexpr int NW = 9 * CIN * COUT + COUT;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int PW = g.PW;
@@ -463,29 +397,17 @@ conv3x3_wgrad_tc_kernel(ConvGeom g, const void* __restrict__ x_, const float* __
   // (whatever follows the last stage is only ever READ, by the junk rows of A)
   uint64_t* s_full = reinterpret_cast<uint64_t*>(smem_raw + (size_t)nb * buf_units * 16);
   uint64_t* s_empty = s_full + kWgMaxBufs;
-  uint64_t* s_done = s_empty + kWgMaxBufs;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_done + 1);
   float* s_bias = reinterpret_cast<float*>(smem_raw);     // reused after the pipeline drains
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     for (int i = 0; i < kWgMaxBufs; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(s_full + i)), "r"(kWgProducers / 32));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_empty + i)));
+      mbar_init(s_full + i, kWgProducers / 32);
+      mbar_init(s_empty + i, kWgMmaThreads / 32);
     }
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_done)));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-  constexpr uint32_t idesc = umma_idesc_mn(64, NN);       // M = 64: 8 channel-group rows of A are read
 
   const int nchunks = (int)((g.Q + KC - 1) / KC);
   const int my_chunks = ((int)blockIdx.x < nchunks) ? (nchunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
@@ -493,51 +415,60 @@ conv3x3_wgrad_tc_kernel(ConvGeom g, const void* __restrict__ x_, const float* __
   float bsum[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) bsum[c] = 0.f;
+  float* dst = partial + (size_t)blockIdx.x * NW;
 
-  if (warp == 0) {
-    // ================================ MMA issuer ===========================================
-    // (the whole warp walks the loop converged; one elected lane issues)
+  if (tid < kWgMmaThreads) {
+    // ================================ MMA warpgroups ========================================
+    const int kh = warp >> 2;
+    float acc[NN / 2];
+#pragma unroll
+    for (int i = 0; i < NN / 2; ++i) acc[i] = 0.f;
+    wgmma_fence_acc<NN / 2>(acc);
     for (int it = 0; it < my_chunks; ++it) {
       const int b = it % nb;
       mbar_wait(s_full + b, (uint32_t)((it / nb) & 1), &timed_out);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t xbase = smem_u32(s_buf + (size_t)b * buf_units);
-        const uint32_t dbase = xbase + SX * xs_units * 16u;
-        // descriptors with start address 0; the address field counts 16-byte units
-        const uint64_t bx = umma_desc(0u, 128u, (uint32_t)LPk * 16u);
-        const uint64_t ad = umma_desc(0u, 128u, (uint32_t)KC * 16u);
-        const uint64_t xh = bx + (xbase >> 4), xl = xh + xs_units;
-        const uint64_t dh = ad + (dbase >> 4), dl = dh + ds_units;
-        const uint32_t acc0 = it > 0 ? 1u : 0u;
+      const uint32_t xbase = smem_u32(s_buf + (size_t)b * buf_units);
+      const uint32_t dbase = xbase + SX * xs_units * 16u;
+      // descriptors with start address 0; the address field counts 16-byte units
+      const uint64_t bx = gmma_desc(0u, 128u, (uint32_t)LPk * 16u);
+      const uint64_t ad = gmma_desc(0u, 128u, (uint32_t)KC * 16u);
+      const uint64_t xh = bx + (xbase >> 4) + (uint64_t)(kh * PW), xl = xh + xs_units;
+      const uint64_t dh = ad + (dbase >> 4), dl = dh + ds_units;
+      wgmma_fence();
 #pragma unroll
-        for (int kh = 0; kh < 3; ++kh) {
-          const uint32_t off = (uint32_t)(kh * PW);
-          const uint32_t d_tmem = tmem_base + (uint32_t)(kh * NN);
+      for (int ks = 0; ks < KC / 16; ++ks) {
+        const uint32_t ko = (uint32_t)(ks * 16);
+        Wgmma<NN>::template mma<1, 1>(acc, dh + ko, xh + ko, 1u);
+        if (SPLIT) Wgmma<NN>::template mma<1, 1>(acc, dl + ko, xh + ko, 1u);
+        if (XSPLIT) Wgmma<NN>::template mma<1, 1>(acc, dh + ko, xl + ko, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                     // the previous chunk's MMAs have read their stage
+      if (it > 0 && lane == 0) mbar_arrive(s_empty + (it - 1) % nb);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc<NN / 2>(acc);
+    // ---- rows 0..COUT-1 of this kernel row's accumulator -> this CTA's partial ----------------
+    const float scale = IN_MODE == IN_U8 ? (1.0f / 255.0f) : 1.0f;
 #pragma unroll
-          for (int ks = 0; ks < KC / 16; ++ks) {
-            const uint32_t ko = (uint32_t)(ks * 16);
-            umma_f16(d_tmem, dh + ko, xh + ko + off, idesc, (ks > 0) ? 1u : acc0);
-            if (SPLIT) umma_f16(d_tmem, dl + ko, xh + ko + off, idesc, 1u);
-            if (XSPLIT) umma_f16(d_tmem, dh + ko, xl + ko + off, idesc, 1u);
+    for (int h = 0; h < 2; ++h) {
+      const int co = 16 * (warp & 3) + (lane >> 2) + 8 * h;
+      if (co < COUT) {
+#pragma unroll
+        for (int j = 0; j < NN / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = 8 * j + 2 * (lane & 3) + e, kw = n / CP, ci = n - kw * CP;
+            if (ci < CIN) dst[((size_t)(kh * 3 + kw) * CIN + ci) * COUT + co] = acc[4 * j + 2 * h + e] * scale;
           }
         }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                         smem_u32(s_empty + b))
-                     : "memory");
       }
-      __syncwarp();
     }
-    if (elect_one())
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                       smem_u32(s_done))
-                   : "memory");
-    __syncwarp();
   } else {
     // ================================ producers ============================================
     // Two register sets: while chunk i is converted into shared memory, the global loads of
     // chunks i+1 and i+2 are already in flight (the producers are pure latency hiding).
-    const int pt = tid - 32;
+    const int pt = tid - kWgMmaThreads;
     constexpr int IX = wg_ix(G, KC);                                  // host checks L*G <= IX*producers
     constexpr int ID = (KC * GO + kWgProducers - 1) / kWgProducers;
     constexpr int DEPTH = (IX + ID <= 4) ? 2 : 1;                     // register sets of prefetched chunks
@@ -657,34 +588,13 @@ conv3x3_wgrad_tc_kernel(ConvGeom g, const void* __restrict__ x_, const float* __
       for (int it = 0; it < my_chunks; ++it) stage(r0, it);
     }
   }
-  // ---- drain: every MMA of this CTA has completed when s_done flips --------------------------
-  mbar_wait(s_done, 0u, &timed_out);
   if (timed_out && error_flag) atomicExch(error_flag, 1);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  __syncthreads();
+  __syncthreads();                          // every MMA has completed: the stages are free
 
-  // ---- epilogue: rows 0..COUT-1 of each kernel row's accumulator -> this CTA's partial -------
-  float* dst = partial + (size_t)blockIdx.x * NW;
-  // UMMA M = 64 accumulator layout (cute tmem_frg_1sm, M_MMA == 64): row m lives in TMEM
-  // lane (m % 16) + 32 * (m / 16), i.e. 16 rows per 32-lane sub-partition.
-  if (warp < (COUT + 15) / 16) {
-    const float scale = IN_MODE == IN_U8 ? (1.0f / 255.0f) : 1.0f;
-#pragma unroll 1
-    for (int t = 0; t < 9; ++t) {                          // t = kh*3 + kw
-      float v[CP];
-      tmem_ld<CP>(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)((t / 3) * NN + (t % 3) * CP), v);
-      const int co = warp * 16 + lane;
-      if (lane < 16 && co < COUT) {
+  // ---- bias partial: fixed-order reduction over the producers that staged each co-group -------
+  if (tid >= kWgMmaThreads) {
 #pragma unroll
-        for (int ci = 0; ci < CIN; ++ci)
-          dst[((size_t)t * CIN + ci) * COUT + co] = my_chunks > 0 ? v[ci] * scale : 0.f;
-      }
-    }
-  }
-  // bias partial: fixed-order reduction over the producers that staged each co-group
-  if (warp > 0) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) s_bias[(tid - 32) * 8 + c] = bsum[c];
+    for (int c = 0; c < 8; ++c) s_bias[(tid - kWgMmaThreads) * 8 + c] = bsum[c];
   }
   __syncthreads();
   if (tid < COUT) {
@@ -692,11 +602,6 @@ conv3x3_wgrad_tc_kernel(ConvGeom g, const void* __restrict__ x_, const float* __
     float sum = 0.f;
     for (int t = go; t < kWgProducers; t += GO) sum += s_bias[t * 8 + c];   // producer t staged group t % GO
     dst[9 * CIN * COUT + tid] = sum;
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TCOLS));
   }
 }
 
@@ -730,7 +635,7 @@ static int launch_wgrad_tc(int N, int H, int W, const void* x, const float* dy, 
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad_tc: batch too large for 32-bit positions");
   constexpr int NW = 9 * CIN * COUT + COUT;
   const long long nchunks = (g.Q + KC - 1) / KC;
-  int grid = kNumSMs;                       // 1 CTA per SM (TMEM-resident accumulators)
+  int grid = kNumSMs;                       // 1 CTA per SM (register-resident accumulators)
   if (grid > nchunks) grid = (int)nchunks;
   // deferred reduction: this layer's partials get their own slice of the batch buffer and are
   // reduced together with every other layer's by ONE launch at the end of the backward pass
@@ -750,6 +655,20 @@ static int launch_wgrad_tc(int N, int H, int W, const void* x, const float* dy, 
     return SEEDRL_OK;
   }
   return wgrad_reduce(grid, 9 * CIN * COUT, COUT, partial, dw, db, st);
+}
+
+// launch_wgrad_tc for the chunk lengths wg_max_chunk allows; longer ones are never instantiated
+template <int CIN, int COUT, int IN_MODE, int KC>
+static int try_wgrad_tc(int split, int N, int H, int W, const void* x, const float* dy, float* dw, float* db,
+                        float* partial, size_t partial_bytes, int* err, WgradBatch* batch, cudaStream_t st) {
+  if constexpr (KC > wg_max_chunk(CIN < 8 ? 8 : CIN)) {
+    return kWgTryNext;
+  } else {
+    return split ? launch_wgrad_tc<CIN, COUT, IN_MODE, true, KC>(N, H, W, x, dy, dw, db, partial, partial_bytes,
+                                                                 err, batch, st)
+                 : launch_wgrad_tc<CIN, COUT, IN_MODE, false, KC>(N, H, W, x, dy, dw, db, partial, partial_bytes,
+                                                                  err, batch, st);
+  }
 }
 
 __global__ void wgrad_reduce_batch_kernel(const __grid_constant__ ReduceTable t) {
@@ -796,15 +715,10 @@ int conv3x3_wgrad_tc(int cin, int cout, int in_mode, int split, int N, int H, in
 #define SEEDRL_WGTC_CASE(CI, CO_, MODE)                                                          \
   if (cin == CI && cout == CO_ && in_mode == MODE) {                                             \
     int rc = kWgTryNext;                                                                         \
-    if (g_wgrad_kc >= 512)                                                                       \
-      rc = split ? launch_wgrad_tc<CI, CO_, MODE, true, 512>(SEEDRL_WGTC_ARGS)                   \
-                 : launch_wgrad_tc<CI, CO_, MODE, false, 512>(SEEDRL_WGTC_ARGS);                 \
+    if (g_wgrad_kc >= 512) rc = try_wgrad_tc<CI, CO_, MODE, 512>(split, SEEDRL_WGTC_ARGS);         \
     if (rc == kWgTryNext && g_wgrad_kc >= 256)                                                   \
-      rc = split ? launch_wgrad_tc<CI, CO_, MODE, true, 256>(SEEDRL_WGTC_ARGS)                   \
-                 : launch_wgrad_tc<CI, CO_, MODE, false, 256>(SEEDRL_WGTC_ARGS);                 \
-    if (rc == kWgTryNext)                                                                        \
-      rc = split ? launch_wgrad_tc<CI, CO_, MODE, true, 128>(SEEDRL_WGTC_ARGS)                   \
-                 : launch_wgrad_tc<CI, CO_, MODE, false, 128>(SEEDRL_WGTC_ARGS);                 \
+      rc = try_wgrad_tc<CI, CO_, MODE, 256>(split, SEEDRL_WGTC_ARGS);                            \
+    if (rc == kWgTryNext) rc = try_wgrad_tc<CI, CO_, MODE, 128>(split, SEEDRL_WGTC_ARGS);          \
     if (rc == kWgTryNext) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad_tc: image too wide"); \
     return rc;                                                                                   \
   }

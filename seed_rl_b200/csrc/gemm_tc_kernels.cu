@@ -1,23 +1,22 @@
-// Dense-layer GEMMs on the 5th-gen tensor cores (tcgen05 + TMEM): the Linear contractions of
+// Dense-layer GEMMs on the Hopper tensor cores (wgmma): the Linear contractions of
 // dmlab/networks.py:105-118,157-169 (Dense(256), LSTM input projection, their data and weight
 // gradients) with fp32 storage, bf16 (or bf16x3) operands and fp32 accumulation.
 //
 //   C[M,N] (=|+=) op(A)[M,K] * op(B)[K,N]      row-major fp32, leading dims lda/ldb/ldc
 //   TA: A is stored [K,M] (C = A^T B).   TB: B is stored [N,K] (C = A B^T).
 //
-// Either storage order of either operand is ALREADY a canonical no-swizzle UMMA layout once
+// Either storage order of either operand is ALREADY a canonical no-swizzle wgmma layout once
 // 8 contiguous elements are packed into one 16-byte bf16 unit:
 //   contiguous along K  -> K-major :  planes [K/8][rows][8 k],  LBO = plane stride, SBO = 128 B
 //   contiguous along MN -> MN-major:  planes [MN/8][k][8 mn],   LBO = 128 B, SBO = plane stride
-// so there is no transpose anywhere: TA / TB only flip the major-ness bits of the instruction
-// descriptor.  A CTA owns a 128 x BN tile of C (UMMA M = 128, N = BN <= 256) and a slice of K
-// (split-K over blockIdx.z); K is walked in blocks of 64 through two shared-memory stages:
-// all 8 warps convert fp32 global -> bf16 units of stage s while the tensor core works on
-// stage s^1 (its MMAs were committed to that stage's mbarrier).  Split = bf16x3: every
-// operand is staged as hi and lo planes and each K-step issues hi*hi + lo*hi + hi*lo.
-// Epilogue: tcgen05.ld (thread = one row, 16 columns at a time) -> bias / relu / mask /
-// accumulate -> C, or -> the split-K workspace, reduced in slice order by
-// gemm_tc_reduce_kernel (deterministic).
+// so there is no transpose anywhere: TA / TB only flip the transpose bits of the instruction.
+// A CTA owns a 128 x BN tile of C (two warpgroups, 64 rows each, BN <= 128 columns of fp32
+// accumulators in registers) and a slice of K (split-K over blockIdx.z); K is walked in blocks
+// through two shared-memory stages: all 8 warps convert fp32 global -> bf16 units of stage s while
+// the MMAs of stage s^1 run (wgmma.wait_group 1 keeps one K-block in flight).  Split = bf16x3:
+// every operand is staged as hi and lo planes and each K-step issues hi*hi + lo*hi + hi*lo.
+// Epilogue: accumulators -> fp32 tile in shared memory -> bias / relu / mask / accumulate -> C, or
+// -> the split-K workspace, reduced in slice order by gemm_tc_reduce_kernel (deterministic).
 #include <cstdlib>
 
 #include "kernels.h"
@@ -27,9 +26,9 @@ namespace seedrl {
 
 constexpr int kGtThreads = 256;
 constexpr int kGtBM = 128;
+constexpr int kGtMaxBN = 128;   // tile width cap: a warpgroup holds 64 x 128 fp32 accumulators = 64 registers/thread
 // K elements per staged block = template parameter BK (64, 32 or 16): a smaller block shrinks the
 // stage so that several CTAs fit an SM and overlap each other's load / convert / MMA / epilogue phases
-// (measured on the learner's nine GEMM shapes: 322 us at BK = 64, 259 us at BK = 32)
 
 struct GemmTcParams {
   int M, N, K;
@@ -37,7 +36,7 @@ struct GemmTcParams {
   const float* B; int ldb;
   float* C; int ldc;            // final output (splits == 1) ...
   float* ws;                    // ... or split-K partials [splits][M][N]
-  int BN;                       // tile width: multiple of 16, <= 256
+  int BN;                       // tile width: multiple of 16, <= kGtMaxBN
   int kblocks_per_split;        // K blocks (of 64) per blockIdx.z
   int vecA, vecB;               // 16-byte aligned rows: float4 loads
   GemmEpi e;
@@ -109,6 +108,21 @@ __device__ __forceinline__ void store_unit(RawUnit r, bool relu, uint4* hi_dst, 
   if (SPLIT) *lo_dst = pack8_bf16(bf16_resid4(r.a), bf16_resid4(r.b));
 }
 
+// D += A * B for one K = 16 step of a warpgroup: the tile width is a runtime value (a multiple of 16)
+template <int TA, int TB>
+__device__ __forceinline__ void gemm_tc_mma(int bn, float* acc, uint64_t a, uint64_t b) {
+  switch (bn) {
+    case 16: Wgmma<16>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 32: Wgmma<32>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 48: Wgmma<48>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 64: Wgmma<64>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 80: Wgmma<80>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 96: Wgmma<96>::mma<TA, TB>(acc, a, b, 1u); break;
+    case 112: Wgmma<112>::mma<TA, TB>(acc, a, b, 1u); break;
+    default: Wgmma<128>::mma<TA, TB>(acc, a, b, 1u); break;
+  }
+}
+
 template <bool TA, bool TB, bool SPLIT, int kGtBK, bool GATHER>
 __global__ void __launch_bounds__(kGtThreads)
 gemm_tc_kernel(const GemmTcParams p) {
@@ -125,34 +139,18 @@ gemm_tc_kernel(const GemmTcParams p) {
   const int b_items = BN * kGtBK / 8;                                  // 16-byte units actually staged
   const uint32_t stage_units = S * (a_units + b_units);
   uint4* s_buf = reinterpret_cast<uint4*>(smem_raw);
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem_raw + (size_t)2 * stage_units * 16);   // [2] stage free
-  uint64_t* s_done = s_bar + 2;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_done + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int m0 = blockIdx.y * kGtBM, n0 = blockIdx.x * BN;
   const int kb0 = blockIdx.z * p.kblocks_per_split;
   const int nkb_total = (p.K + kGtBK - 1) / kGtBK;
   const int nkb = min(p.kblocks_per_split, nkb_total - kb0);
-  const uint32_t tcols = BN <= 32 ? 32u : (BN <= 64 ? 64u : (BN <= 128 ? 128u : 256u));
-
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar + 1)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_done)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(tcols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-  // instruction descriptor: bf16 x bf16 -> f32, M = 128, N = BN; bit 15 / 16: A / B MN-major
-  const uint32_t idesc = umma_idesc(kGtBM, BN) | (TA ? (1u << 15) : 0u) | (TB ? 0u : (1u << 16));
-  bool ok = true;
+  // warpgroup wg multiplies rows [64 wg, 64 wg + 64) of the tile: K-major A holds a row per 16-byte
+  // unit of a plane, MN-major A 8 rows per plane
+  const uint32_t a_wg = TA ? (uint32_t)wg * 8u * a_ps * 16u : (uint32_t)wg * 64u * 16u;
+  float acc[kGtMaxBN / 2];
+#pragma unroll
+  for (int i = 0; i < kGtMaxBN / 2; ++i) acc[i] = 0.f;
+  wgmma_fence_acc<kGtMaxBN / 2>(acc);
 
   for (int kb = 0; kb < nkb; ++kb) {
     const int st = kb & 1;
@@ -161,8 +159,8 @@ gemm_tc_kernel(const GemmTcParams p) {
     uint4* sB = sA + (size_t)S * a_units;
     // ---- stage the K-block: every global load is issued before the first conversion -------
     // consecutive threads take consecutive 8-element groups of the SAME row (coalesced).
-    constexpr int AI = (kGtBM * kGtBK / 8) / kGtThreads;   // 4 A units per thread
-    constexpr int BI = (256 * kGtBK / 8) / kGtThreads;     // <= 8 B units per thread
+    constexpr int AI = (kGtBM * kGtBK / 8) / kGtThreads;       // A units per thread
+    constexpr int BI = (kGtMaxBN * kGtBK / 8) / kGtThreads;    // <= BI B units per thread
     RawUnit ra[AI], rb[BI];
 #pragma unroll
     for (int r = 0; r < AI; ++r) {
@@ -184,8 +182,9 @@ gemm_tc_kernel(const GemmTcParams p) {
         else    rb[r] = load_raw(p.B, p.ldb, k0 + u / bng, n0 + (u % bng) * 8, p.K, p.N, p.vecB != 0); // B[K,N]
       }
     }
-    // the MMAs that read this stage two K-blocks ago have completed
-    if (kb >= 2) ok = mbar_wait_bounded(s_bar + st, (uint32_t)(((kb >> 1) - 1) & 1)) && ok;
+    // the MMAs that read this stage two K-blocks ago have completed, in both warpgroups
+    if (kb >= 2) wgmma_wait<1>();
+    __syncthreads();
 #pragma unroll
     for (int r = 0; r < AI; ++r) {
       const int u = tid + r * kGtThreads;
@@ -205,81 +204,62 @@ gemm_tc_kernel(const GemmTcParams p) {
     // generic-proxy smem writes -> visible to the tensor core's async proxy
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (warp == 0 && elect_one()) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
+    wgmma_fence();
+    const uint32_t a_addr = smem_u32(sA) + a_wg, b_addr = smem_u32(sB);
 #pragma unroll
-      for (int ks = 0; ks < kGtBK / 16; ++ks) {
-        // K-major: two K-groups = two planes (LBO = plane stride);  MN-major: 16 k-rows = 256 B
-        const uint64_t da = TA ? umma_desc(a_addr + ks * 256u, 128u, a_ps * 16u)
-                               : umma_desc(a_addr + ks * 2u * a_ps * 16u, a_ps * 16u, 128u);
-        const uint64_t db = TB ? umma_desc(b_addr + ks * 2u * b_ps * 16u, b_ps * 16u, 128u)
-                               : umma_desc(b_addr + ks * 256u, 128u, b_ps * 16u);
-        const uint32_t acc = (kb > 0 || ks > 0) ? 1u : 0u;
-        umma_f16(tmem_base, da, db, idesc, acc);
-        if (SPLIT) {   // the address field counts 16-byte units
-          umma_f16(tmem_base, da + a_units, db, idesc, 1u);
-          umma_f16(tmem_base, da, db + b_units, idesc, 1u);
-        }
+    for (int ks = 0; ks < kGtBK / 16; ++ks) {
+      // K-major: two K-groups = two planes (LBO = plane stride);  MN-major: 16 k-rows = 256 B
+      const uint64_t da = TA ? gmma_desc(a_addr + ks * 256u, 128u, a_ps * 16u)
+                             : gmma_desc(a_addr + ks * 2u * a_ps * 16u, a_ps * 16u, 128u);
+      const uint64_t db = TB ? gmma_desc(b_addr + ks * 2u * b_ps * 16u, b_ps * 16u, 128u)
+                             : gmma_desc(b_addr + ks * 256u, 128u, b_ps * 16u);
+      gemm_tc_mma<TA ? 1 : 0, TB ? 0 : 1>(BN, acc, da, db);
+      if (SPLIT) {   // + lo(a)*hi(b) + hi(a)*lo(b); the address field counts 16-byte units
+        gemm_tc_mma<TA ? 1 : 0, TB ? 0 : 1>(BN, acc, da + a_units, db);
+        gemm_tc_mma<TA ? 1 : 0, TB ? 0 : 1>(BN, acc, da, db + b_units);
       }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                       smem_u32(s_bar + st))
-                   : "memory");
-      if (kb == nkb - 1)
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                         smem_u32(s_done))
-                     : "memory");
     }
+    wgmma_commit();
   }
-  if (nkb > 0) ok = mbar_wait_bounded(s_done, 0u) && ok;
-  if (!ok && p.error_flag) atomicExch(p.error_flag, 1);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  wgmma_wait<0>();
+  wgmma_fence_acc<kGtMaxBN / 2>(acc);
 
-  // ---- epilogue: TMEM -> registers (thread = row) -> per-warp 32x32 transpose in shared memory
-  // -> row-contiguous 128-byte global accesses (a thread-per-row store would touch 32 different
-  // sectors per instruction: measured 17 us per 128x256 tile).  The operand stages are free now.
+  // ---- epilogue: registers -> fp32 tile in shared memory (aliasing the operand stages, which no
+  // MMA reads any more once both warpgroups are here) -> row-contiguous global accesses
   __syncthreads();
   {
-    const int q = warp & 3, half = warp >> 2;          // TMEM lane quadrant, column-block parity
-    float* scratch = reinterpret_cast<float*>(smem_raw) + warp * (32 * 33);
-    const bool partial = p.ws != nullptr;
-    const int row0 = m0 + q * 32;
-    for (int cb = half; cb * 32 < BN; cb += 2) {
-      float v[32];
-      if (nkb > 0) {
-        tmem_ld<32>(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(cb * 32), v);
-      } else {
+    const int ld = BN + 4;
+    float* tile = reinterpret_cast<float*>(smem_raw);
+    const int w = (tid >> 5) & 3, l = tid & 31;
+    const int r0 = wg * 64 + 16 * w + (l >> 2), c0 = 2 * (l & 3);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
+    for (int j = 0; j < kGtMaxBN / 8; ++j) {
+      if (8 * j < BN) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(tile + (size_t)(r0 + 8 * h) * ld + 8 * j + c0) =
+              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) scratch[lane * 33 + j] = v[j];
-      __syncwarp();
-      const int gn = n0 + cb * 32 + lane;
-      const bool col_ok = gn < p.N && cb * 32 + lane < BN;
-      const float bias = (!partial && p.e.bias && col_ok) ? __ldg(p.e.bias + gn) : 0.f;
-#pragma unroll 4
-      for (int r = 0; r < 32; ++r) {
-        const int gm = row0 + r;
-        if (gm < p.M && col_ok) {
-          float x = scratch[r * 33 + lane];
-          if (partial) {
-            p.ws[((size_t)blockIdx.z * p.M + gm) * p.N + gn] = x;
-          } else {
-            x += bias;
-            if (p.e.relu) x = fmaxf(x, 0.f);
-            if (p.e.mask) x = __ldg(p.e.mask + (size_t)gm * p.e.ldm + gn) > 0.f ? x : 0.f;
-            float* c = p.C + (size_t)gm * p.ldc + gn;
-            *c = p.e.accumulate ? *c + x : x;
-          }
+    }
+    __syncthreads();
+    const bool partial = p.ws != nullptr;
+    for (int i = tid; i < kGtBM * BN; i += kGtThreads) {
+      const int r = i / BN, c = i - r * BN;
+      const int gm = m0 + r, gn = n0 + c;
+      if (gm < p.M && gn < p.N) {
+        float x = tile[(size_t)r * ld + c];
+        if (partial) {
+          p.ws[((size_t)blockIdx.z * p.M + gm) * p.N + gn] = x;
+        } else {
+          if (p.e.bias) x += __ldg(p.e.bias + gn);
+          if (p.e.relu) x = fmaxf(x, 0.f);
+          if (p.e.mask) x = __ldg(p.e.mask + (size_t)gm * p.e.ldm + gn) > 0.f ? x : 0.f;
+          float* cp = p.C + (size_t)gm * p.ldc + gn;
+          *cp = p.e.accumulate ? *cp + x : x;
         }
       }
-      __syncwarp();
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tcols));
 }
 
 // C = epilogue(sum_z ws[z]) in slice order.  VEC: four columns per thread (N % 4 == 0; the
@@ -398,7 +378,7 @@ int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, in
   p.e = e; p.error_flag = err;
   const int n16 = ((N + 15) / 16) * 16;
   const int BK = g_gemm_bk;
-  int bn = split ? 128 : 256;                           // shared memory: 2 stages x (hi + lo)
+  int bn = kGtMaxBN;
   if (bn > n16) bn = n16;
   // narrower tiles until the grid can cover the SMs (with split-K below)
   const int nkb_all = ceil_div(K, BK);
@@ -424,8 +404,8 @@ int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, in
   const int S = split ? 2 : 1;
   const size_t a_un = ta ? (size_t)(kGtBM / 8) * (BK + 1) : (size_t)(BK / 8) * (kGtBM + 1);
   const size_t b_un = tb ? (size_t)(BK / 8) * (p.BN + 1) : (size_t)(p.BN / 8) * (BK + 1);
-  size_t smem = (size_t)2 * S * (a_un + b_un) * 16 + 64;
-  const size_t epi = (size_t)(kGtThreads / 32) * 32 * 33 * 4;      // the epilogue's transpose scratch aliases the stages
+  size_t smem = (size_t)2 * S * (a_un + b_un) * 16;
+  const size_t epi = (size_t)kGtBM * (p.BN + 4) * 4;      // the epilogue's fp32 tile aliases the stages
   if (smem < epi) smem = epi;
   dim3 grid(ceil_div(N, p.BN), ceil_div(M, kGtBM), splits);
 #define SEEDRL_GT_LAUNCH2(TA_, TB_, SP_, BK_, G_)                                               \

@@ -72,12 +72,12 @@ struct ReduceJob { const float* partial; float* dw; float* db; int nparts, nw, n
 struct ReduceTable { ReduceJob jobs[kMaxReduceJobs]; };
 struct WgradBatch { float* buf; size_t cap_floats, used; int n; ReduceJob jobs[kMaxReduceJobs]; };
 
-// conv_tc_kernels.cu (tcgen05 tensor-core path)
+// conv_tc_kernels.cu (wgmma tensor-core path)
 bool conv3x3_tc_supported(int cin, int cout, int in_mode);
 int conv3x3_tc_pack_weights(int cin, int cout, int flip, int split, const float* w, void* wq,
                             cudaStream_t st);
 bool conv3x3_wgrad_tc_supported(int cin, int cout, int in_mode);
-void conv3x3_wgrad_tc_set_chunk(int kc);   // upper bound: 512 (default), 256 or 128
+void conv3x3_wgrad_tc_set_chunk(int kc);   // upper bound: 512 (8-channel inputs only), 256 (default) or 128
 int conv3x3_wgrad_tc(int cin, int cout, int in_mode, int split, int N, int H, int W, const void* x,
                      const float* dy, float* dw, float* db, float* partial, size_t partial_bytes,
                      int* err, WgradBatch* batch, cudaStream_t st);
@@ -89,7 +89,7 @@ int conv3x3_tc_forward(int cin, int cout, int in_mode, int split, int N, int H, 
                        float* out, int variant, int* err, cudaStream_t st);
 
 // conv_planes.cu ("planes" path: activations stored in HBM as bf16 hi/lo channel-group planes of
-// the padded tall image = the UMMA operand format; TMA-fed, warp-specialised kernels)
+// the padded tall image = the wgmma operand format; TMA-fed, warp-specialised kernels)
 constexpr int kPlanesTryNext = -12347;
 #define SEEDRL_TRY_RC(expr)             \
   do {                                  \
@@ -176,7 +176,7 @@ int sgemm(bool ta, bool tb, int M, int N, int K, const float* A, int lda, const 
 // enables the row-slab path for tall matrices.
 int colsum(int M, int N, const float* X, int ld, float* out, cudaStream_t st, float* ws = nullptr,
            size_t ws_bytes = 0);
-// gemm_tc_kernels.cu (tcgen05): same contract as sgemm; split = bf16x3 operands; `ws` holds
+// gemm_tc_kernels.cu (wgmma): same contract as sgemm; split = bf16x3 operands; `ws` holds
 // split-K partials (gemm_tc_workspace_bytes()); *err is set if a bounded mbarrier wait expires.
 bool gemm_tc_supported(int M, int N, int K);
 void gemm_tc_set_bk(int bk);                 // K elements per staged block: 64 or 32 (tuning knob)

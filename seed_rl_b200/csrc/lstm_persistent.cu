@@ -2,7 +2,7 @@
 // dmlab/networks.py:157-169) -- forward and BPTT -- as ONE cooperative kernel each.
 //
 // The recurrence is latency-bound: per step only B x 256 x 1024 MACs (B = 64) but 2 x T
-// dependent steps.  Launching a GEMM + a pointwise kernel per step costs ~40-90 us/step;
+// dependent steps.  Launching a GEMM + a pointwise kernel per step pays two launches per step;
 // here 128 CTAs stay resident for all T steps, each owning 2 hidden units (8 gate
 // columns): its slice of the recurrent matrix U stays in shared memory, the cell state
 // (forward) / cell-state gradient (backward) of its units stays on chip, and the only

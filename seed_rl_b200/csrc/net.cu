@@ -49,7 +49,7 @@ struct seedrl_net {
   int sh_h1, sh_w1, sh_h2, sh_w2;
   int flat;                                // conv features fed to Dense(256)
   int lstm_mode = 2;                       // 2 = tiled persistent kernels (lstm_tiled.cu), 1 = first persistent form, 0 = per-step launches
-  int conv_mode = 0;                       // 0 = fp32 SIMT, 1 = tcgen05 bf16, 2 = tcgen05 bf16x3 (fp32-faithful)
+  int conv_mode = 0;                       // 0 = fp32 SIMT, 1 = wgmma bf16, 2 = wgmma bf16x3 (fp32-faithful)
   int core_in;                             // 256 + 1 + A
 };
 
@@ -96,7 +96,7 @@ struct StackBufs {
 };
 
 // packed-weight slot: (hi + lo) x 9 x 32 x 32 bf16; deferred weight-gradient partials of all
-// 15 convs: 148 CTAs x 97 680 floats (57.8 MB) rounded up
+// 15 convs: at most one CTA per SM x 97 680 floats (51.6 MB on 132 SMs) rounded up
 constexpr size_t kPackSlotBytes = 2 * 9 * 32 * 32 * 2;
 constexpr size_t kPartialAllBytes = (size_t)64 << 20;
 
@@ -249,7 +249,7 @@ static inline T* W(void* ws, size_t off) {
   return reinterpret_cast<T*>(reinterpret_cast<char*>(ws) + off);
 }
 
-// One dense contraction of the schedule: tcgen05 when the net runs in tensor-core mode and the
+// One dense contraction of the schedule: wgmma when the net runs in tensor-core mode and the
 // shape is worth a 128-row tile, else the fp32 SIMT kernel.
 static int run_gemm(const seedrl_net* n, void* ws, const Plan& pl, bool ta, bool tb, int M, int N, int K,
                     const float* A, int lda, const float* B, int ldb, float* C, int ldc, const GemmEpi& e,
@@ -305,7 +305,7 @@ static const void* find_packed(const float* w, int flip) {
 }
 
 // One 3x3 'same' convolution of the schedule.  flip != 0: data-gradient (weights flipped and
-// transposed; cin/cout are those of the *gradient* convolution).  Dispatches to the tcgen05
+// transposed; cin/cout are those of the *gradient* convolution).  Dispatches to the wgmma
 // kernel when the net runs in tensor-core mode and the shape is supported, else fp32 SIMT.
 static int run_conv(const seedrl_net* n, void* ws, const Plan& pl, int cin, int cout, int in_mode,
                     int N, int H, int Wd, const void* in, const float* w, const float* bias,
@@ -435,7 +435,7 @@ extern "C" int seedrl_net_set_lstm_mode(seedrl_net* net, int mode) {
 }
 extern "C" int seedrl_net_set_conv_mode(seedrl_net* net, int mode) {
   SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 3,
-                   "mode must be 0 (fp32 SIMT), 1 (tcgen05 bf16), 2 (tcgen05 bf16x3) or 3 (bf16x3 plane tensors)");
+                   "mode must be 0 (fp32 SIMT), 1 (wgmma bf16), 2 (wgmma bf16x3) or 3 (bf16x3 plane tensors)");
   SEEDRL_CHECK_ARG(mode != 3 || net->cfg.net == SEEDRL_NET_DEEP, "mode 3 is built for the deep net");
   net->conv_mode = mode;
   return SEEDRL_OK;
@@ -490,7 +490,7 @@ static int torso_forward_deep(const seedrl_net* n, const float* prm, const Plan&
 }
 
 // conv_mode 3: the same _Stack schedule on plane tensors (conv_planes.cu).  The first conv reads the
-// uint8 frames with the staged tcgen05 kernel (bf16x3) and writes fp32 NHWC for the max-pool; from
+// uint8 frames with the staged wgmma kernel (bf16x3) and writes fp32 NHWC for the max-pool; from
 // there on every conv input is a TMA tile of an HBM-resident operand.
 static int planes_conv(const seedrl_net* n, void* ws, const Plan& pl, int cin, int cout, int N, int H, int Wd,
                        const void* in, const float* w, int flip, const float* bias, const void* mask,
@@ -571,7 +571,7 @@ static int torso_forward_shallow(const seedrl_net* n, const float* prm, const Pl
   float* a1 = W<float>(ws, pl.sh_a1);
   float* a2 = W<float>(ws, pl.sh_a2);
   if (n->conv_mode >= 1 && n->cfg.obs_c % 4 == 0) {
-    // tensor-core modes: im2col + tcgen05 GEMM with bias + ReLU in the epilogue (the R2D2 body's path)
+    // tensor-core modes: im2col + wgmma GEMM with bias + ReLU in the epilogue (the R2D2 body's path)
     const int C = n->cfg.obs_c, K0 = 64 * C, K1 = 16 * 16;
     float* col0 = W<float>(ws, pl.sh_col0); float* col1 = W<float>(ws, pl.sh_col1);
     GemmEpi e = epi_none();
@@ -615,7 +615,7 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int N = pl.N, A = n->cfg.num_actions, CI = n->core_in;
-  // bounded-wait error flag of the tcgen05 / persistent kernels: cleared here, set by any kernel of
+  // bounded-wait error flag of the wgmma / persistent kernels: cleared here, set by any kernel of
   // this forward or the matching backward, read back by seedrl_net_check_error
   SEEDRL_CUDA(cudaMemsetAsync(W<int>(ws, pl.tcerr), 0, sizeof(int), st));
   const float* flat_src;
@@ -698,7 +698,7 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
 }
 
 // Reads back the device-side error flag of the last forward/backward that used this workspace
-// (set when a bounded mbarrier / grid-barrier wait of a tcgen05 or persistent kernel expired, i.e.
+// (set when a bounded mbarrier / grid-barrier wait of a wgmma or persistent kernel expired, i.e.
 // the results are garbage).  Synchronises `stream`.
 extern "C" int seedrl_net_check_error(const seedrl_net* n, int T1, int B, void* ws, size_t ws_bytes,
                                       seedrl_stream_t stream) {
@@ -1006,7 +1006,7 @@ extern "C" int seedrl_debug_maxpool(int backward, int N, int H, int W, int C, co
   if (backward) return maxpool3s2_backward(N, H, W, C, x_or_dy, idx, y_or_dx, (cudaStream_t)stream);
   return maxpool3s2_forward(N, H, W, C, x_or_dy, y_or_dx, idx, (cudaStream_t)stream);
 }
-// tcgen05 GEMM test hook (same contract as seedrl_debug_sgemm; split != 0: bf16x3 operands;
+// wgmma GEMM test hook (same contract as seedrl_debug_sgemm; split != 0: bf16x3 operands;
 // ws: >= ws_bytes of scratch for split-K partials, may be null).
 extern "C" int seedrl_debug_gemm_tc(int ta, int tb, int split, int M, int N, int K, const float* A, int lda,
                                     const float* B, int ldb, float* C, int ldc, const float* bias,
@@ -1040,7 +1040,7 @@ extern "C" int seedrl_debug_colsum(int M, int N, const float* X, int ld, float* 
   return colsum(M, N, X, ld, out, (cudaStream_t)stream, ws, ws_bytes);
 }
 
-// tcgen05 conv test hook: packs fp32 HWIO weights (optionally flipped/transposed for the
+// wgmma conv test hook: packs fp32 HWIO weights (optionally flipped/transposed for the
 // data-gradient) into `wq_scratch` (>= 2*9*max(cin,16)*cout*2 bytes) and runs the tensor-core conv.
 // `variant` bit0/bit1 swap LBO/SBO of the A/B descriptors (bring-up aid); *error_flag is
 // set to 1 by the kernel if its bounded mbarrier wait expires.

@@ -1,4 +1,4 @@
-// R2D2 (SURVEY 8(a) row a11) post-network kernels for sm_100a:
+// R2D2 (SURVEY 8(a) row a11) post-network kernels for sm_90a:
 //
 //   r2d2_stack_frames_kernel   atari/networks.py:57-173   bit-packed frame stacking (uint8/int32)
 //   r2d2_loss_kernel           agents/r2d2/learner.py:180-330  h / h^-1, n-step double-DQN
@@ -8,7 +8,7 @@
 //   global-norm clip           tf.clip_by_global_norm, learner.py:608 (clip_norm = 40)
 //
 // Parity: tests/test_gpu_r2d2.py against oracle/r2d2_oracle.py / oracle/r2d2_learner_oracle.py (frame
-// stacking and replay indices bit-exact, loss / priorities / dq within fp32 rounding), on a B200.
+// stacking and replay indices bit-exact, loss / priorities / dq within fp32 rounding), on an H100.
 // The network itself (DuelingLSTMDQNNet forward / backward) is csrc/r2d2_net.cu.  Nothing on the
 // V-trace path calls these kernels.
 //
@@ -170,7 +170,7 @@ extern "C" int seedrl_clip_by_global_norm(size_t n, float* grads, float clip_nor
                                           void* scratch, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(grads && scratch && clip_norm > 0.f, "bad arguments");
   if (n == 0) return SEEDRL_OK;
-  const int parts = 592;                                 // 148 SMs x 4
+  const int parts = 4 * kNumSMs;
   float* partial = reinterpret_cast<float*>(scratch);
   cudaStream_t st = (cudaStream_t)stream;
   sumsq_partial_kernel<<<parts, 256, 0, st>>>(n, grads, partial);

@@ -39,7 +39,7 @@ struct RConv { int k, s, cin, cout, hin, win, hout, wout, w, b; };
 
 struct seedrl_r2d2_net {
   int A, H, W, C;
-  int mode;                               // 0 = fp32 SIMT GEMMs, 2 = tcgen05 bf16x3
+  int mode;                               // 0 = fp32 SIMT GEMMs, 2 = wgmma bf16x3
   int lstm_mode = 2;                      // 2 = tiled persistent LSTM (lstm_tiled.cu), 1 = first persistent form
   std::vector<seedrl::RParam> params;
   size_t arena_floats, logical_params;
@@ -359,7 +359,7 @@ extern "C" int seedrl_r2d2_net_num_param_tensors(const seedrl_r2d2_net* net) {
 extern "C" size_t seedrl_r2d2_net_num_params(const seedrl_r2d2_net* net) { return net ? net->logical_params : 0; }
 extern "C" size_t seedrl_r2d2_net_arena_floats(const seedrl_r2d2_net* net) { return net ? net->arena_floats : 0; }
 extern "C" int seedrl_r2d2_net_set_mode(seedrl_r2d2_net* net, int mode) {
-  SEEDRL_CHECK_ARG(net && (mode == 0 || mode == 2), "mode must be 0 (fp32 SIMT) or 2 (tcgen05 bf16x3)");
+  SEEDRL_CHECK_ARG(net && (mode == 0 || mode == 2), "mode must be 0 (fp32 SIMT) or 2 (wgmma bf16x3)");
   net->mode = mode;
   return SEEDRL_OK;
 }

@@ -1,4 +1,4 @@
-// V-trace kernels for sm_100a.
+// V-trace kernels for sm_90a.
 //
 //  vtrace_kernel            (a1)  common/vtrace.py:34-148
 //  categorical_*_kernel     (a3)  common/parametric_distribution.py:66-74
@@ -893,7 +893,7 @@ static int pick_bb(int T, int B, int A, size_t* smem_bytes) {
   int BB = 16;
   while (BB >= 1 && loss_smem_bytes(T, A, BB) > 200 * 1024) BB >>= 1;
   if (BB == 0) return 0;
-  while (BB > 1 && ceil_div(B, BB) < 148 && (((BB / 2) * A) & 3) == 0) BB >>= 1;
+  while (BB > 1 && ceil_div(B, BB) < kNumSMs && (((BB / 2) * A) & 3) == 0) BB >>= 1;
   *smem_bytes = loss_smem_bytes(T, A, BB);
   return BB;
 }
@@ -912,7 +912,7 @@ static int num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = kNumSMs;
   }
   return n;
 }
@@ -1088,7 +1088,7 @@ extern "C" int seedrl_categorical_sample_counter(int N, int A, const float* logi
 
 extern "C" size_t seedrl_vtrace_loss_scratch_bytes(int T1, int B, int A) {
   (void)T1; (void)A;   // one partial slot per CTA; at most one CTA per column
-  return 256 + (size_t)(B > 148 ? B : 148) * kLossPartials * sizeof(float);
+  return 256 + (size_t)(B > kNumSMs ? B : kNumSMs) * kLossPartials * sizeof(float);
 }
 
 extern "C" int seedrl_vtrace_loss_fwd_bwd(

@@ -34,8 +34,8 @@ class _CudaAgent(object):
   def __init__(self, num_actions, obs_shape=(84, 84, 4), seed=0, device=None, conv_mode='simt',
                lstm_mode='tiled'):
     """conv_mode selects the arithmetic of every contraction (3x3 convs, Dense, LSTM input
-    projection, policy head): 'simt' = fp32 CUDA cores (the 2e-3 parity path), 'tc' = tcgen05
-    tensor cores with bf16 operands and fp32 accumulation, 'tc3' = tcgen05 with bf16x3 split
+    projection, policy head): 'simt' = fp32 CUDA cores (the 2e-3 parity path), 'tc' = wgmma
+    tensor cores with bf16 operands and fp32 accumulation, 'tc3' = wgmma with bf16x3 split
     operands (fp32-faithful)."""
     L = _lib.lib()
     self._num_actions = int(num_actions)

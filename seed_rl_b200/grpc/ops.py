@@ -376,7 +376,7 @@ class Server(object):
           ctypes.byref(h)))
       if name in self._fns:
         raise ValueError('seed_rl_b200: one function per name (round-robin over devices is the '
-                         'multi-process launcher\'s job on B200).')
+                         'multi-process launcher\'s job).')
       self._fns[name] = _Bound(name, f, in_specs, out_specs, f.output_signature, n, h,
                                f.input_signature)
 

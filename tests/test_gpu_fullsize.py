@@ -17,17 +17,15 @@ Tolerances (stated, per mode):
                     sensitivity to a 1e-6 relative parameter perturbation where the step is
                     ill-conditioned (same rule as test_gpu_parity.py:476-496).
 
-Measured on a B200 (round 2): the oracle's OWN gradients move by up to 5.1e-3 (max-rel) under a
-1e-6 relative parameter perturbation at this size -- the step is piecewise smooth (ReLU masks,
-max-pool argmax, rho clipping) and a random-init net sits on many of the kinks.  fp32 SIMT:
-forward 1e-6, worst gradient tensor 1.4e-3.  bf16x3 ('tc3'/'tc3p', ~2^-16 per product): forward
-1.6e-5 / 2.5e-5, gradients 3e-3 typical, 9.2e-3 on the most sensitive tensor (oracle sensitivity
-there 5.1e-3).  So the bf16x3 modes are asserted at 5e-3 (or 4x sensitivity), not at the fp32
-path's 2e-3: that is what the arithmetic meets, and it is stated rather than hidden.
+The oracle's OWN gradients (a CPU computation) move by up to 5.1e-3 (max-rel) under a 1e-6
+relative parameter perturbation at this size -- the step is piecewise smooth (ReLU masks, max-pool
+argmax, rho clipping) and a random-init net sits on many of the kinks.  bf16x3 ('tc3'/'tc3p') carries
+~2^-16 relative rounding per product, so those modes are asserted at 5e-3 (or 4x sensitivity), not at
+the fp32 path's 2e-3: that is what the arithmetic can meet, and it is stated rather than hidden.
 'tc3p' additionally STORES every 16/32-channel activation and gradient as a bf16 hi+lo pair
 (2^-17 = 7.6e-6 relative, i.e. 7.6x the 1e-6 probe perturbation the sensitivity is measured with),
-so its bound is 8x the oracle's sensitivity: measured worst tensors 9.5e-3 / 2.0e-2 where the
-oracle itself moves 2.1e-3 / 5.1e-3 under the probe.
+so its bound is 8x the oracle's sensitivity (the oracle itself moves 2.1e-3 / 5.1e-3 under the probe
+on the two most sensitive tensors).
 """
 import numpy as np
 import pytest

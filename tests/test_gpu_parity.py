@@ -1,6 +1,6 @@
 """GPU parity tests proper: every CUDA entry point, through the C-ABI, against the CPU
 oracle on the same seeded inputs, against the committed golden fixtures, and -- at the
-BASELINE sizes -- through size-independent properties.  Run with `-m gpu` on a B200.
+BASELINE sizes -- through size-independent properties.  Run with `-m gpu` on an H100.
 
 Stated tolerances (fp32):
   V-trace / losses          rtol=atol=1e-5   (expf ulp differences x 20-step accumulation)

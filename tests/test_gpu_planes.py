@@ -1,5 +1,5 @@
 """GPU: the plane-tensor convolution path (csrc/conv_planes.cu, conv_mode 'tc3p') kernel by kernel
-against float64 references: the HBM operand format itself, the TMA-fed tcgen05 forward /
+against float64 references: the HBM operand format itself, the TMA-fed wgmma forward /
 data-gradient conv with every epilogue option (bias, ReLU mask, residual, raw / ReLU'd / fp32
 outputs), the weight + bias gradient, and max-pool forward / backward -- then one toy-size
 learner step against the CPU oracle (the BASELINE-size step is in test_gpu_fullsize.py).
@@ -272,14 +272,13 @@ def test_inference_step_planes_matches_tc3():
 
 @pytest.mark.parametrize('T,B', [(3, 2), (20, 8)])
 def test_first_layer_fused_kernels_match_dense_path(T, B):
-  """csrc/conv_first.cu -- forward: first conv + bias + max-pool in one tcgen05 kernel (im2col in
+  """csrc/conv_first.cu -- forward: first conv + bias + max-pool in one wgmma kernel (im2col in
   shared memory, pooled planes + arg-max taps out); backward: weight gradient of the first conv
-  gathered from the POOLED gradient and the taps -- against the path they replace (staged tcgen05
+  gathered from the POOLED gradient and the taps -- against the path they replace (staged wgmma
   conv -> fp32 NHWC -> pool kernel; pool backward -> full-resolution gradient -> dense weight-gradient
   conv).  Same arithmetic (bf16x3 products, fp32 accumulation), different summation order: loss,
   learner outputs agree to 1e-5 and every gradient tensor to 2e-3 of its max-abs (3e-2 in the conv
-  stacks, whose gradients are sums over 10^5..10^6 cancelling terms: measured 3e-3 .. 1e-2 on these tiny
-  batches; a wrong tap or channel would be an O(1) error; a pooling near-tie may also route one
+  stacks, whose gradients are sums over 10^5..10^6 cancelling terms even on these tiny batches; a wrong tap or channel would be an O(1) error; a pooling near-tie may also route one
   gradient element to the neighbouring tap).  The oracle comparison at full size is test_gpu_fullsize.py."""
   from oracle import learner_oracle, loss_oracle, net_oracle
   from seed_rl_b200 import _lib
@@ -312,7 +311,7 @@ def test_first_layer_fused_kernels_match_dense_path(T, B):
     a, w = grads[0][k], grads[1][k]
     # the first conv's own kernel / bias gradient: exact fp32 products and a different summation
     # tree in the gather vs bf16x3 split of a 75 %-zero full-resolution gradient in the dense path
-    # (measured 3e-3 .. 7e-3 apart: both are sums of ~10^6 cancelling terms)
+    # (both are sums of ~10^6 cancelling terms)
     tol = 3e-2 if k.startswith('stack') else 2e-3     # conv stacks: sums over 10^5..10^6 cancelling terms
     assert np.abs(a - w).max() <= tol * np.abs(w).max() + 1e-12, (k, np.abs(a - w).max() / np.abs(w).max())
 

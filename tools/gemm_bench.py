@@ -1,4 +1,4 @@
-"""Timing of the learner's dense GEMM shapes (N = 1344 rows) on the tcgen05 GEMM:
+"""Timing of the learner's dense GEMM shapes (N = 1344 rows) on the wgmma GEMM:
 back-to-back launches between CUDA events.   python tools/gemm_bench.py [split]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

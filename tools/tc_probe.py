@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 kernels: one launch per case, error vs the CPU oracle
+"""Bring-up probe for the wgmma kernels: one launch per case, error vs the CPU oracle
 printed per case; each case runs in a fresh subprocess so a faulting case cannot poison the
 others.  Usage: python tools/tc_probe.py [case_index]"""
 import os
