@@ -240,6 +240,24 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
           }
         }
         wgmma_commit();
+        // thread = (position row, every other channel group) in the epilogue.  Its mask / residual
+        // operands are loaded while the MMAs run, so their latency is not added after the wait.
+        const int row = (tid & 127) & 63;
+        const int p = tile * MT + m * 64 + row;
+        const int sp = p + PW + 1;
+        const int pix = out_pixel(a.g, p);
+        uint4 mk[GO / 2], rh[GO / 2], rl[GO / 2];
+        if (pix >= 0) {
+#pragma unroll
+          for (int k = 0; k < GO / 2; ++k) {
+            const int go = ((tid & 127) >> 6) + 2 * k;
+            if (a.mask) mk[k] = __ldg(a.mask + (size_t)go * plane_u + sp);
+            if (a.res) {
+              rh[k] = __ldg(a.res + (size_t)go * plane_u + sp);
+              rl[k] = __ldg(a.res + (size_t)(GO + go) * plane_u + sp);
+            }
+          }
+        }
         wgmma_wait<0>();
         wgmma_fence_acc<COUT>(acc);
         // this warpgroup's last block of the tile: its MMAs no longer read the stage
@@ -255,20 +273,16 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
                               acc[4 * j + 2 * h + 1] + acc[4 * (j + COUT / 8) + 2 * h + 1]);
         }
         warpgroup_sync(cw);
-        // thread = (position row, every other channel group): bias / mask / residual -> stores
-        const int row = (tid & 127) & 63;
-        const int p = tile * MT + m * 64 + row;
-        const int sp = p + PW + 1;
-        const int pix = out_pixel(a.g, p);
+        // bias / mask / residual -> stores
         const bool in_store = sp < a.Lp;
 #pragma unroll
-        for (int go = (tid & 127) >> 6; go < GO; go += 2) {
+        for (int k = 0; k < GO / 2; ++k) {
+          const int go = ((tid & 127) >> 6) + 2 * k;
           float x[8];
 #pragma unroll
           for (int e = 0; e < 8; ++e) x[e] = scr[row * SLD + go * 8 + e] + s_bias[go * 8 + e];
           if (pix >= 0 && a.mask) {
-            const uint4 mk = __ldg(a.mask + (size_t)go * plane_u + sp);
-            const uint32_t mw[4] = {mk.x, mk.y, mk.z, mk.w};
+            const uint32_t mw[4] = {mk[k].x, mk[k].y, mk[k].z, mk[k].w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               x[2 * e] = bf16lo(mw[e]) > 0.f ? x[2 * e] : 0.f;
@@ -276,9 +290,8 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
             }
           }
           if (pix >= 0 && a.res) {
-            const uint4 rh = __ldg(a.res + (size_t)go * plane_u + sp), rl = __ldg(a.res + (size_t)(GO + go) * plane_u + sp);
-            const uint32_t hw[4] = {rh.x, rh.y, rh.z, rh.w};
-            const uint32_t lw[4] = {rl.x, rl.y, rl.z, rl.w};
+            const uint32_t hw[4] = {rh[k].x, rh[k].y, rh[k].z, rh[k].w};
+            const uint32_t lw[4] = {rl[k].x, rl[k].y, rl[k].z, rl[k].w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               x[2 * e] += bf16lo(hw[e]) + bf16lo(lw[e]);
