@@ -159,11 +159,15 @@ enum { SEEDRL_NET_DEEP = 0, SEEDRL_NET_SHALLOW = 1 };
 typedef struct seedrl_net_config {
   int32_t net;            /* SEEDRL_NET_* */
   int32_t num_actions;    /* A */
-  int32_t obs_h, obs_w, obs_c;   /* uint8 NHWC observation */
+  int32_t obs_h, obs_w, obs_c;   /* uint8 NHWC observation; SEEDRL_NET_DEEP: obs_c in 1..16 */
 } seedrl_net_config;
 
 typedef struct seedrl_net seedrl_net;   /* opaque: layer table + offsets only */
 
+/* SEEDRL_NET_DEEP takes frames of 1 to 16 channels (anything else: SEEDRL_ERR_INVALID_ARGUMENT); the
+ * first conv kernel keeps the frame's shape [3,3,obs_c,16].  Frames of 3 or 4 channels run in every
+ * conv mode.  Other channel counts run in modes 0 and 3 (mode 3: frames at most 107 pixels wide); the
+ * first layer reads them as they are and zero-fills them to 4, 8 or 16 channels in shared memory. */
 int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out);
 void seedrl_net_destroy(seedrl_net* net);
 int seedrl_net_num_param_tensors(const seedrl_net* net);       /* 39 for deep */
@@ -177,7 +181,9 @@ size_t seedrl_net_arena_floats(const seedrl_net* net);
  * operands with fp32 accumulation, 2 = wgmma with bf16x3 split operands (hi*hi + lo*hi +
  * hi*lo: fp32-faithful to ~2^-16 relative), 3 = the same bf16x3 arithmetic with the 16/32-channel
  * activations and gradients kept in HBM as bf16 hi/lo channel-group planes (the wgmma operand
- * format): TMA-fed, warp-specialised conv kernels (csrc/conv_planes.cu; deep net only). */
+ * format): TMA-fed, warp-specialised conv kernels (csrc/conv_planes.cu; deep net only).
+ * Deep net on frames of other than 3 or 4 channels: modes 1 and 2 return SEEDRL_ERR_INVALID_ARGUMENT,
+ * and so does mode 3 for frames wider or taller than the fused first layer takes (W > 107, or < 3). */
 int seedrl_net_set_conv_mode(seedrl_net* net, int mode);
 /* LSTM recurrence: 2 (default) = one persistent kernel for all T steps each way with CTA = (batch
  * tile, 16 hidden units) and one barrier counter per batch tile (csrc/lstm_tiled.cu); 1 = the first
@@ -434,12 +440,24 @@ int seedrl_debug_set_gemm_bk(int bk);     /* gemm_tc_kernel K elements per stage
  * gathering them while the GEMM stages its operand (default 1; bit-identical results). */
 int seedrl_debug_set_gemm_gather(int on);
 /* 1 = conv_mode 3 keeps the dense first-layer backward (pool backward + full-resolution weight
- * gradient) instead of csrc/conv_first.cu's gather from the pooled gradient (A/B parity tests). */
+ * gradient) instead of csrc/conv_first.cu's gather from the pooled gradient (A/B parity tests).
+ * Process-global; a conv_mode 3 forward or backward of a deep net on frames of other than 3 or 4
+ * channels returns SEEDRL_ERR_INVALID_ARGUMENT while it is on. */
 int seedrl_debug_set_first_layer_dense(int on);
 /* The fused first layer (conv 4->16 on uint8 frames + bias + max-pool 3x3/2 SAME) on its own:
  * pooled plane tensors (raw, ReLU'd) + arg-max taps [N,Ho,Wo,16]. */
 int seedrl_debug_conv0pool(int N, int H, int W, const uint8_t* frames, const float* w, const float* bias,
                            void* praw, void* prelu, uint8_t* idx, int* err, seedrl_stream_t stream);
+/* The same on [N,H,W,C] frames, C in 1..16, weights [3,3,C,16] (3 <= H, 3 <= W <= 107; C = 4 also
+ * needs W % 4 == 0). */
+int seedrl_debug_conv0pool_c(int N, int H, int W, int C, const uint8_t* frames, const float* w, const float* bias,
+                             void* praw, void* prelu, uint8_t* idx, int* err, seedrl_stream_t stream);
+/* The fused first layer's weight gradient on its own: dw [3,3,C,16] and db [16] from [N,H,W,C] frames,
+ * the pooled gradient (16-channel plane tensor [N,Ho,Wo]) and the forward's arg-max taps [N,Ho,Wo,16].
+ * partial: scratch of partial_bytes (3 * 132 * (9*C*16 + 16) floats suffice). */
+int seedrl_debug_first_wgrad_pooled_c(int N, int H, int W, int C, const uint8_t* frames, const void* g_planes,
+                                      const uint8_t* idx, float* dw, float* db, float* partial,
+                                      size_t partial_bytes, seedrl_stream_t stream);
 int seedrl_debug_conv3x3_wgrad(int cin, int cout, int in_mode, int N, int H, int W,
                                const void* x, const float* dy, float* dw, float* db,
                                float* partial, size_t partial_bytes,

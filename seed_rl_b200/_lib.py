@@ -163,6 +163,8 @@ SIGNATURES = {
     'seedrl_debug_set_gemm_bk': (c_int, [c_int]),
     'seedrl_debug_set_first_layer_dense': (c_int, [c_int]),
     'seedrl_debug_conv0pool': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P]),
+    'seedrl_debug_conv0pool_c': (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P]),
+    'seedrl_debug_first_wgrad_pooled_c': (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, c_size_t, P]),
     'seedrl_debug_conv3x3_wgrad_tc':
         (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, c_size_t, P, P]),
     'seedrl_debug_conv3x3_wgrad':

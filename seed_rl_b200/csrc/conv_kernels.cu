@@ -19,11 +19,21 @@
 
 namespace seedrl {
 
+// channels 4*c4 .. 4*c4+3 of pixel pix of [.., C] uint8 frames, zero at and above C
+__device__ __forceinline__ uchar4 load_u8_padded(const void* frames, int pix, int C, int c4) {
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(frames) + (size_t)pix * C + 4 * c4;
+  const int c = 4 * c4;
+  return make_uchar4(c < C ? __ldg(p) : 0, c + 1 < C ? __ldg(p + 1) : 0, c + 2 < C ? __ldg(p + 2) : 0,
+                     c + 3 < C ? __ldg(p + 3) : 0);
+}
+
 // ---------------------------------------------------------------------------
 // conv3x3 (forward, and data-gradient with flipped/transposed weights).
 //   out[pix, co] = epi( sum_{tap,ci} tin(in)[pix+tap, ci] * w[tap][ci][co] )
 //   epi(v) = v (+ bias[co]) ; if mask: v = mask[pix,co] > 0 ? v : 0 ; (+ res[pix,co])
 // 128 threads; warp = (position-warp, output-channel group of 16).
+// IN_U8 with cin_src < CIN: frames of cin_src channels, zero-filled to CIN in shared memory, and
+// weights [3,3,cin_src,COUT] with zero rows for the padding channels (first conv of C-channel frames).
 template <int CIN, int COUT, int IN_MODE>
 struct Conv3x3Cfg {
   static constexpr int kThreads = 128;
@@ -36,7 +46,7 @@ struct Conv3x3Cfg {
 
 template <int CIN, int COUT, int IN_MODE>
 __global__ void __launch_bounds__(128)
-conv3x3_kernel(ConvGeom g, const void* __restrict__ in_, const float* __restrict__ w,
+conv3x3_kernel(ConvGeom g, int cin_src, const void* __restrict__ in_, const float* __restrict__ w,
                const float* __restrict__ bias, const float* __restrict__ mask,
                const float* __restrict__ res, float* __restrict__ out) {
   using Cfg = Conv3x3Cfg<CIN, COUT, IN_MODE>;
@@ -51,7 +61,12 @@ conv3x3_kernel(ConvGeom g, const void* __restrict__ in_, const float* __restrict
   const int q0 = blockIdx.x * QC;
 
   // weights -> smem (vectorised, L2-resident)
-  {
+  if (IN_MODE == IN_U8 && cin_src != CIN) {
+    for (int i = tid; i < 9 * CIN * COUT; i += Cfg::kThreads) {
+      const int co = i % COUT, ci = (i / COUT) % CIN, tap = i / (CIN * COUT);
+      s_w[i] = ci < cin_src ? __ldg(w + (tap * cin_src + ci) * COUT + co) : 0.f;
+    }
+  } else {
     const float4* w4 = reinterpret_cast<const float4*>(w);
     float4* s4 = reinterpret_cast<float4*>(s_w);
     for (int i = tid; i < 9 * CIN * COUT / 4; i += Cfg::kThreads) s4[i] = __ldg(w4 + i);
@@ -65,7 +80,8 @@ conv3x3_kernel(ConvGeom g, const void* __restrict__ in_, const float* __restrict
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (pix >= 0) {
         if (IN_MODE == IN_U8) {
-          const uchar4 u = __ldg(reinterpret_cast<const uchar4*>(in_) + (size_t)pix * C4 + c4);
+          const uchar4 u = cin_src == CIN ? __ldg(reinterpret_cast<const uchar4*>(in_) + (size_t)pix * C4 + c4)
+                                          : load_u8_padded(in_, pix, cin_src, c4);
           const float k = 1.0f / 255.0f;     // dmlab/networks.py:98-100
           v = make_float4(u.x * k, u.y * k, u.z * k, u.w * k);
           // NOTE: x/255 and x*(1/255) differ by <=1 ulp; tolerance documented in tests.
@@ -149,7 +165,7 @@ conv3x3_kernel(ConvGeom g, const void* __restrict__ in_, const float* __restrict
 
 template <int CIN, int COUT, int IN_MODE>
 static int launch_conv3x3(int N, int H, int W, const void* in, const float* w, const float* bias,
-                          const float* mask, const float* res, float* out, cudaStream_t st) {
+                          const float* mask, const float* res, float* out, cudaStream_t st, int cin_src = CIN) {
   using Cfg = Conv3x3Cfg<CIN, COUT, IN_MODE>;
   const ConvGeom g = make_geom(N, H, W);
   const int L = Cfg::QC + 2 * g.PW + 2;
@@ -164,7 +180,7 @@ static int launch_conv3x3(int N, int H, int W, const void* in, const float* w, c
   if (g.Q + Cfg::QC + 4 * g.PW >= (1LL << 31))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3: batch too large for 32-bit positions");
   const long long grid = (g.Q + Cfg::QC - 1) / Cfg::QC;
-  conv3x3_kernel<CIN, COUT, IN_MODE><<<(unsigned)grid, Cfg::kThreads, smem, st>>>(g, in, w, bias,
+  conv3x3_kernel<CIN, COUT, IN_MODE><<<(unsigned)grid, Cfg::kThreads, smem, st>>>(g, cin_src, in, w, bias,
                                                                                  mask, res, out);
   count_launch(g_conv_cat, st);
   SEEDRL_CHECK_LAUNCH();
@@ -187,6 +203,16 @@ int conv3x3_forward(int cin, int cout, int in_mode, int N, int H, int W, const v
   SEEDRL_CONV_CASE(32, 32, IN_RELU)
 #undef SEEDRL_CONV_CASE
   return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3: unsupported (cin,cout,mode)");
+}
+
+// First conv of the deep net on [N,H,W,C] uint8 frames, C in 1..16, 16 output channels: the 4-, 8- or
+// 16-channel kernel with the frames and weights zero-filled to that width in shared memory.
+int conv3x3_u8_forward(int C, int N, int H, int W, const uint8_t* frames, const float* w, const float* bias,
+                       float* out, cudaStream_t st) {
+  if (C >= 1 && C <= 4) return launch_conv3x3<4, 16, IN_U8>(N, H, W, frames, w, bias, nullptr, nullptr, out, st, C);
+  if (C >= 5 && C <= 8) return launch_conv3x3<8, 16, IN_U8>(N, H, W, frames, w, bias, nullptr, nullptr, out, st, C);
+  if (C >= 9 && C <= 16) return launch_conv3x3<16, 16, IN_U8>(N, H, W, frames, w, bias, nullptr, nullptr, out, st, C);
+  return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3_u8: channels must be 1..16");
 }
 
 // w[tap][ci][co] -> wt[8-tap][co][ci]   (data-gradient weights)
@@ -226,8 +252,8 @@ struct WgradCfg {
 
 template <int CIN, int COUT, int IN_MODE>
 __global__ void __launch_bounds__(256)
-conv3x3_wgrad_kernel(ConvGeom g, const void* __restrict__ x_, const float* __restrict__ dy,
-                     float* __restrict__ partial /* [grid][9*CIN*COUT + COUT] */) {
+conv3x3_wgrad_kernel(ConvGeom g, int cin_src, const void* __restrict__ x_, const float* __restrict__ dy,
+                     float* __restrict__ partial /* [grid][9*cin_src*COUT + COUT] */) {
   using Cfg = WgradCfg<CIN, COUT>;
   constexpr int QC = Cfg::QC, G = Cfg::G, PPG = Cfg::PPG, TPG = Cfg::TPG;
   extern __shared__ float smem[];
@@ -261,7 +287,8 @@ conv3x3_wgrad_kernel(ConvGeom g, const void* __restrict__ x_, const float* __res
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (pix >= 0) {
           if (IN_MODE == IN_U8) {
-            const uchar4 u = __ldg(reinterpret_cast<const uchar4*>(x_) + (size_t)pix * C4 + c4);
+            const uchar4 u = cin_src == CIN ? __ldg(reinterpret_cast<const uchar4*>(x_) + (size_t)pix * C4 + c4)
+                                            : load_u8_padded(x_, pix, cin_src, c4);
             const float k = 1.0f / 255.0f;
             v = make_float4(u.x * k, u.y * k, u.z * k, u.w * k);
           } else {
@@ -330,11 +357,18 @@ conv3x3_wgrad_kernel(ConvGeom g, const void* __restrict__ x_, const float* __res
     mine[9 * CIN * COUT + cog * 4 + 2] = bacc.z; mine[9 * CIN * COUT + cog * 4 + 3] = bacc.w;
   }
   __syncthreads();
-  float* dst = partial + (size_t)blockIdx.x * NW;
-  for (int i = tid; i < NW; i += Cfg::kThreads) {
+  // partial in the real [3][3][cin_src][COUT] order (rows of the padding channels are dropped)
+  const int nwr = 9 * cin_src * COUT;
+  float* dst = partial + (size_t)blockIdx.x * (nwr + COUT);
+  for (int i = tid; i < nwr + COUT; i += Cfg::kThreads) {
+    int j = i;
+    if (cin_src != CIN) {
+      const int co = i % COUT, cr = i / COUT, tap = cr / cin_src;
+      j = i < nwr ? (tap * CIN + cr - tap * cin_src) * COUT + co : 9 * CIN * COUT + i - nwr;
+    }
     float s = 0.f;
 #pragma unroll
-    for (int k = 0; k < G; ++k) s += s_red[(size_t)k * NW + i];
+    for (int k = 0; k < G; ++k) s += s_red[(size_t)k * NW + j];
     dst[i] = s;
   }
 }
@@ -351,7 +385,7 @@ __global__ void wgrad_reduce_kernel(int nparts, int nw, int nb, const float* __r
 
 template <int CIN, int COUT, int IN_MODE>
 static int launch_wgrad(int N, int H, int W, const void* x, const float* dy, float* dw, float* db,
-                        float* partial, size_t partial_bytes, cudaStream_t st) {
+                        float* partial, size_t partial_bytes, cudaStream_t st, int cin_src = CIN) {
   using Cfg = WgradCfg<CIN, COUT>;
   const ConvGeom g = make_geom(N, H, W);
   const int L = Cfg::QC + 2 * g.PW + 2;
@@ -373,10 +407,11 @@ static int launch_wgrad(int N, int H, int W, const void* x, const float* dy, flo
   if (grid > nchunks) grid = (int)nchunks;
   if ((size_t)grid * NW * sizeof(float) > partial_bytes)
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad: partial buffer too small");
-  conv3x3_wgrad_kernel<CIN, COUT, IN_MODE><<<grid, Cfg::kThreads, smem, st>>>(g, x, dy, partial);
+  conv3x3_wgrad_kernel<CIN, COUT, IN_MODE><<<grid, Cfg::kThreads, smem, st>>>(g, cin_src, x, dy, partial);
   count_launch(PC_CONV_WGRAD, st);
   SEEDRL_CHECK_LAUNCH();
-  wgrad_reduce_kernel<<<ceil_div(NW, 256), 256, 0, st>>>(grid, 9 * CIN * COUT, COUT, partial, dw, db);
+  wgrad_reduce_kernel<<<ceil_div(9 * cin_src * COUT + COUT, 256), 256, 0, st>>>(grid, 9 * cin_src * COUT, COUT,
+                                                                                 partial, dw, db);
   count_launch(PC_CONV_WGRAD, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
@@ -408,6 +443,18 @@ int conv3x3_wgrad(int cin, int cout, int in_mode, int N, int H, int W, const voi
   SEEDRL_WG_CASE(32, 32, IN_RELU)
 #undef SEEDRL_WG_CASE
   return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad: unsupported (cin,cout,mode)");
+}
+
+// Weight gradient of conv3x3_u8_forward: dw in the real [3,3,C,16] layout.
+int conv3x3_u8_wgrad(int C, int N, int H, int W, const uint8_t* frames, const float* dy, float* dw, float* db,
+                     float* partial, size_t partial_bytes, cudaStream_t st) {
+  if (C >= 1 && C <= 4)
+    return launch_wgrad<4, 16, IN_U8>(N, H, W, frames, dy, dw, db, partial, partial_bytes, st, C);
+  if (C >= 5 && C <= 8)
+    return launch_wgrad<8, 16, IN_U8>(N, H, W, frames, dy, dw, db, partial, partial_bytes, st, C);
+  if (C >= 9 && C <= 16)
+    return launch_wgrad<16, 16, IN_U8>(N, H, W, frames, dy, dw, db, partial, partial_bytes, st, C);
+  return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad_u8: channels must be 1..16");
 }
 
 // ---------------------------------------------------------------------------

@@ -121,18 +121,23 @@ int poolp_forward(int N, int H, int W, int C, const float* x, void* out_raw, voi
 int poolp_backward(int N, int H, int W, int C, const void* dy, const uint8_t* idx, void* dx_planes,
                    float* dx_nhwc, cudaStream_t st);
 
-// conv_first.cu (first layer of the deep net: weight gradient straight from the pooled gradient)
+// conv_first.cu (first layer of the deep net on [N,H,W,C] uint8 frames, C in 1..16: fused conv + pool
+// forward; weight gradient straight from the pooled gradient)
 bool first_wgrad_pooled_supported(int cin, int cout, int H, int W);
-int first_wgrad_pooled(int N, int H, int W, const uint8_t* frames, const void* g_planes, const uint8_t* idx,
+int first_wgrad_pooled(int N, int H, int W, int C, const uint8_t* frames, const void* g_planes, const uint8_t* idx,
                        float* dw, float* db, WgradBatch* batch, cudaStream_t st);
 bool conv0pool_supported(int cin, int cout, int H, int W);
-int conv0pool_forward(int N, int H, int W, const uint8_t* frames, const float* w, const float* bias, void* praw,
-                      void* prelu, uint8_t* idx, int* err, cudaStream_t st);
+int conv0pool_forward(int N, int H, int W, int C, const uint8_t* frames, const float* w, const float* bias,
+                      void* praw, void* prelu, uint8_t* idx, int* err, cudaStream_t st);
 
 // conv_kernels.cu
 int conv3x3_forward(int cin, int cout, int in_mode, int N, int H, int W, const void* in,
                     const float* w, const float* bias, const float* mask, const float* res,
                     float* out, cudaStream_t st);
+int conv3x3_u8_forward(int C, int N, int H, int W, const uint8_t* frames, const float* w, const float* bias,
+                       float* out, cudaStream_t st);
+int conv3x3_u8_wgrad(int C, int N, int H, int W, const uint8_t* frames, const float* dy, float* dw, float* db,
+                     float* partial, size_t partial_bytes, cudaStream_t st);
 int conv3x3_flip_weights(int cin, int cout, const float* w, float* wt, cudaStream_t st);
 size_t conv3x3_wgrad_partial_bytes();
 int wgrad_reduce(int nparts, int nw, int nb, const float* partial, float* dw, float* db,

@@ -272,6 +272,14 @@ static thread_local void* t_head_ready = nullptr;   // cudaEvent_t recorded by s
 // test hook: 1 = keep the dense (pool backward + full-resolution weight gradient) first-layer path
 static int g_first_dense = 0;
 
+// Channels of the frames the deep net's first layer reads: 3-channel frames run on their zero-padded
+// 4-channel copy (PadScope); every other count (1..16) is read as it is, zero-filled in shared memory.
+static inline int first_c(const seedrl_net* n) { return n->cfg.obs_c == 3 ? 4 : n->cfg.obs_c; }
+// frames that only the channel-generic first-layer kernels take (conv modes 0 and 3)
+static inline bool generic_first(const seedrl_net* n) {
+  return n->cfg.net == SEEDRL_NET_DEEP && first_c(n) != 4;
+}
+
 // Packs the weights of every conv of the deep torso with one launch: forward forms, or the
 // flipped/transposed forms of the data-gradient convolutions (all but the first layer).
 static int pack_all_weights(const seedrl_net* n, const float* prm, void* ws, const Plan& pl, int flip,
@@ -285,6 +293,7 @@ static int pack_all_weights(const seedrl_net* n, const float* prm, void* ws, con
     for (int i = 0; i < 5; ++i) {
       const ConvLayer& l = *ls[i];
       if (flip && s == 0 && i == 0) continue;          // no data gradient into the frames
+      if (s == 0 && i == 0 && generic_first(n)) continue;   // conv0pool packs its own [3,3,C,16] weights
       const int cin = flip ? l.cout : l.cin, cout = flip ? l.cin : l.cout;
       if (ctx->packed.n >= kMaxPackJobs) return SEEDRL_OK;
       PackJob j;
@@ -370,10 +379,10 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
   n->p_base_b = add_param(n, "baseline/bias", {1});
   int flat = 0;
   if (cfg->net == SEEDRL_NET_DEEP) {
-    if (cfg->obs_c != 4 && cfg->obs_c != 3) {
+    if (cfg->obs_c < 1 || cfg->obs_c > 16) {
       delete n;
       return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
-                       "seedrl_net_create: the deep net takes 3- or 4-channel uint8 frames");
+                       "seedrl_net_create: the deep net takes uint8 frames with 1 to 16 channels");
     }
     int h = cfg->obs_h, w = cfg->obs_w;
     const int chans[3] = {16, 32, 32};
@@ -398,7 +407,8 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
     for (int s = 0; s < 3; ++s) {
       Stack st;
       const std::string pre = "stack" + std::to_string(s);
-      st.hin = h; st.win = w; st.cin = (s == 0 && c == 3) ? 4 : c; st.c = chans[s];
+      // stack 0: the kernels see the frame's channels zero-padded to 4, 8 or 16
+      st.hin = h; st.win = w; st.cin = s == 0 ? (c <= 4 ? 4 : (c <= 8 ? 8 : 16)) : c; st.c = chans[s];
       st.hout = (h + 1) / 2; st.wout = (w + 1) / 2;
       st.conv = add_conv(n, pre + "/conv", 3, c, st.c);      // the parameter keeps the frame's channel count
       st.conv.cin = st.cin;                                  // ... the kernels see the padded one
@@ -437,6 +447,11 @@ extern "C" int seedrl_net_set_conv_mode(seedrl_net* net, int mode) {
   SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 3,
                    "mode must be 0 (fp32 SIMT), 1 (wgmma bf16), 2 (wgmma bf16x3) or 3 (bf16x3 plane tensors)");
   SEEDRL_CHECK_ARG(mode != 3 || net->cfg.net == SEEDRL_NET_DEEP, "mode 3 is built for the deep net");
+  SEEDRL_CHECK_ARG(!generic_first(net) || (mode != 1 && mode != 2),
+                   "conv modes 1 (tc) and 2 (tc3) take 3- or 4-channel frames in the deep net; use 0 (simt) or 3 (tc3p)");
+  SEEDRL_CHECK_ARG(!generic_first(net) || mode != 3 ||
+                       conv0pool_supported(first_c(net), 16, net->cfg.obs_h, net->cfg.obs_w),
+                   "conv mode 3 (tc3p) takes frames of 3 to 107 pixels per side for this channel count; use 0 (simt)");
   net->conv_mode = mode;
   return SEEDRL_OK;
 }
@@ -472,8 +487,12 @@ static int torso_forward_deep(const seedrl_net* n, const float* prm, const Plan&
     float* c0 = W<float>(ws, b.c0); float* o0 = W<float>(ws, b.o0);
     float* c1 = W<float>(ws, b.c1); float* o1 = W<float>(ws, b.o1);
     // _Stack.__call__, dmlab/networks.py:46-60
-    SEEDRL_TRY(run_conv(n, ws, pl, k.cin, k.c, in_mode, N, k.hin, k.win, in, P(n, prm, k.conv.w),
-                        P(n, prm, k.conv.b), nullptr, nullptr, a0, 0, st));
+    if (s == 0 && generic_first(n))
+      SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, P(n, prm, k.conv.w), P(n, prm, k.conv.b), a0,
+                                    st));
+    else
+      SEEDRL_TRY(run_conv(n, ws, pl, k.cin, k.c, in_mode, N, k.hin, k.win, in, P(n, prm, k.conv.w),
+                          P(n, prm, k.conv.b), nullptr, nullptr, a0, 0, st));
     SEEDRL_TRY(maxpool3s2_forward(N, k.hin, k.win, k.c, a0, p, W<uint8_t>(ws, b.idx), st));
     SEEDRL_TRY(run_conv(n, ws, pl, k.c, k.c, IN_RELU, N, k.hout, k.wout, p, P(n, prm, k.r00.w),
                         P(n, prm, k.r00.b), nullptr, nullptr, c0, 0, st));
@@ -520,10 +539,15 @@ static int torso_forward_planes(const seedrl_net* n, const float* prm, const Pla
     void* c0r = W<void>(ws, b.c0r); void* o0raw = W<void>(ws, b.o0raw);
     void* o0relu = W<void>(ws, b.o0relu); void* c1r = W<void>(ws, b.c1r);
     const bool last = s + 1 == ns;
-    if (s == 0 && conv0pool_supported(k.cin, k.c, k.hin, k.win) && !g_first_dense) {
+    if (s == 0 && generic_first(n) && g_first_dense)
+      return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
+                       "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
+    if (s == 0 && conv0pool_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
       // first conv + bias + max-pool in one kernel: the full-resolution activation never reaches HBM
-      SEEDRL_TRY(conv0pool_forward(N, k.hin, k.win, obs, P(n, prm, k.conv.w), P(n, prm, k.conv.b), praw, prelu,
-                                   W<uint8_t>(ws, b.idx), W<int>(ws, pl.tcerr), st));
+      SEEDRL_TRY(conv0pool_forward(N, k.hin, k.win, first_c(n), obs, P(n, prm, k.conv.w), P(n, prm, k.conv.b), praw,
+                                   prelu, W<uint8_t>(ws, b.idx), W<int>(ws, pl.tcerr), st));
+    } else if (s == 0 && generic_first(n)) {
+      return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv mode 3: the fused first layer takes frames up to 107 pixels wide");
     } else {
       if (s == 0)
         SEEDRL_TRY(run_conv(n, ws, pl, k.cin, k.c, IN_U8, N, k.hin, k.win, obs, P(n, prm, k.conv.w),
@@ -760,8 +784,12 @@ static int torso_backward_deep(const seedrl_net* n, const float* prm, float* grd
     // max-pool, then the stack's first conv
     SEEDRL_TRY(maxpool3s2_backward(N, k.hin, k.win, k.c, gA, W<uint8_t>(ws, b.idx), gF, st));
     const void* x = s == 0 ? (const void*)obs : (const void*)W<float>(ws, pl.st[s - 1].o1);
-    SEEDRL_TRY(conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, x, s == 0 ? IN_U8 : IN_F32, gF, nullptr,
-                        nullptr, s == 0 ? nullptr : gA, ws, pl, st));
+    if (s == 0 && generic_first(n))
+      SEEDRL_TRY(conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, G(n, grd, k.conv.w), G(n, grd, k.conv.b),
+                                  W<float>(ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
+    else
+      SEEDRL_TRY(conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, x, s == 0 ? IN_U8 : IN_F32, gF, nullptr,
+                          nullptr, s == 0 ? nullptr : gA, ws, pl, st));
   }
   return SEEDRL_OK;
 }
@@ -805,11 +833,14 @@ static int torso_backward_planes(const seedrl_net* n, const float* prm, float* g
     SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r01, N, H, Wd, c0r, g3, c0r, nullptr, g2, ws, pl, st));
     SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r00, N, H, Wd, prelu, g2, prelu, g3, g1, ws, pl, st));
     // max-pool, then the stack's first conv
-    if (s == 0 && t_ctx && first_wgrad_pooled_supported(k.cin, k.c, k.hin, k.win) && !g_first_dense) {
+    if (s == 0 && t_ctx && first_wgrad_pooled_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
       // no gradient flows into the frames: the weight gradient is taken straight from the pooled
       // gradient and the pool's arg-max taps (conv_first.cu), the full-resolution tensor never exists
-      SEEDRL_TRY(first_wgrad_pooled(N, k.hin, k.win, obs, g1, W<uint8_t>(ws, b.idx), G(n, grd, k.conv.w),
+      SEEDRL_TRY(first_wgrad_pooled(N, k.hin, k.win, first_c(n), obs, g1, W<uint8_t>(ws, b.idx), G(n, grd, k.conv.w),
                                     G(n, grd, k.conv.b), &t_ctx->wb, st));
+    } else if (s == 0 && generic_first(n)) {
+      return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
+                       "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
     } else if (s == 0) {
       SEEDRL_TRY(poolp_backward(N, k.hin, k.win, k.c, g1, W<uint8_t>(ws, b.idx), nullptr, gF, st));
       SEEDRL_TRY(conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, obs, IN_U8, gF, nullptr, nullptr, nullptr, ws, pl,
@@ -1075,7 +1106,23 @@ extern "C" int seedrl_debug_conv0pool(int N, int H, int W, const uint8_t* frames
                                       void* praw, void* prelu, uint8_t* idx, int* err, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(frames && w && bias && praw && prelu && idx && err, "null pointer");
   SEEDRL_CHECK_ARG(conv0pool_supported(4, 16, H, W), "unsupported frame size");
-  return conv0pool_forward(N, H, W, frames, w, bias, praw, prelu, idx, err, (cudaStream_t)stream);
+  return conv0pool_forward(N, H, W, 4, frames, w, bias, praw, prelu, idx, err, (cudaStream_t)stream);
+}
+extern "C" int seedrl_debug_conv0pool_c(int N, int H, int W, int C, const uint8_t* frames, const float* w,
+                                        const float* bias, void* praw, void* prelu, uint8_t* idx, int* err,
+                                        seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(frames && w && bias && praw && prelu && idx && err, "null pointer");
+  SEEDRL_CHECK_ARG(N >= 1 && conv0pool_supported(C, 16, H, W), "unsupported frame shape");
+  return conv0pool_forward(N, H, W, C, frames, w, bias, praw, prelu, idx, err, (cudaStream_t)stream);
+}
+extern "C" int seedrl_debug_first_wgrad_pooled_c(int N, int H, int W, int C, const uint8_t* frames,
+                                                 const void* g_planes, const uint8_t* idx, float* dw, float* db,
+                                                 float* partial, size_t partial_bytes, seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(frames && g_planes && idx && dw && db && partial, "null pointer");
+  SEEDRL_CHECK_ARG(N >= 1 && first_wgrad_pooled_supported(C, 16, H, W), "unsupported frame shape");
+  WgradBatch wb{partial, partial_bytes / sizeof(float), 0, 0, {}};
+  SEEDRL_TRY(first_wgrad_pooled(N, H, W, C, frames, g_planes, idx, dw, db, &wb, (cudaStream_t)stream));
+  return wgrad_reduce_batch(&wb, (cudaStream_t)stream);
 }
 extern "C" int seedrl_debug_set_first_layer_dense(int on) {
   g_first_dense = on ? 1 : 0;

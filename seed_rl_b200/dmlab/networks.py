@@ -37,9 +37,12 @@ class _CudaAgent(object):
     projection, policy head): 'simt' = fp32 CUDA cores (the 2e-3 parity path), 'tc' = wgmma
     tensor cores with bf16 operands and fp32 accumulation, 'tc3' = wgmma with bf16x3 split
     operands (fp32-faithful)."""
-    L = _lib.lib()
     self._num_actions = int(num_actions)
     self._obs_shape = tuple(int(x) for x in obs_shape)
+    if self._NET == _lib.NET_DEEP and (len(self._obs_shape) != 3 or not 1 <= self._obs_shape[2] <= 16):
+      raise ValueError('ImpalaDeep takes (H, W, C) uint8 frames with 1 to 16 channels, got %s'
+                       % (self._obs_shape,))
+    L = _lib.lib()
     cfg = _lib.NetConfig(self._NET, self._num_actions, *self._obs_shape)
     h = ctypes.c_void_p()
     _lib.check(L.seedrl_net_create(ctypes.byref(cfg), ctypes.byref(h)))
