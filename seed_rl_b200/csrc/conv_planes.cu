@@ -19,13 +19,14 @@
 //   (kh * PW + kw) * 16 bytes.
 //
 // Kernels (all persistent, 1 CTA / SM, warp-specialised, mbarrier pipelines, bounded waits):
-//   convp_kernel<CIN, COUT, NSUB>   forward / data gradient.  warp 0 = TMA producer (one
-//       cp.async.bulk.tensor.3d per tile: box = chunks of positions x (2 * CIN/8 planes), two
-//       smem stages), warps 4..11 = two warpgroups that each take every other 64-position block
-//       of a tile: 9*CIN/16*2 wgmma 64 x {2 COUT, COUT} x 16 into registers, release the stage
-//       on its empty barrier, then the epilogue (accumulators -> per-warpgroup fp32 scratch ->
-//       bias / ReLU-mask / residual -> hi/lo split -> coalesced 16-byte plane stores; optionally
-//       a second, ReLU'd copy for the next conv, or fp32 NHWC for the max-pool / Dense consumers).
+//   convp_kernel<CIN, COUT, NSUB>   forward / data gradient.  warp 16 = TMA producer (one
+//       cp.async.bulk.tensor.3d per tile: box = chunks of positions x (2 * CIN/8 planes), 2..4
+//       smem stages), warps 0..15 = four warpgroups that take the CTA's 64-position blocks
+//       round-robin: 9*CIN/16*2 wgmma 64 x {2 COUT, COUT} x 16 into registers, release the stage
+//       on its empty barrier, then the epilogue straight from the accumulator registers (quad
+//       shuffles -> bias / ReLU-mask / residual -> hi/lo split -> coalesced 16-byte plane stores;
+//       optionally a second, ReLU'd copy for the next conv, or fp32 NHWC for the max-pool / Dense
+//       consumers) while the other warpgroups' MMAs keep the tensor pipe busy.
 //   wgradp_kernel<CP, COUT, KC>     weight + bias gradient: M = (kw, ci) rows from three
 //       kw-shifted TMA copies of the x planes (+ a constant ones row whose accumulator is the bias
 //       gradient), N = (kh, c_out) from three kh-shifted copies of the dy planes, K = positions; one
@@ -134,6 +135,7 @@ struct ConvpArgs {
   int nch;                     // chunks per staged tile (box_chunks of the map)
   int chunk;                   // positions per chunk
   int ntiles;
+  int nb;                      // smem stages
   const uint4* wq;             // packed weights [hi | lo], conv_tc_kernels.cu layout
   const float* bias;           // [COUT] or null
   const uint4* mask;           // hi planes of the ReLU'd forward activation (COUT/8 planes) or null
@@ -144,33 +146,51 @@ struct ConvpArgs {
   int* err;
 };
 
-constexpr int kCpThreads = 384;
+constexpr int kCpWarpgroups = 4;                         // MMA + epilogue warpgroups: warps 0 .. 15
+constexpr int kCpThreads = 128 * kCpWarpgroups + 32;     // + the TMA producer warp
 constexpr int kCpM = 128;
+constexpr int kCpMaxStages = 4;
+
+// 4 x 4 transpose of float2 elements across the lanes of a quad (q = lane & 3): on entry slot u of
+// lane s holds element (s, u), on exit slot s of lane u holds it.  Two butterfly stages; in stage b
+// an element moves iff bit b of its lane and of its slot differ.
+__device__ __forceinline__ void quad_transpose(float2 (&t)[4], int q) {
+#pragma unroll
+  for (int b = 1; b <= 2; b <<= 1) {
+    const bool up = (q & b) != 0;
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (u & b) continue;
+      const float2 send = up ? t[u] : t[u | b];
+      const float2 r = make_float2(__shfl_xor_sync(0xffffffffu, send.x, b), __shfl_xor_sync(0xffffffffu, send.y, b));
+      if (up) t[u] = r; else t[u | b] = r;
+    }
+  }
+}
 
 template <int CIN, int COUT, int NSUB>
 __global__ void __launch_bounds__(kCpThreads, 1)
 convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
   constexpr int G = CIN / 8, GO = COUT / 8, NS = CIN / 16;
   constexpr int MT = NSUB * kCpM;
-  constexpr int SLD = COUT + 4;                          // scratch row pitch (floats)
+  constexpr int NBLK = 2 * NSUB;                         // 64-position blocks per tile
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int PW = a.g.PW;
+  const int PW = a.g.PW, nb = a.nb;
   const uint32_t P = (uint32_t)(a.nch * a.chunk) * 16u;  // plane stride in a stage (bytes)
   const uint32_t stage_bytes = 2u * G * P;
-  uint8_t* s_stage = smem_raw;                           // [2][hi G planes | lo G planes]
-  uint4* s_b = reinterpret_cast<uint4*>(smem_raw + 2 * (size_t)stage_bytes);   // 2 * 9*CIN*COUT bf16
-  float* s_scr = reinterpret_cast<float*>(s_b + 2 * 9 * CIN * COUT / 8);      // [2 warpgroups][64][SLD]
-  float* s_bias = s_scr + 2 * 64 * SLD;
+  uint8_t* s_stage = smem_raw;                           // [nb][hi G planes | lo G planes]
+  uint4* s_b = reinterpret_cast<uint4*>(smem_raw + (size_t)nb * stage_bytes);   // 2 * 9*CIN*COUT bf16
+  float* s_bias = reinterpret_cast<float*>(s_b + 2 * 9 * CIN * COUT / 8);
   uint64_t* s_full = reinterpret_cast<uint64_t*>(s_bias + COUT);
-  uint64_t* s_empty = s_full + 2;
+  uint64_t* s_empty = s_full + kCpMaxStages;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   for (int i = tid; i < 2 * 9 * CIN * COUT / 8; i += kCpThreads) s_b[i] = __ldg(a.wq + i);
   if (tid < COUT) s_bias[tid] = a.bias ? __ldg(a.bias + tid) : 0.f;
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < nb; ++i) {
       mbar_init(s_full + i, 1);
-      mbar_init(s_empty + i, 8);                       // the 8 consumer warps
+      mbar_init(s_empty + i, 4 * kCpWarpgroups);       // every consumer warp, once per tile
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_in)) : "memory");
@@ -181,48 +201,57 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
   const int my_tiles = ((int)blockIdx.x < a.ntiles) ? (a.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   bool timed_out = false;
 
-  if (warp == 0) {
+  if (warp == 4 * kCpWarpgroups) {
     // ================================ TMA producer ============================================
     if (elect_one()) {
       for (int it = 0; it < my_tiles; ++it) {
-        const int s = it & 1;
-        if (it >= 2 && !mbar_wait_bounded(s_empty + s, (uint32_t)(((it >> 1) - 1) & 1))) { timed_out = true; break; }
+        const int s = it % nb;
+        if (it >= nb && !mbar_wait_bounded(s_empty + s, (uint32_t)(((it / nb) - 1) & 1))) { timed_out = true; break; }
         const int tile = (int)blockIdx.x + it * (int)gridDim.x;
         mbar_expect_tx(s_full + s, stage_bytes);
         tma_load_3d(s_stage + (size_t)s * stage_bytes, &tm_in, 0, tile * MT / a.chunk, 0, s_full + s);
       }
     }
     __syncwarp();
-  } else if (warp >= 4) {
+  } else {
     // ============================ MMA + epilogue warpgroups ===================================
     // The tensor core reads the A tile (positions x 16 channels) from shared memory for EVERY
     // instruction -- that, not the FLOP rate, bounds small-N MMAs.  So the bf16x3 product is issued
     // as TWO reads of the activations per (tap, slab): hi(a) x [hi(w) | lo(w)] as one N = 2*COUT
     // instruction, lo(a) x hi(w) accumulated onto its first half; the epilogue adds the halves.
-    const int cw = (warp - 4) >> 2;               // consumer warpgroup 0 / 1
-    const int et = tid - 128;                     // 0 .. 255
-    float* scr = s_scr + cw * 64 * SLD;
+    // Each warpgroup runs one block's MMAs and then its epilogue; the epilogue overlaps the MMAs of
+    // the other warpgroups, which take the next blocks.
+    const int cw = warp >> 2;
     const size_t plane_u = (size_t)a.Lp;          // plane stride in 16-byte units (global)
     if (blockIdx.x == 0) {                        // head margin s in [0, PW + 1): zeros
       const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-      for (int i = et; i < (PW + 1) * 2 * GO; i += kCpThreads - 128) {
+      for (int i = tid; i < (PW + 1) * 2 * GO; i += 128 * kCpWarpgroups) {
         const int pl = i / (PW + 1), s = i - pl * (PW + 1);
         if (a.out_raw) a.out_raw[(size_t)pl * plane_u + s] = z;
         if (a.out_relu) a.out_relu[(size_t)pl * plane_u + s] = z;
       }
     }
+    // epilogue thread = (position row, every other channel group).  In the accumulator the 4 lanes
+    // of a quad hold rows r and r + 8, two channels of every group each; after the quad transposes
+    // lane l holds all 8 channels of row r + 8 (l & 1) in channel groups (l & 3) / 2 + 2k.
+    const int q = lane & 3;
+    const int row = 16 * (warp & 3) + (lane >> 2) + 8 * (q & 1);
     const uint32_t b_base = smem_u32(s_b);
     const uint64_t db0 = gmma_desc(b_base, (uint32_t)(2 * GO) * 128u, 128u);
     for (int it = 0; it < my_tiles; ++it) {
-      const int s = it & 1;
+      const int s = it % nb;
       const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-      if (!mbar_wait_bounded(s_full + s, (uint32_t)((it >> 1) & 1))) { timed_out = true; break; }
+      if (!mbar_wait_bounded(s_full + s, (uint32_t)((it / nb) & 1))) { timed_out = true; break; }
+      // the CTA's blocks, concatenated over its tiles, go round-robin to the warpgroups; one with
+      // no block in this tile releases the stage at once
+      const int m0 = (cw - it * NBLK) & (kCpWarpgroups - 1);
+      if (m0 >= NBLK && lane == 0) mbar_arrive(s_empty + s);
       const uint32_t a_base = smem_u32(s_stage + (size_t)s * stage_bytes);
       // descriptors are advanced by adding to their address field (16-byte units)
       const uint64_t da0 = gmma_desc(a_base, P, 128u);
       const uint64_t lo_off = (uint64_t)((G * P) >> 4), slab_off = (uint64_t)((2 * P) >> 4);
 #pragma unroll 1
-      for (int m = cw; m < 2 * NSUB; m += 2) {
+      for (int m = m0; m < NBLK; m += kCpWarpgroups) {
         float acc[COUT];                          // 64 x 2*COUT: [a*hi(w) + lo(a)*hi(w) | hi(a)*lo(w)]
 #pragma unroll
         for (int i = 0; i < COUT; ++i) acc[i] = 0.f;
@@ -240,9 +269,8 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
           }
         }
         wgmma_commit();
-        // thread = (position row, every other channel group) in the epilogue.  Its mask / residual
-        // operands are loaded while the MMAs run, so their latency is not added after the wait.
-        const int row = (tid & 127) & 63;
+        // the mask / residual operands are loaded while the MMAs run, so their latency is not
+        // added after the wait
         const int p = tile * MT + m * 64 + row;
         const int sp = p + PW + 1;
         const int pix = out_pixel(a.g, p);
@@ -250,7 +278,7 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
         if (pix >= 0) {
 #pragma unroll
           for (int k = 0; k < GO / 2; ++k) {
-            const int go = ((tid & 127) >> 6) + 2 * k;
+            const int go = (q >> 1) + 2 * k;
             if (a.mask) mk[k] = __ldg(a.mask + (size_t)go * plane_u + sp);
             if (a.res) {
               rh[k] = __ldg(a.res + (size_t)go * plane_u + sp);
@@ -261,26 +289,27 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
         wgmma_wait<0>();
         wgmma_fence_acc<COUT>(acc);
         // this warpgroup's last block of the tile: its MMAs no longer read the stage
-        if (m + 2 >= 2 * NSUB && lane == 0) mbar_arrive(s_empty + s);
-        {
-          const int w = warp & 3, r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-          for (int j = 0; j < COUT / 8; ++j)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              *reinterpret_cast<float2*>(scr + (r0 + 8 * h) * SLD + 8 * j + c0) =
-                  make_float2(acc[4 * j + 2 * h] + acc[4 * (j + COUT / 8) + 2 * h],
-                              acc[4 * j + 2 * h + 1] + acc[4 * (j + COUT / 8) + 2 * h + 1]);
-        }
-        warpgroup_sync(cw);
+        if (m + kCpWarpgroups >= NBLK && lane == 0) mbar_arrive(s_empty + s);
         // bias / mask / residual -> stores
         const bool in_store = sp < a.Lp;
 #pragma unroll
         for (int k = 0; k < GO / 2; ++k) {
-          const int go = ((tid & 127) >> 6) + 2 * k;
+          const int go = (q >> 1) + 2 * k;
+          // slot u: hi + lo halves of channel group 2k + u/2, row r + 8 (u & 1), channels 2q, 2q + 1
+          float2 t[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const int j = 2 * k + (u >> 1), h = u & 1;
+            t[u] = make_float2(acc[4 * j + 2 * h] + acc[4 * (j + GO) + 2 * h],
+                               acc[4 * j + 2 * h + 1] + acc[4 * (j + GO) + 2 * h + 1]);
+          }
+          quad_transpose(t, q);
           float x[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) x[e] = scr[row * SLD + go * 8 + e] + s_bias[go * 8 + e];
+          for (int e = 0; e < 4; ++e) {
+            x[2 * e] = t[e].x + s_bias[go * 8 + 2 * e];
+            x[2 * e + 1] = t[e].y + s_bias[go * 8 + 2 * e + 1];
+          }
           if (pix >= 0 && a.mask) {
             const uint32_t mw[4] = {mk[k].x, mk[k].y, mk[k].z, mk[k].w};
 #pragma unroll
@@ -318,7 +347,6 @@ convp_kernel(const __grid_constant__ CUtensorMap tm_in, const ConvpArgs a) {
             o[0] = xa; o[1] = xb;
           }
         }
-        warpgroup_sync(cw);                       // the scratch is rewritten by the next block
       }
     }
   }
@@ -336,8 +364,11 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
   const int CH = planes_chunk();
   const int nch = (L + CH - 1) / CH;
   const size_t stage = (size_t)2 * (CIN / 8) * nch * CH * 16;
-  const size_t smem = 2 * stage + (size_t)2 * 9 * CIN * COUT * 2 + (size_t)2 * 64 * (COUT + 4) * 4 + COUT * 4 + 4 * 8;
-  if (smem > 227 * 1024) return kPlanesTryNext;
+  const size_t fixed = (size_t)2 * 9 * CIN * COUT * 2 + COUT * 4 + 2 * kCpMaxStages * 8;
+  int nb = kCpMaxStages;
+  while (nb > 1 && nb * stage + fixed > 227 * 1024) --nb;
+  if (nb < 2) return kPlanesTryNext;
+  const size_t smem = nb * stage + fixed;
   CUtensorMap tm;
   SEEDRL_TRY_RC(make_plane_map(&tm, c.in, Lp, 2 * (CIN / 8), 0, CH, nch, 2 * (CIN / 8)));
   static bool attr = false;
@@ -347,7 +378,7 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
     attr = true;
   }
   ConvpArgs a;
-  a.g = g; a.Lp = (int)Lp; a.nch = nch; a.chunk = CH;
+  a.g = g; a.Lp = (int)Lp; a.nch = nch; a.chunk = CH; a.nb = nb;
   a.ntiles = (int)((Lp - g.PW - 1 + MT - 1) / MT);       // every storage position >= PW + 1 is written
   a.wq = reinterpret_cast<const uint4*>(c.wq); a.bias = c.bias;
   a.mask = reinterpret_cast<const uint4*>(c.mask); a.res = reinterpret_cast<const uint4*>(c.res);

@@ -56,11 +56,6 @@ __device__ __forceinline__ void wgmma_fence_acc(float* d) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// barrier over the 128 threads of warpgroup `wg` (named barriers 1.. ; 0 is __syncthreads)
-__device__ __forceinline__ void warpgroup_sync(int wg) {
-  asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory");
-}
-
 __device__ __forceinline__ uint4 pack8_bf16(float4 a, float4 c) {
   __nv_bfloat162 p0 = __floats2bfloat162_rn(a.x, a.y), p1 = __floats2bfloat162_rn(a.z, a.w);
   __nv_bfloat162 p2 = __floats2bfloat162_rn(c.x, c.y), p3 = __floats2bfloat162_rn(c.z, c.w);
