@@ -27,11 +27,12 @@
 //       shuffles -> bias / ReLU-mask / residual -> hi/lo split -> coalesced 16-byte plane stores;
 //       optionally a second, ReLU'd copy for the next conv, or fp32 NHWC for the max-pool / Dense
 //       consumers) while the other warpgroups' MMAs keep the tensor pipe busy.
-//   wgradp_kernel<CP, COUT, KC>     weight + bias gradient: M = (kw, ci) rows from three
-//       kw-shifted TMA copies of the x planes (+ a constant ones row whose accumulator is the bias
-//       gradient), N = (kh, c_out) from three kh-shifted copies of the dy planes, K = positions; one
-//       warpgroup per 64 rows holds its accumulator in registers; per-CTA partials reduced in
-//       fixed order by the deferred reduce of conv_tc_kernels.cu.
+//   wgradp_kernel<CP, COUT, KC>     weight + bias gradient: one TMA copy of x and of dy per K chunk
+//       (+ halo); M = (kw, ci) rows (+ a constant row whose accumulator is the bias gradient) built
+//       in registers by ldmatrix with the kw shift in each lane's address, N = (hi | lo, c_out) per
+//       kh as a descriptor offset into dy, K = positions; three warpgroups per 64 rows (one per kh)
+//       for 16-channel inputs, one for 32; every warpgroup takes every chunk of the CTA in order;
+//       per-CTA partials reduced in fixed order by the deferred reduce of conv_tc_kernels.cu.
 //   poolp_fwd / poolp_bwd / to_planes / from_planes: elementwise format kernels.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -420,132 +421,155 @@ int convp_forward(int cin, int cout, const PlaneConv& c, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------------
 // weight + bias gradient
 //   dW[kh][kw][ci][co] = sum_p x~[p + kh*PW + kw][ci] * dy[p][co]
-//                      = sum_j x~[j + PW + kw][ci] * dy[j + (1 - kh)*PW][co]        (j = p + (kh-1)*PW)
-// GEMM with K = positions j (chunks of KC), M = (kw, ci) rows, N = (kh, co) columns:
-//   A  = three kw-shifted TMA copies of the x planes (no halo) + one constant plane whose first
-//        channel is 1 (its accumulator row is the bias gradient);  MN-major, 128 rows
-//   B  = three kh-shifted TMA copies of the dy planes; MN-major, hi planes then lo planes
-// so the activation tile -- the operand whose shared-memory read bounds small-N MMAs -- is read
-// TWICE per 16 positions:
-//   hi(x) x [hi(dy) kh=0..2 | lo(dy) kh=0..2]   N = 6*COUT   -> D[:, 0 : 6*COUT]
-//   lo(x) x  hi(dy) kh=0..2                     N = 3*COUT   -> accumulated onto D[:, 0 : 3*COUT]
-// Terms with j < 0 pair the zero row above the first image with dy and vanish.  Warp 0 issues the
-// TMA copies; warpgroup c (warps 4 + 4c ..) multiplies rows [64 c, 64 c + 64) of M (one warpgroup for
-// 16-channel inputs: 3*16 + 1 rows, two for 32-channel inputs) and keeps the 64 x 6*COUT accumulator
-// in registers across all chunks of the CTA.
+//                      = sum_j x~[j + PW + kw][ci] * dy[j + (2 - kh)*PW + 1][co]      (storage positions,
+//                                                                                    j = p + (kh-1)*PW)
+// GEMM with K = positions j (chunks of KC), M = (kw, ci) rows (+ one row whose accumulator is the
+// bias gradient), N = (hi | lo, co) columns, one MMA per kh.  Each operand is copied from L2 ONCE
+// per chunk, plus a halo, and the nine tap shifts are made on chip:
+//   x  hi + lo planes over [j0 + PW, j0 + PW + KC + 8)           -> A, built in registers:
+//      ldmatrix.trans with each lane's row address moved by its kw; the bias row (1.0 in channel
+//      0) and the rows past it are constant fragments
+//   dy hi + lo planes over [j0 + 1, j0 + 1 + KC + T), T = 2*PW rounded up to 8   -> B, MN-major in
+//      shared memory; kh is the descriptor start address moved by (2 - kh) * PW positions
+// A stage is copied per plane as KC/CH rows of CH positions plus a halo of 8-position rows, so the
+// halo is not rounded up to a whole CH-position row.  Per 16 positions and kh:
+//   hi(x) x [hi(dy) | lo(dy)]   N = 2*COUT
+//   lo(x) x  hi(dy)             N = COUT, accumulated onto the first half
+// Terms with j < 0 pair the zero row above the first image with dy and vanish.  Warp 4*NCW issues
+// the TMA copies.  Each 64-row M-tile has KSPL warpgroups that split the three kh between them (one
+// each for 16-channel inputs, so one warpgroup's fragment loads and waits run under the others'
+// MMAs; one for all three at 32 channels, where two M-tiles already give two warpgroups).  Every
+// warpgroup multiplies every chunk of the CTA, in order, into its own accumulator columns: each
+// output element is summed over the same positions, in the same order and in the same MMA
+// groupings whichever warpgroup holds it, so the partials do not depend on the split.
 struct WgradpArgs {
-  int PW, nchx, nchunks, nb;            // TMA chunks per box (x and dy alike); K chunks; stages
-  int chunk;                            // positions per TMA chunk
+  int PW, T, nchunks, nb;               // dy halo positions per chunk; K chunks; stages
+  int chunk;                            // positions per TMA box row of the main copies
   float* partial;                       // [grid][9*CIN*COUT + COUT]
   int* err;
 };
 
-constexpr int kWpMaxStages = 4;
-__host__ __device__ constexpr int wgradp_mrows(int CP) { return 3 * (CP / 8) + 1 <= 8 ? 64 : 128; }
-__host__ __device__ constexpr int wgradp_threads(int CP) { return 128 + 2 * wgradp_mrows(CP); }
+constexpr int kWpMaxStages = 6;
+constexpr int kWpHaloRow = 8;           // positions per TMA box row of the halo copies
+__host__ __device__ constexpr int wgradp_mtiles(int CP) { return 3 * CP + 1 <= 64 ? 1 : 2; }
+__host__ __device__ constexpr int wgradp_khsplit(int CP) { return CP == 16 ? 3 : 1; }   // warpgroups per M-tile
+__host__ __device__ constexpr int wgradp_threads(int CP) { return 128 * wgradp_mtiles(CP) * wgradp_khsplit(CP) + 32; }
 
-struct WgradMaps { CUtensorMap x[3], dy[3]; };
+struct WgradMaps { CUtensorMap x, x_halo, dy, dy_halo; };
 
 template <int CP, int COUT, int KC>
 __global__ void __launch_bounds__(wgradp_threads(CP), 1)
 wgradp_kernel(const __grid_constant__ WgradMaps tm, const WgradpArgs a) {
   constexpr int G = CP / 8, GO = COUT / 8;
-  constexpr int XG = 3 * G + 1;                          // M groups per half: (kw, g) planes + ones/zeros plane
-  constexpr int MROWS = wgradp_mrows(CP);                // 64: the 16-channel case fills 49 rows of one warpgroup
-  constexpr int NCW = MROWS / 64;                        // MMA warpgroups
-  constexpr int THREADS = wgradp_threads(CP);
+  constexpr int MT = wgradp_mtiles(CP), KSPL = wgradp_khsplit(CP), NCW = MT * KSPL;
+  constexpr int NKH = 3 / KSPL;                             // kh per warpgroup
   constexpr int NW = 9 * CP * COUT + COUT;
+  constexpr uint32_t Px = (KC + kWpHaloRow) * 16;           // x plane stride in a stage (bytes)
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int nb = a.nb;
-  const uint32_t Pk = (uint32_t)(a.nchx * a.chunk) * 16u;   // plane stride (bytes), x and dy alike
-  const uint32_t xh_bytes = (uint32_t)XG * Pk;
-  const uint32_t dh_bytes = (uint32_t)(3 * GO) * Pk;
-  const uint32_t stage_bytes = 2u * xh_bytes + 2u * dh_bytes;   // [x hi | x lo | dy hi (kh,go) | dy lo (kh,go)]
+  const int nb = a.nb, PW = a.PW;
+  const uint32_t Pd = (uint32_t)(KC + a.T) * 16u;           // dy plane stride
+  const uint32_t x_bytes = 2u * G * Px;
+  const uint32_t stage_bytes = x_bytes + 2u * GO * Pd;      // [x hi | x lo | dy hi | dy lo]
   uint64_t* s_full = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* s_empty = s_full + kWpMaxStages;
   uint8_t* s_stage = smem_raw + 128;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  // the constant planes of every stage: ones (x hi, channel 0 of each position) and zeros (x lo)
-  for (int i = tid; i < nb * (int)(Pk / 16); i += THREADS) {
-    const int sg = i / (int)(Pk / 16), k = i - sg * (int)(Pk / 16);
-    uint4* xh = reinterpret_cast<uint4*>(s_stage + (size_t)sg * stage_bytes + (size_t)(XG - 1) * Pk);
-    uint4* xl = reinterpret_cast<uint4*>(s_stage + (size_t)sg * stage_bytes + xh_bytes + (size_t)(XG - 1) * Pk);
-    xh[k] = make_uint4(0x00003F80u, 0u, 0u, 0u);        // bf16 1.0 in channel 0
-    xl[k] = make_uint4(0u, 0u, 0u, 0u);
-  }
   if (tid == 0) {
     for (int i = 0; i < kWpMaxStages; ++i) { mbar_init(s_full + i, 1); mbar_init(s_empty + i, 4 * NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
 
   const int my_chunks = ((int)blockIdx.x < a.nchunks) ? (a.nchunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   bool timed_out = false;
 
-  if (warp == 0) {
+  if (warp == 4 * NCW) {
     if (elect_one()) {
-      const uint32_t tx = (uint32_t)(6 * G + 6 * GO) * Pk;
       for (int it = 0; it < my_chunks; ++it) {
         const int s = it % nb;
         if (it >= nb && !mbar_wait_bounded(s_empty + s, (uint32_t)(((it / nb) - 1) & 1))) { timed_out = true; break; }
-        const int c0 = ((int)blockIdx.x + it * (int)gridDim.x) * KC / a.chunk;
-        uint8_t* base = s_stage + (size_t)s * stage_bytes;
-        mbar_expect_tx(s_full + s, tx);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          tma_load_3d(base + (size_t)(k * G) * Pk, &tm.x[k], 0, c0, 0, s_full + s);                  // x hi, kw = k
-          tma_load_3d(base + xh_bytes + (size_t)(k * G) * Pk, &tm.x[k], 0, c0, G, s_full + s);       // x lo
-          tma_load_3d(base + 2 * (size_t)xh_bytes + (size_t)(k * GO) * Pk, &tm.dy[k], 0, c0, 0, s_full + s);   // dy hi, kh = k
-          tma_load_3d(base + 2 * (size_t)xh_bytes + dh_bytes + (size_t)(k * GO) * Pk, &tm.dy[k], 0, c0, GO, s_full + s);
+        const int j0 = ((int)blockIdx.x + it * (int)gridDim.x) * KC;
+        uint8_t* xs = s_stage + (size_t)s * stage_bytes;
+        uint8_t* ds = xs + x_bytes;
+        mbar_expect_tx(s_full + s, stage_bytes);
+        for (int p = 0; p < 2 * G; ++p) {
+          tma_load_3d(xs + p * Px, &tm.x, 0, j0 / a.chunk, p, s_full + s);
+          tma_load_3d(xs + p * Px + KC * 16, &tm.x_halo, 0, (j0 + KC) / kWpHaloRow, p, s_full + s);
+        }
+        for (int p = 0; p < 2 * GO; ++p) {
+          tma_load_3d(ds + p * Pd, &tm.dy, 0, j0 / a.chunk, p, s_full + s);
+          tma_load_3d(ds + p * Pd + KC * 16, &tm.dy_halo, 0, (j0 + KC) / kWpHaloRow, p, s_full + s);
         }
       }
     }
     __syncwarp();
-  } else if (warp >= 4) {
-    // both operands MN-major
-    const int cw = (warp - 4) >> 2;
-    float acc[3 * COUT];                          // 64 x 6*COUT: [x * hi(dy) kh=0..2 | hi(x) * lo(dy) kh=0..2]
+  } else {
+    const int cw = warp >> 2, mt = cw % MT, kh0 = (cw / MT) * NKH;
+    // M group m (8 rows) = (kw, g) = (m / G, m % G) for m < 3G.  This lane gives row (lane & 7) of
+    // ldmatrix matrix lane >> 3: M group mg0 + ((lane >> 3) & 1), K half lane >> 4
+    const int mg0 = 8 * mt + 2 * (warp & 3);
+    const int mg = mg0 + ((lane >> 3) & 1);
+    const uint32_t a_off = (mg < 3 * G ? (uint32_t)(mg % G) * Px + (uint32_t)(mg / G) * 16u : 0u) +
+                           (uint32_t)((lane >> 4) * 8 + (lane & 7)) * 16u;
+    // groups past the data: group 3G is the bias row (row 0 = 1.0, its lo part 0), the rest zeros
+    const bool data0 = mg0 < 3 * G, data1 = mg0 + 1 < 3 * G;
+    const uint32_t one = (lane >> 2) == 0 ? 0x3F803F80u : 0u;
+    const uint32_t c0 = mg0 == 3 * G ? one : 0u, c1 = mg0 + 1 == 3 * G ? one : 0u;
+    float acc[NKH][COUT];                         // per kh: 64 x 2*COUT [x * hi(dy) | hi(x) * lo(dy)]
 #pragma unroll
-    for (int i = 0; i < 3 * COUT; ++i) acc[i] = 0.f;
-    wgmma_fence_acc<3 * COUT>(acc);
-    // descriptors with start address 0 (the address field counts 16-byte units)
-    const uint64_t d0 = gmma_desc(0u, 128u, Pk);
+    for (int i = 0; i < NKH * COUT; ++i) (&acc[0][0])[i] = 0.f;
+    wgmma_fence_acc<NKH * COUT>(&acc[0][0]);
+    // B descriptors: the start address is in the low word (beside LBO), so offsets are 32-bit adds
+    const uint64_t desc0 = gmma_desc(0u, 128u, Pd);
+    const uint32_t desc_lo = (uint32_t)desc0, desc_hi = (uint32_t)(desc0 >> 32);
     for (int it = 0; it < my_chunks; ++it) {
       const int s = it % nb;
       if (!mbar_wait_bounded(s_full + s, (uint32_t)((it / nb) & 1))) { timed_out = true; break; }
-      const uint32_t xb = smem_u32(s_stage + (size_t)s * stage_bytes);
-      const uint32_t db = xb + 2u * xh_bytes;
-      const uint64_t xh = d0 + (xb >> 4) + (uint64_t)cw * ((8u * Pk) >> 4), xl = xh + (xh_bytes >> 4);
-      const uint64_t dh = d0 + (db >> 4);
-      wgmma_fence();
+      const uint32_t sb = smem_u32(s_stage + (size_t)s * stage_bytes);
+      const uint32_t xb = sb + a_off;
+      const uint32_t db = desc_lo + ((sb + x_bytes) >> 4) + (uint32_t)((2 - kh0) * PW);     // kh = kh0
+      uint32_t ah[2][4], al[2][4];                // fragments of 16 positions, double-buffered
 #pragma unroll
       for (int ks = 0; ks < KC / 16; ++ks) {
-        const uint32_t ko = (uint32_t)(ks * 16);
-        Wgmma<6 * COUT>::template mma<1, 1>(acc, xh + ko, dh + ko, 1u);
-        Wgmma<3 * COUT>::template mma<1, 1>(acc, xl + ko, dh + ko, 1u);
+        uint32_t(&h)[4] = ah[ks & 1];
+        uint32_t(&l)[4] = al[ks & 1];
+        ldsm_x4_trans(h, xb + ks * 256);
+        ldsm_x4_trans(l, xb + G * Px + ks * 256);
+        if (!data0) { h[0] = h[2] = c0; l[0] = l[2] = 0u; }
+        if (!data1) { h[1] = h[3] = c1; l[1] = l[3] = 0u; }
+        wgmma_fence();
+#pragma unroll
+        for (int kh = 0; kh < NKH; ++kh) {
+          const uint64_t b = make_desc64(db - (uint32_t)(kh * PW) + (uint32_t)(ks * 16), desc_hi);
+          WgmmaRA<2 * COUT>::template mma<1>(acc[kh], h, b, 1u);
+          WgmmaRA<COUT>::template mma<1>(acc[kh], l, b, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                          // ks - 1 is done: its fragment buffer is free
       }
-      wgmma_commit();
-      wgmma_wait<1>();                            // the previous chunk's MMAs have read their stage
-      if (it > 0 && lane == 0) mbar_arrive(s_empty + (it - 1) % nb);
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(s_empty + s);
     }
-    wgmma_wait<0>();
-    wgmma_fence_acc<3 * COUT>(acc);
+    wgmma_fence_acc<NKH * COUT>(&acc[0][0]);
     // ---- rows (kw, ci) of the accumulator -> this CTA's partial ------------------------------------
     float* dst = a.partial + (size_t)blockIdx.x * NW;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int row = 64 * cw + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+      const int row = 64 * mt + 16 * (warp & 3) + (lane >> 2) + 8 * h;
       const int kw = row / CP, ci = row - kw * CP;
 #pragma unroll
-      for (int j = 0; j < 3 * COUT / 8; ++j) {
+      for (int k = 0; k < NKH; ++k) {
+        const int kh = kh0 + k;
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int n = 8 * j + 2 * (lane & 3) + e, kh = n / COUT, co = n - kh * COUT;
-          const float v = acc[4 * j + 2 * h + e] + acc[4 * (j + 3 * COUT / 8) + 2 * h + e];
-          if (row < 3 * CP) dst[((size_t)(kh * 3 + kw) * CP + ci) * COUT + co] = v;
-          else if (row == 3 * CP && kh == 1) dst[9 * CP * COUT + co] = v;   // ones row x the unshifted dy copy
+        for (int j = 0; j < GO; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = 8 * j + 2 * (lane & 3) + e;
+            const float v = acc[k][4 * j + 2 * h + e] + acc[k][4 * j + 2 * h + e + COUT / 2];
+            if (row < 3 * CP) dst[((size_t)(kh * 3 + kw) * CP + ci) * COUT + co] = v;
+            else if (row == 3 * CP && kh == 1) dst[9 * CP * COUT + co] = v;   // bias row x the kh = 1 view
+          }
         }
       }
     }
@@ -558,25 +582,20 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
                          WgradBatch* batch, cudaStream_t st) {
   const ConvGeom g = make_geom(N, H, W);
   const long long Lp = planes_positions(N, H, W);
-  constexpr int G = CP / 8, GO = COUT / 8, XG = 3 * G + 1;
+  constexpr int G = CP / 8, GO = COUT / 8;
   const int CH = planes_chunk() < KC ? planes_chunk() : KC;    // K chunks start on multiples of KC
   if (KC % CH) return kPlanesTryNext;
-  const int nchx = KC / CH;
-  const size_t Pk = (size_t)KC * 16;
-  const size_t stage = 2 * XG * Pk + 2 * 3 * GO * Pk;
-  // the MMAs read 8 * (M / 64) row groups from each x half: groups past XG are junk rows (never
-  // read back) whose addresses stay inside the stage (x lo is followed by the dy planes)
-  const long long over = (long long)(wgradp_mrows(CP) / 8 - XG) * (long long)Pk - (long long)(6 * GO) * (long long)Pk;
-  const size_t tail = (over > 0 ? (size_t)over : 0) + 256;
+  const int T = (2 * g.PW + kWpHaloRow - 1) / kWpHaloRow * kWpHaloRow;
+  const size_t stage = (size_t)2 * G * (KC + kWpHaloRow) * 16 + (size_t)2 * GO * (KC + T) * 16;
   int nb = kWpMaxStages;
-  while (nb > 1 && 128 + nb * stage + tail > 227 * 1024) --nb;
+  while (nb > 1 && 128 + nb * stage > 227 * 1024) --nb;
   if (nb < 2) return kPlanesTryNext;
-  const size_t smem = 128 + nb * stage + tail;
+  const size_t smem = 128 + nb * stage;
   WgradMaps tm;
-  for (int k = 0; k < 3; ++k) {
-    SEEDRL_TRY_RC(make_plane_map(&tm.x[k], x, Lp, 2 * G, g.PW + k, CH, nchx, G));               // kw = k
-    SEEDRL_TRY_RC(make_plane_map(&tm.dy[k], dy, Lp, 2 * GO, (2 - k) * g.PW + 1, CH, nchx, GO));  // kh = k
-  }
+  SEEDRL_TRY_RC(make_plane_map(&tm.x, x, Lp, 2 * G, g.PW, CH, KC / CH, 1));
+  SEEDRL_TRY_RC(make_plane_map(&tm.x_halo, x, Lp, 2 * G, g.PW, kWpHaloRow, 1, 1));
+  SEEDRL_TRY_RC(make_plane_map(&tm.dy, dy, Lp, 2 * GO, 1, CH, KC / CH, 1));
+  SEEDRL_TRY_RC(make_plane_map(&tm.dy_halo, dy, Lp, 2 * GO, 1, kWpHaloRow, T / kWpHaloRow, 1));
   static bool attr = false;
   if (!attr) {
     SEEDRL_CUDA(cudaFuncSetAttribute(wgradp_kernel<CP, COUT, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -584,10 +603,10 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
     attr = true;
   }
   static const bool dbg = getenv("SEEDRL_DEBUG_LAUNCH") != nullptr;
-  if (dbg) fprintf(stderr, "wgradp<%d,%d,%d> CH=%d nb=%d stage=%zu smem=%zu\n", CP, COUT, KC, CH, nb, stage, smem);
+  if (dbg) fprintf(stderr, "wgradp<%d,%d,%d> CH=%d T=%d nb=%d stage=%zu smem=%zu\n", CP, COUT, KC, CH, T, nb, stage, smem);
   constexpr int NW = 9 * CP * COUT + COUT;
   WgradpArgs a;
-  a.PW = g.PW; a.nchx = nchx; a.nb = nb; a.err = err; a.chunk = CH;
+  a.PW = g.PW; a.T = T; a.nb = nb; a.err = err; a.chunk = CH;
   a.nchunks = (int)((g.Q + g.PW + KC - 1) / KC);        // j = p + (kh - 1) * PW ranges over [0, Q + PW)
   const int grid = a.nchunks < kNumSMs ? a.nchunks : kNumSMs;
   if (!batch || batch->n >= kMaxReduceJobs || batch->used + (size_t)grid * NW > batch->cap_floats)
@@ -603,17 +622,22 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
 
 int wgradp(int cin, int cout, int N, int H, int W, const void* x, const void* dy, float* dw, float* db,
            int* err, WgradBatch* batch, cudaStream_t st) {
-#define SEEDRL_WP_CASE(CI, CO_)                                                                          \
-  if (cin == CI && cout == CO_) {                                                                        \
-    int rc = launch_wgradp<CI, CO_, 256>(N, H, W, x, dy, dw, db, err, batch, st);                        \
-    if (rc == kPlanesTryNext) rc = launch_wgradp<CI, CO_, 128>(N, H, W, x, dy, dw, db, err, batch, st);  \
-    if (rc == kPlanesTryNext) rc = launch_wgradp<CI, CO_, 64>(N, H, W, x, dy, dw, db, err, batch, st);   \
-    if (rc == kPlanesTryNext) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgradp: does not fit");     \
-    return rc;                                                                                           \
+  // KC = 256 positions for 16 -> 16 and 128 for 32 output channels: the chunks, and so each CTA's
+  // positions and their order, of the weight gradient this path has always computed, so the learner's
+  // results stay bit-identical to it.  A shorter chunk only where two stages of the halo'd tiles do
+  // not fit (very wide images).
+#define SEEDRL_WP_CASE(CI, CO_, KC0)                                                                        \
+  if (cin == CI && cout == CO_) {                                                                           \
+    int rc = kPlanesTryNext;                                                                                \
+    if constexpr (KC0 >= 256) rc = launch_wgradp<CI, CO_, 256>(N, H, W, x, dy, dw, db, err, batch, st);     \
+    if (rc == kPlanesTryNext) rc = launch_wgradp<CI, CO_, 128>(N, H, W, x, dy, dw, db, err, batch, st);     \
+    if (rc == kPlanesTryNext) rc = launch_wgradp<CI, CO_, 64>(N, H, W, x, dy, dw, db, err, batch, st);      \
+    if (rc == kPlanesTryNext) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgradp: does not fit");        \
+    return rc;                                                                                              \
   }
-  SEEDRL_WP_CASE(16, 16)
-  SEEDRL_WP_CASE(16, 32)
-  SEEDRL_WP_CASE(32, 32)
+  SEEDRL_WP_CASE(16, 16, 256)
+  SEEDRL_WP_CASE(16, 32, 128)
+  SEEDRL_WP_CASE(32, 32, 128)
 #undef SEEDRL_WP_CASE
   return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgradp: unsupported (cin,cout)");
 }
