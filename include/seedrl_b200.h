@@ -494,6 +494,23 @@ int seedrl_debug_sgemm(int ta, int tb, int M, int N, int K, const float* A, int 
                        const float* B, int ldb, float* C, int ldc, const float* bias,
                        const float* mask, int ldm, int relu, int accumulate, int a_relu,
                        seedrl_stream_t stream);
+/* One K x K / stride S 'valid' convolution of the R2D2 body / shallow net (csrc/r2d2_net.cu), making
+ * exactly the calls the networks make for one layer: conv_gather_setup + a gathered gemm_tc, or
+ * im2col_nhwc + gemm_tc / sgemm; colsum for the bias gradient; gemm_tc(tb) / sgemm + col2im_nhwc for the
+ * data gradient.  x: [N,H,W,C] uint8 (in_u8, scaled by 1/255) or fp32; w: HWIO [K,K,C,cout].
+ *   op 0: out[M, ldo] = relu(im2col(x) w + bias), M = N * Ho * Wo (columns past cout untouched);
+ *   op 1: out[K*K*C, ldo] = im2col(x)^T dy, dbias[cout] = column sums of dy [M, cout];
+ *   op 2: out[N,H,W,C] = col2im(dy w^T) * (mask > 0) (C % 4 == 0, 16-byte aligned buffers).
+ * mode: 0 fp32 SIMT sgemm, 1 bf16 gemm_tc, 2 bf16x3 gemm_tc (a GEMM gemm_tc does not take runs on
+ * sgemm, as in the networks).  gather != 0 gathers the im2col operand where conv_gather_setup allows
+ * it (ops 0 and 1); otherwise it is materialised in col (col_bytes >= M*K*K*C*4; op 2 always uses it).
+ * ws: split-K / colsum scratch (gemm_tc_workspace_bytes: 48 MiB).  *gathered (may be NULL) = 1 if the
+ * operand was gathered. */
+int seedrl_debug_strided_conv(int op, int mode, int gather, int in_u8, int N, int H, int W, int C, int K,
+                              int S, int cout, const void* x, const float* w, const float* bias,
+                              const float* dy, const float* mask, float* out, int ldo, float* dbias,
+                              float* col, size_t col_bytes, float* ws, size_t ws_bytes, int* error_flag,
+                              int* gathered, seedrl_stream_t stream);
 
 /* ---- plane-tensor convolution path (conv_mode 3) test hooks: single kernels of
  * csrc/conv_planes.cu, so the GPU parity tests can localise a failure.  Not on the product path. */

@@ -178,6 +178,9 @@ SIGNATURES = {
     'seedrl_debug_sgemm':
         (c_int, [c_int, c_int, c_int, c_int, c_int, P, c_int, P, c_int, P, c_int, P, P, c_int,
                  c_int, c_int, c_int, P]),
+    'seedrl_debug_strided_conv':
+        (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P,
+                 c_int, P, P, c_size_t, P, c_size_t, P, ctypes.POINTER(c_int), P]),
 }
 
 _lib = None

@@ -117,13 +117,23 @@ int sgemm(bool ta, bool tb, int M, int N, int K, const float* A, int lda, const 
     SEEDRL_CHECK_LAUNCH();
     return SEEDRL_OK;
   }
-  dim3 grid(ceil_div(N, 64), ceil_div(M, 64));
-  if (!ta && !tb) sgemm_kernel<false, false><<<grid, 256, 0, st>>>(M, N, K, A, lda, B, ldb, C, ldc, e);
-  else if (ta && !tb) sgemm_kernel<true, false><<<grid, 256, 0, st>>>(M, N, K, A, lda, B, ldb, C, ldc, e);
-  else if (!ta && tb) sgemm_kernel<false, true><<<grid, 256, 0, st>>>(M, N, K, A, lda, B, ldb, C, ldc, e);
-  else sgemm_kernel<true, true><<<grid, 256, 0, st>>>(M, N, K, A, lda, B, ldb, C, ldc, e);
-  count_launch(PC_GEMM, st);
-  SEEDRL_CHECK_LAUNCH();
+  // grid.y is capped at 65535 tiles of 64 rows: taller products (the im2col convolutions past 4.19 M output
+  // positions) run as several launches over row slabs
+  constexpr int kRowsPerLaunch = 65535 * 64;
+  for (int r0 = 0; r0 < M; r0 += kRowsPerLaunch) {
+    const int m = M - r0 < kRowsPerLaunch ? M - r0 : kRowsPerLaunch;
+    const float* Ar = ta ? A + r0 : A + (size_t)r0 * lda;
+    float* Cr = C + (size_t)r0 * ldc;
+    GemmEpi er = e;
+    if (e.mask) er.mask = e.mask + (size_t)r0 * e.ldm;
+    dim3 grid(ceil_div(N, 64), ceil_div(m, 64));
+    if (!ta && !tb) sgemm_kernel<false, false><<<grid, 256, 0, st>>>(m, N, K, Ar, lda, B, ldb, Cr, ldc, er);
+    else if (ta && !tb) sgemm_kernel<true, false><<<grid, 256, 0, st>>>(m, N, K, Ar, lda, B, ldb, Cr, ldc, er);
+    else if (!ta && tb) sgemm_kernel<false, true><<<grid, 256, 0, st>>>(m, N, K, Ar, lda, B, ldb, Cr, ldc, er);
+    else sgemm_kernel<true, true><<<grid, 256, 0, st>>>(m, N, K, Ar, lda, B, ldb, Cr, ldc, er);
+    count_launch(PC_GEMM, st);
+    SEEDRL_CHECK_LAUNCH();
+  }
   return SEEDRL_OK;
 }
 

@@ -142,10 +142,13 @@ static int r_gemm(const seedrl_r2d2_net* n, void* ws, const RPlan& pl, bool ta, 
 // Tensor-core modes read the im2col matrix of a convolution straight from its NHWC input while the
 // GEMM stages its A blocks (kernels.h ConvGather): nothing is materialised for the forward or the
 // weight gradient.  False: geometry without aligned 8-element groups, SIMT mode, or switched off.
-static bool conv_gathered(const seedrl_r2d2_net* n, int N, const RConv& c, bool u8, const void* x, ConvGather* cg) {
+static bool strided_gathered(int mode, bool on, int N, const RConv& c, bool u8, const void* x, ConvGather* cg) {
   const int K = c.k * c.k * c.cin, M = N * c.hout * c.wout;
-  return n->mode >= 1 && gemm_tc_gather_enabled() && gemm_tc_supported(M, c.cout, K) &&
-         gemm_tc_supported(K, c.cout, M) && conv_gather_setup(x, u8 ? 1 : 0, N, c.hin, c.win, c.cin, c.k, c.s, cg);
+  return mode >= 1 && on && gemm_tc_supported(M, c.cout, K) && gemm_tc_supported(K, c.cout, M) &&
+         conv_gather_setup(x, u8 ? 1 : 0, N, c.hin, c.win, c.cin, c.k, c.s, cg);
+}
+static bool conv_gathered(const seedrl_r2d2_net* n, int N, const RConv& c, bool u8, const void* x, ConvGather* cg) {
+  return strided_gathered(n->mode, gemm_tc_gather_enabled(), N, c, u8, x, cg);
 }
 static int r_gemm_gather(const seedrl_r2d2_net* n, void* ws, const RPlan& pl, bool ta, int M, int N, int K,
                          const ConvGather& cg, const float* B, int ldb, float* C, int ldc, const GemmEpi& e,
@@ -205,7 +208,9 @@ int col2im_nhwc(int N, int H, int W, int C, int K, int S, const float* dcol, con
 }
 
 static int im2col(int N, const RConv& c, bool u8, const void* x, float* col, cudaStream_t st) {
-  const int vec = (c.cin % 4 == 0) ? 4 : 1;
+  // 4-channel vectors need uchar4 / float4-aligned input and float4-aligned columns
+  const uintptr_t xa = reinterpret_cast<uintptr_t>(x), ca = reinterpret_cast<uintptr_t>(col);
+  const int vec = (c.cin % 4 == 0 && (xa & (u8 ? 3 : 15)) == 0 && (ca & 15) == 0) ? 4 : 1;
   const long long total = (long long)N * c.hout * c.wout * c.k * c.k * (c.cin / vec);
   const unsigned grid = (unsigned)((total + 255) / 256);
 #define SEEDRL_I2C(U8_, V_) \
@@ -553,6 +558,59 @@ extern "C" int seedrl_r2d2_net_backward(const seedrl_r2d2_net* n, const float* p
     }
   }
   return SEEDRL_OK;
+}
+
+// One 'valid' strided convolution of the R2D2 body / shallow net through the calls the network makes
+// for a layer: conv_gather_setup + gathered gemm_tc, or im2col + gemm_tc / sgemm (r_gemm's choice);
+// colsum for the bias gradient; gemm_tc(tb) / sgemm + col2im for the data gradient.
+extern "C" int seedrl_debug_strided_conv(int op, int mode, int gather, int in_u8, int N, int H, int W, int C, int K,
+                                         int S, int cout, const void* x, const float* w, const float* bias,
+                                         const float* dy, const float* mask, float* out, int ldo, float* dbias,
+                                         float* col, size_t col_bytes, float* ws, size_t ws_bytes, int* error_flag,
+                                         int* gathered, seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(op >= 0 && op <= 2 && mode >= 0 && mode <= 2, "op and mode must be in 0..2");
+  SEEDRL_CHECK_ARG(N >= 1 && C >= 1 && K >= 1 && S >= 1 && H >= K && W >= K && cout >= 1, "bad shape");
+  SEEDRL_CHECK_ARG(w && out && (op == 2 || ldo >= cout), "null output / weights or ldo < cout");
+  RConv c;
+  c.k = K; c.s = S; c.cin = C; c.cout = cout; c.hin = H; c.win = W; c.hout = (H - K) / S + 1; c.wout = (W - K) / S + 1;
+  c.w = c.b = 0;
+  const long long Ml = (long long)N * c.hout * c.wout;
+  SEEDRL_CHECK_ARG(Ml * (K * K * C > cout ? K * K * C : cout) < (1ll << 31), "problem too large");
+  const int M = (int)Ml, KC = K * K * C;
+  const bool col_ok = col && col_bytes >= (size_t)M * KC * sizeof(float);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (gathered) *gathered = 0;
+  auto gemm = [&](bool ta, bool tb, int m, int n, int k, const float* A, int lda, const float* B, int ldb, float* Cm,
+                  int ldc, const GemmEpi& e) {
+    if (mode >= 1 && gemm_tc_supported(m, n, k))
+      return gemm_tc(ta, tb, mode >= 2, m, n, k, A, lda, B, ldb, Cm, ldc, e, ws, ws_bytes, error_flag, st);
+    return sgemm(ta, tb, m, n, k, A, lda, B, ldb, Cm, ldc, e, st);
+  };
+  ConvGather cg;
+  if (op == 0 || op == 1) {
+    SEEDRL_CHECK_ARG(x && (op == 0 || (dy && dbias)), "null pointer");
+    const bool g = strided_gathered(mode, gather != 0, N, c, in_u8 != 0, x, &cg);
+    if (gathered) *gathered = g ? 1 : 0;
+    GemmEpi e = epi_none();
+    if (op == 0) { e.bias = bias; e.relu = 1; }
+    if (g) {
+      SEEDRL_TRY(op == 0 ? gemm_tc(false, false, mode >= 2, M, cout, KC, nullptr, 0, w, cout, out, ldo, e, ws,
+                                   ws_bytes, error_flag, st, &cg)
+                         : gemm_tc(true, false, mode >= 2, KC, cout, M, nullptr, 0, dy, cout, out, ldo, e, ws,
+                                   ws_bytes, error_flag, st, &cg));
+    } else {
+      SEEDRL_CHECK_ARG(col_ok, "column scratch too small");
+      SEEDRL_TRY(im2col(N, c, in_u8 != 0, x, col, st));
+      SEEDRL_TRY(op == 0 ? gemm(false, false, M, cout, KC, col, KC, w, cout, out, ldo, e)
+                         : gemm(true, false, KC, cout, M, col, KC, dy, cout, out, ldo, e));
+    }
+    return op == 0 ? SEEDRL_OK : colsum(M, cout, dy, cout, dbias, st, ws, ws_bytes);
+  }
+  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  SEEDRL_CHECK_ARG(dy && mask && col_ok && C % 4 == 0 && al16(col) && al16(mask) && al16(out),
+                   "data gradient: null pointer, column scratch too small, C % 4 != 0 or unaligned buffers");
+  SEEDRL_TRY(gemm(false, true, M, KC, cout, dy, cout, w, cout, col, KC, epi_none()));
+  return col2im(N, c, col, mask, out, st);
 }
 
 extern "C" int seedrl_r2d2_net_check_error(const seedrl_r2d2_net* n, int T, int B, void* ws, size_t ws_bytes,
