@@ -19,7 +19,11 @@ inline int set_error(int code, const std::string& msg) {
   return code;
 }
 
-
+#define SEEDRL_TRY(expr)                \
+  do {                                  \
+    const int rc__ = (expr);            \
+    if (rc__ != SEEDRL_OK) return rc__; \
+  } while (0)
 
 #define SEEDRL_CHECK_ARG(cond, msg)                                         \
   do {                                                                      \

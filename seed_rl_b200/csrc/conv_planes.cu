@@ -371,7 +371,7 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
   if (nb < 2) return kPlanesTryNext;
   const size_t smem = nb * stage + fixed;
   CUtensorMap tm;
-  SEEDRL_TRY_RC(make_plane_map(&tm, c.in, Lp, 2 * (CIN / 8), 0, CH, nch, 2 * (CIN / 8)));
+  SEEDRL_TRY(make_plane_map(&tm, c.in, Lp, 2 * (CIN / 8), 0, CH, nch, 2 * (CIN / 8)));
   static bool attr = false;
   if (!attr) {
     SEEDRL_CUDA(cudaFuncSetAttribute(convp_kernel<CIN, COUT, NSUB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -592,10 +592,10 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
   if (nb < 2) return kPlanesTryNext;
   const size_t smem = 128 + nb * stage;
   WgradMaps tm;
-  SEEDRL_TRY_RC(make_plane_map(&tm.x, x, Lp, 2 * G, g.PW, CH, KC / CH, 1));
-  SEEDRL_TRY_RC(make_plane_map(&tm.x_halo, x, Lp, 2 * G, g.PW, kWpHaloRow, 1, 1));
-  SEEDRL_TRY_RC(make_plane_map(&tm.dy, dy, Lp, 2 * GO, 1, CH, KC / CH, 1));
-  SEEDRL_TRY_RC(make_plane_map(&tm.dy_halo, dy, Lp, 2 * GO, 1, kWpHaloRow, T / kWpHaloRow, 1));
+  SEEDRL_TRY(make_plane_map(&tm.x, x, Lp, 2 * G, g.PW, CH, KC / CH, 1));
+  SEEDRL_TRY(make_plane_map(&tm.x_halo, x, Lp, 2 * G, g.PW, kWpHaloRow, 1, 1));
+  SEEDRL_TRY(make_plane_map(&tm.dy, dy, Lp, 2 * GO, 1, CH, KC / CH, 1));
+  SEEDRL_TRY(make_plane_map(&tm.dy_halo, dy, Lp, 2 * GO, 1, kWpHaloRow, T / kWpHaloRow, 1));
   static bool attr = false;
   if (!attr) {
     SEEDRL_CUDA(cudaFuncSetAttribute(wgradp_kernel<CP, COUT, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -91,11 +91,6 @@ int conv3x3_tc_forward(int cin, int cout, int in_mode, int split, int N, int H, 
 // conv_planes.cu ("planes" path: activations stored in HBM as bf16 hi/lo channel-group planes of
 // the padded tall image = the wgmma operand format; TMA-fed, warp-specialised kernels)
 constexpr int kPlanesTryNext = -12347;
-#define SEEDRL_TRY_RC(expr)             \
-  do {                                  \
-    const int rc__ = (expr);            \
-    if (rc__ != SEEDRL_OK) return rc__; \
-  } while (0)
 long long planes_positions(int N, int H, int W);          // storage positions per plane (Lp)
 size_t planes_bytes(int N, int H, int W, int C);          // 2 * C/8 planes x Lp x 16 B
 struct PlaneConv {
@@ -160,10 +155,8 @@ int convgen_wgrad(int N, int H, int W, int cin, int cout, int k, int stride, int
                   const void* x, const float* dy, float* dw, float* db, float* partial,
                   size_t partial_bytes, cudaStream_t st);
 
-// r2d2_net.cu: 'valid' strided convolutions as im2col + GEMM (R2D2 body, shallow IMPALA net)
-int im2col_nhwc(int N, int H, int W, int C, int K, int S, int in_u8, const void* x, float* col, cudaStream_t st);
-int col2im_nhwc(int N, int H, int W, int C, int K, int S, const float* dcol, const float* xmask, float* dx,
-                cudaStream_t st);
+// strided_conv.cu: 'valid' strided convolutions as im2col + GEMM (R2D2 body, shallow IMPALA net) are
+// schedule.h's StridedConv
 
 // gemm_kernels.cu
 struct GemmEpi {

@@ -8,24 +8,11 @@
 // (_baseline, _conv_to_linear, _core, _policy_logits, _stacks...), Keras layouts,
 // every tensor start aligned to 64 floats (256 B), then the scalar entropy_cost_param
 // (learner.py:225-234).
-#include <string.h>
-
-#include <vector>
-
-#include "kernels.h"
+#include "schedule.h"
 
 namespace seedrl {
 
 constexpr int kHidden = 256;   // LSTMCell(256), Dense(256)
-constexpr size_t kAlignFloats = 64;
-
-struct ParamInfo {
-  std::string name;
-  int rank;
-  int64_t dims[4];
-  size_t offset;   // floats
-  size_t size;     // floats
-};
 
 struct ConvLayer {
   int cin, cout;
@@ -40,13 +27,12 @@ struct Stack {
 
 struct seedrl_net {
   seedrl_net_config cfg;
-  std::vector<seedrl::ParamInfo> params;   // network tensors, then entropy_cost_param
-  size_t arena_floats;
+  seedrl::ParamTable params;               // network tensors, then entropy_cost_param
   size_t logical_params;
   int p_base_w, p_base_b, p_dense_w, p_dense_b, p_core_w, p_core_u, p_core_b, p_pol_w, p_pol_b;
   std::vector<seedrl::Stack> stacks;       // deep
-  int sh_c0w, sh_c0b, sh_c1w, sh_c1b;      // shallow
-  int sh_h1, sh_w1, sh_h2, sh_w2;
+  seedrl::StridedConv sh[2];               // shallow: conv 8x8/4 -> 16, conv 4x4/2 -> 32
+  int sh_w[2], sh_b[2];                    // their param indices
   int flat;                                // conv features fed to Dense(256)
   int lstm_mode = 2;                       // 2 = tiled persistent kernels (lstm_tiled.cu), 1 = first persistent form, 0 = per-step launches
   int conv_mode = 0;                       // 0 = fp32 SIMT, 1 = wgmma bf16, 2 = wgmma bf16x3 (fp32-faithful)
@@ -55,39 +41,15 @@ struct seedrl_net {
 
 namespace seedrl {
 
-static int add_param(seedrl_net* n, const std::string& name, std::initializer_list<int64_t> dims) {
-  ParamInfo p;
-  p.name = name;
-  p.rank = (int)dims.size();
-  size_t sz = 1;
-  int i = 0;
-  for (int64_t d : dims) { p.dims[i++] = d; sz *= (size_t)d; }
-  for (; i < 4; ++i) p.dims[i] = 1;
-  p.size = sz;
-  p.offset = n->arena_floats;
-  n->arena_floats += (sz + kAlignFloats - 1) / kAlignFloats * kAlignFloats;
-  n->params.push_back(p);
-  return (int)n->params.size() - 1;
-}
-
 static ConvLayer add_conv(seedrl_net* n, const std::string& prefix, int k, int cin, int cout) {
   ConvLayer l;
   l.cin = cin; l.cout = cout;
-  l.w = add_param(n, prefix + "/kernel", {k, k, cin, cout});
-  l.b = add_param(n, prefix + "/bias", {cout});
+  l.w = n->params.add(prefix + "/kernel", {k, k, cin, cout});
+  l.b = n->params.add(prefix + "/bias", {cout});
   return l;
 }
 
 // ---- workspace plan -----------------------------------------------------------
-struct Bump {
-  size_t off = 0;
-  size_t take(size_t bytes) {
-    const size_t o = off;
-    off += (bytes + 255) / 256 * 256;
-    return o;
-  }
-};
-
 struct StackBufs {
   size_t a0, p, idx, c0, o0, c1, o1;
   // conv_mode 3 (plane tensors, conv_planes.cu): raw / ReLU'd pooled activation, ReLU'd c0 / c1,
@@ -150,13 +112,14 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
     }
     p.sh_a1 = p.sh_a2 = 0;
   } else {
-    const size_t a1 = N * n->sh_h1 * n->sh_w1 * 16, a2 = N * n->sh_h2 * n->sh_w2 * 32;
+    const StridedConv &l0 = n->sh[0], &l1 = n->sh[1];
+    const size_t a1 = N * l0.hout * l0.wout * l0.cout, a2 = N * l1.hout * l1.wout * l1.cout;
     p.sh_a1 = b.take(a1 * 4);
     p.sh_a2 = b.take(a2 * 4);
     p.sh_col0 = p.sh_col1 = 0;
     if (n->conv_mode >= 1) {
-      p.sh_col0 = b.take(N * n->sh_h1 * n->sh_w1 * (size_t)(64 * n->cfg.obs_c) * 4);
-      p.sh_col1 = b.take(N * n->sh_h2 * n->sh_w2 * (size_t)(16 * 16) * 4);
+      p.sh_col0 = b.take(N * l0.hout * l0.wout * (size_t)(l0.k * l0.k * l0.cin) * 4);
+      p.sh_col1 = b.take(N * l1.hout * l1.wout * (size_t)(l1.k * l1.k * l1.cin) * 4);
     }
     pooled_max = a1 > a2 ? a1 : a2;
     full_max = 0;
@@ -203,28 +166,34 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
   return p;
 }
 
-#define SEEDRL_TRY(expr)              \
-  do {                                \
-    const int rc__ = (expr);          \
-    if (rc__ != SEEDRL_OK) return rc__; \
-  } while (0)
+// State of one forward or backward call, passed down the schedule: the GEMM execution, the weights
+// pre-packed for this call, the deferred weight-gradient reductions, the head-ready event, and for
+// 3-channel frames the zero-padded first-conv weights and their gradient (pad_first_layer), which
+// stand in for that one parameter in P() / G().
+struct Call {
+  const seedrl_net* n;
+  const Plan& pl;
+  const float* prm;
+  float* grd;                        // backward only
+  void* ws;
+  GemmExec ex;
+  PackTable packed;
+  WgradBatch wb;
+  cudaEvent_t head_ready = nullptr;  // recorded when the gradients of the first arena bucket are final
+  int w0_index = -1;
+  const float* w0_pad = nullptr;
+  float* dw0_pad = nullptr;
 
-// 3-channel frames (DMLab's 72x96x3, dmlab/env.py:44-54): the first convolution's kernels are built
-// for 4 input channels, so a forward/backward call works on a zero-padded copy of the frames and of
-// the first conv's weights ([3,3,3,16] -> [3,3,4,16]); its weight gradient is computed in the padded
-// shape and copied back without the 4th channel.  These thread-local overrides redirect the one
-// parameter for the duration of a call.
-static thread_local int t_w0_index = -1;
-static thread_local const float* t_w0_pad = nullptr;
-static thread_local float* t_dw0_pad = nullptr;
-static inline const float* P(const seedrl_net* n, const float* arena, int idx) {
-  if (idx == t_w0_index && t_w0_pad) return t_w0_pad;
-  return arena + n->params[idx].offset;
-}
-static inline float* G(const seedrl_net* n, float* arena, int idx) {
-  if (idx == t_w0_index && t_dw0_pad) return t_dw0_pad;
-  return arena + n->params[idx].offset;
-}
+  Call(const seedrl_net* n_, const Plan& pl_, const float* prm_, float* grd_, void* ws_, cudaStream_t st)
+      : n(n_), pl(pl_), prm(prm_), grd(grd_), ws(ws_),
+        ex{n_->conv_mode >= 2 ? 2 : n_->conv_mode, gemm_tc_gather_enabled(), W<float>(ws_, pl_.gemm_ws),
+           gemm_tc_workspace_bytes(), W<int>(ws_, pl_.tcerr), st},
+        wb{nullptr, 0, 0, 0, {}} {
+    packed.n = 0;
+  }
+  const float* P(int idx) const { return idx == w0_index && w0_pad ? w0_pad : prm + n->params.offset(idx); }
+  float* G(int idx) const { return idx == w0_index && dw0_pad ? dw0_pad : grd + n->params.offset(idx); }
+};
 
 __global__ void pad_frames3_kernel(size_t npix, const uint8_t* __restrict__ src, uchar4* __restrict__ dst) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -244,36 +213,12 @@ __global__ void unpad_dw0_kernel(int cout, const float* __restrict__ dwp, float*
   const int co = i % cout, ci = (i / cout) % 3, tap = i / (3 * cout);
   dw[i] = dwp[(tap * 4 + ci) * cout + co];
 }
-template <typename T>
-static inline T* W(void* ws, size_t off) {
-  return reinterpret_cast<T*>(reinterpret_cast<char*>(ws) + off);
-}
 
-// One dense contraction of the schedule: wgmma when the net runs in tensor-core mode and the
-// shape is worth a 128-row tile, else the fp32 SIMT kernel.
-static int run_gemm(const seedrl_net* n, void* ws, const Plan& pl, bool ta, bool tb, int M, int N, int K,
-                    const float* A, int lda, const float* B, int ldb, float* C, int ldc, const GemmEpi& e,
-                    cudaStream_t st) {
-  if (n->conv_mode >= 1 && gemm_tc_supported(M, N, K))
-    return gemm_tc(ta, tb, n->conv_mode >= 2, M, N, K, A, lda, B, ldb, C, ldc, e, W<float>(ws, pl.gemm_ws),
-                   gemm_tc_workspace_bytes(), W<int>(ws, pl.tcerr), st);
-  return sgemm(ta, tb, M, N, K, A, lda, B, ldb, C, ldc, e, st);
-}
-
-// Per-call context of the tensor-core path (thread-local: forward/backward of different nets
-// may run on different host threads): where the pre-packed weights of this call live and the
-// deferred weight-gradient reductions.
-struct StepCtx {
-  PackTable packed;
-  WgradBatch wb;
-};
-static thread_local StepCtx* t_ctx = nullptr;
-static thread_local void* t_head_ready = nullptr;   // cudaEvent_t recorded by seedrl_net_backward_overlap
 // test hook: 1 = keep the dense (pool backward + full-resolution weight gradient) first-layer path
 static int g_first_dense = 0;
 
 // Channels of the frames the deep net's first layer reads: 3-channel frames run on their zero-padded
-// 4-channel copy (PadScope); every other count (1..16) is read as it is, zero-filled in shared memory.
+// 4-channel copy (pad_first_layer); every other count (1..16) is read as it is, zero-filled in shared memory.
 static inline int first_c(const seedrl_net* n) { return n->cfg.obs_c == 3 ? 4 : n->cfg.obs_c; }
 // frames that only the channel-generic first-layer kernels take (conv modes 0 and 3)
 static inline bool generic_first(const seedrl_net* n) {
@@ -282,11 +227,11 @@ static inline bool generic_first(const seedrl_net* n) {
 
 // Packs the weights of every conv of the deep torso with one launch: forward forms, or the
 // flipped/transposed forms of the data-gradient convolutions (all but the first layer).
-static int pack_all_weights(const seedrl_net* n, const float* prm, void* ws, const Plan& pl, int flip,
-                            StepCtx* ctx, cudaStream_t st) {
-  ctx->packed.n = 0;
+static int pack_all_weights(Call& c, int flip) {
+  const seedrl_net* n = c.n;
+  c.packed.n = 0;
   if (n->conv_mode < 1 || n->cfg.net != SEEDRL_NET_DEEP) return SEEDRL_OK;
-  char* base = W<char>(ws, pl.wq_all);
+  char* base = W<char>(c.ws, c.pl.wq_all);
   for (size_t s = 0; s < n->stacks.size(); ++s) {
     const Stack& k = n->stacks[s];
     const ConvLayer* ls[5] = {&k.conv, &k.r00, &k.r01, &k.r10, &k.r11};
@@ -295,71 +240,71 @@ static int pack_all_weights(const seedrl_net* n, const float* prm, void* ws, con
       if (flip && s == 0 && i == 0) continue;          // no data gradient into the frames
       if (s == 0 && i == 0 && generic_first(n)) continue;   // conv0pool packs its own [3,3,C,16] weights
       const int cin = flip ? l.cout : l.cin, cout = flip ? l.cin : l.cout;
-      if (ctx->packed.n >= kMaxPackJobs) return SEEDRL_OK;
+      if (c.packed.n >= kMaxPackJobs) return SEEDRL_OK;
       PackJob j;
-      j.w = P(n, prm, l.w);
-      j.wq = base + (size_t)ctx->packed.n * kPackSlotBytes;
+      j.w = c.P(l.w);
+      j.wq = base + (size_t)c.packed.n * kPackSlotBytes;
       j.ck = cin < 16 ? 16 : cin; j.cout = cout; j.cin_src = cin; j.flip = flip;
       j.legacy = (s == 0 && i == 0) ? 1 : 0;           // the uint8 first conv runs the staged kernel
-      ctx->packed.jobs[ctx->packed.n++] = j;
+      c.packed.jobs[c.packed.n++] = j;
     }
   }
-  return conv3x3_tc_pack_weights_batch(ctx->packed, n->conv_mode == 3 ? 2 : (n->conv_mode >= 2 ? 1 : 0), st);
+  return conv3x3_tc_pack_weights_batch(c.packed, n->conv_mode == 3 ? 2 : (n->conv_mode >= 2 ? 1 : 0), c.ex.st);
 }
-static const void* find_packed(const float* w, int flip) {
-  if (!t_ctx) return nullptr;
-  for (int i = 0; i < t_ctx->packed.n; ++i)
-    if (t_ctx->packed.jobs[i].w == w && t_ctx->packed.jobs[i].flip == flip) return t_ctx->packed.jobs[i].wq;
-  return nullptr;
+// The packed form of `w` from this call's table, or packed into the single-layer scratch slot.
+static int packed_weights(const Call& c, int cin, int cout, const float* w, int flip, int split, const void** wq) {
+  for (int i = 0; i < c.packed.n; ++i)
+    if (c.packed.jobs[i].w == w && c.packed.jobs[i].flip == flip) {
+      *wq = c.packed.jobs[i].wq;
+      return SEEDRL_OK;
+    }
+  void* scratch = W<void>(c.ws, c.pl.wq);
+  SEEDRL_TRY(conv3x3_tc_pack_weights(cin, cout, flip, split, w, scratch, c.ex.st));
+  *wq = scratch;
+  return SEEDRL_OK;
 }
 
 // One 3x3 'same' convolution of the schedule.  flip != 0: data-gradient (weights flipped and
 // transposed; cin/cout are those of the *gradient* convolution).  Dispatches to the wgmma
 // kernel when the net runs in tensor-core mode and the shape is supported, else fp32 SIMT.
-static int run_conv(const seedrl_net* n, void* ws, const Plan& pl, int cin, int cout, int in_mode,
-                    int N, int H, int Wd, const void* in, const float* w, const float* bias,
-                    const float* mask, const float* res, float* out, int flip, cudaStream_t st) {
-  if (n->conv_mode >= 1 && conv3x3_tc_supported(cin, cout, in_mode)) {
-    const int split = n->conv_mode >= 2;
-    const void* wq = find_packed(w, flip);
-    if (!wq) {
-      void* scratch = W<void>(ws, pl.wq);
-      SEEDRL_TRY(conv3x3_tc_pack_weights(cin, cout, flip, split, w, scratch, st));
-      wq = scratch;
-    }
-    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, in, wq, bias, mask, res, out, 0,
-                              W<int>(ws, pl.tcerr), st);
+static int run_conv(const Call& c, int cin, int cout, int in_mode, int N, int H, int Wd, const void* in,
+                    const float* w, const float* bias, const float* mask, const float* res, float* out, int flip) {
+  cudaStream_t st = c.ex.st;
+  if (c.n->conv_mode >= 1 && conv3x3_tc_supported(cin, cout, in_mode)) {
+    const int split = c.n->conv_mode >= 2;
+    const void* wq;
+    SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, split, &wq));
+    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, in, wq, bias, mask, res, out, 0, c.ex.err, st);
   }
   if (flip) {
-    float* wt = W<float>(ws, pl.wt);
+    float* wt = W<float>(c.ws, c.pl.wt);
     SEEDRL_TRY(conv3x3_flip_weights(cout, cin, w, wt, st));   // source layout is [tap][cout][cin]
     return conv3x3_forward(cin, cout, in_mode, N, H, Wd, in, wt, bias, mask, res, out, st);
   }
   return conv3x3_forward(cin, cout, in_mode, N, H, Wd, in, w, bias, mask, res, out, st);
 }
 
-// Scope of one forward/backward call on 3-channel frames: builds the padded frames and first-conv
-// weights in the workspace and installs the parameter overrides; no-op for 4-channel frames.
-struct PadScope {
-  int rc = SEEDRL_OK;
-  bool active = false;
-  const uint8_t* obs;
-  PadScope(const seedrl_net* n, const float* prm, const Plan& pl, const uint8_t* observation, void* ws,
-           cudaStream_t st) : obs(observation) {
-    if (n->cfg.net != SEEDRL_NET_DEEP || n->cfg.obs_c != 3) return;
-    active = true;
-    const size_t npix = (size_t)pl.N * n->cfg.obs_h * n->cfg.obs_w;
-    pad_frames3_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(npix, observation, W<uchar4>(ws, pl.obs4));
-    count_launch(PC_MISC, st);
-    const int wi = n->stacks[0].conv.w;
-    pad_w0_kernel<<<ceil_div(9 * 4 * 16, 128), 128, 0, st>>>(16, prm + n->params[wi].offset, W<float>(ws, pl.w0pad));
-    count_launch(PC_MISC, st);
-    if (cudaGetLastError() != cudaSuccess) rc = set_error(SEEDRL_ERR_INTERNAL, "3-channel padding launch failed");
-    obs = W<uint8_t>(ws, pl.obs4);
-    t_w0_index = wi; t_w0_pad = W<float>(ws, pl.w0pad); t_dw0_pad = W<float>(ws, pl.dw0pad);
-  }
-  ~PadScope() { t_w0_index = -1; t_w0_pad = nullptr; t_dw0_pad = nullptr; }
-};
+// 3-channel frames (DMLab's 72x96x3, dmlab/env.py:44-54): the first convolution's kernels are built
+// for 4 input channels, so a forward/backward call works on a zero-padded copy of the frames and of
+// the first conv's weights ([3,3,3,16] -> [3,3,4,16]); its weight gradient is computed in the padded
+// shape and copied back without the 4th channel.  Builds both copies in the workspace, points *obs at
+// the padded frames and redirects the first conv's parameter of this call; no-op for other frames.
+static int pad_first_layer(Call& c, const uint8_t** obs) {
+  const seedrl_net* n = c.n;
+  if (n->cfg.net != SEEDRL_NET_DEEP || n->cfg.obs_c != 3) return SEEDRL_OK;
+  const Plan& pl = c.pl;
+  cudaStream_t st = c.ex.st;
+  const size_t npix = (size_t)pl.N * n->cfg.obs_h * n->cfg.obs_w;
+  pad_frames3_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(npix, *obs, W<uchar4>(c.ws, pl.obs4));
+  count_launch(PC_MISC, st);
+  const int wi = n->stacks[0].conv.w;
+  pad_w0_kernel<<<ceil_div(9 * 4 * 16, 128), 128, 0, st>>>(16, c.prm + n->params.offset(wi), W<float>(c.ws, pl.w0pad));
+  count_launch(PC_MISC, st);
+  if (cudaGetLastError() != cudaSuccess) return set_error(SEEDRL_ERR_INTERNAL, "3-channel padding launch failed");
+  *obs = W<uint8_t>(c.ws, pl.obs4);
+  c.w0_index = wi; c.w0_pad = W<float>(c.ws, pl.w0pad); c.dw0_pad = W<float>(c.ws, pl.dw0pad);
+  return SEEDRL_OK;
+}
 
 }  // namespace seedrl
 
@@ -371,12 +316,11 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
   SEEDRL_CHECK_ARG(cfg->num_actions >= 1 && cfg->obs_h > 0 && cfg->obs_w > 0, "bad shape");
   seedrl_net* n = new seedrl_net();
   n->cfg = *cfg;
-  n->arena_floats = 0;
   const int A = cfg->num_actions;
   n->core_in = kHidden + 1 + A;
   // tf.Module order: _baseline, _conv_to_linear, _core, _policy_logits, _stacks
-  n->p_base_w = add_param(n, "baseline/kernel", {kHidden, 1});
-  n->p_base_b = add_param(n, "baseline/bias", {1});
+  n->p_base_w = n->params.add("baseline/kernel", {kHidden, 1});
+  n->p_base_b = n->params.add("baseline/bias", {1});
   int flat = 0;
   if (cfg->net == SEEDRL_NET_DEEP) {
     if (cfg->obs_c < 1 || cfg->obs_c > 16) {
@@ -389,18 +333,18 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
     for (int s = 0; s < 3; ++s) { h = (h + 1) / 2; w = (w + 1) / 2; }
     flat = h * w * chans[2];
   } else {
-    n->sh_h1 = (cfg->obs_h - 8) / 4 + 1; n->sh_w1 = (cfg->obs_w - 8) / 4 + 1;
-    n->sh_h2 = (n->sh_h1 - 4) / 2 + 1;   n->sh_w2 = (n->sh_w1 - 4) / 2 + 1;
-    flat = n->sh_h2 * n->sh_w2 * 32;
+    n->sh[0] = StridedConv(8, 4, cfg->obs_c, 16, cfg->obs_h, cfg->obs_w);
+    n->sh[1] = StridedConv(4, 2, 16, 32, n->sh[0].hout, n->sh[0].wout);
+    flat = n->sh[1].hout * n->sh[1].wout * 32;
   }
   n->flat = flat;
-  n->p_dense_w = add_param(n, "conv_to_linear/kernel", {flat, kHidden});
-  n->p_dense_b = add_param(n, "conv_to_linear/bias", {kHidden});
-  n->p_core_w = add_param(n, "core/kernel", {n->core_in, 4 * kHidden});
-  n->p_core_u = add_param(n, "core/recurrent_kernel", {kHidden, 4 * kHidden});
-  n->p_core_b = add_param(n, "core/bias", {4 * kHidden});
-  n->p_pol_w = add_param(n, "policy_logits/kernel", {kHidden, A});
-  n->p_pol_b = add_param(n, "policy_logits/bias", {A});
+  n->p_dense_w = n->params.add("conv_to_linear/kernel", {flat, kHidden});
+  n->p_dense_b = n->params.add("conv_to_linear/bias", {kHidden});
+  n->p_core_w = n->params.add("core/kernel", {n->core_in, 4 * kHidden});
+  n->p_core_u = n->params.add("core/recurrent_kernel", {kHidden, 4 * kHidden});
+  n->p_core_b = n->params.add("core/bias", {4 * kHidden});
+  n->p_pol_w = n->params.add("policy_logits/kernel", {kHidden, A});
+  n->p_pol_b = n->params.add("policy_logits/bias", {A});
   if (cfg->net == SEEDRL_NET_DEEP) {
     int h = cfg->obs_h, w = cfg->obs_w, c = cfg->obs_c;
     const int chans[3] = {16, 32, 32};
@@ -421,23 +365,25 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
       h = st.hout; w = st.wout; c = st.c;
     }
   } else {
-    ConvLayer c0 = add_conv(n, "conv0", 8, cfg->obs_c, 16);
-    ConvLayer c1 = add_conv(n, "conv1", 4, 16, 32);
-    n->sh_c0w = c0.w; n->sh_c0b = c0.b; n->sh_c1w = c1.w; n->sh_c1b = c1.b;
+    for (int i = 0; i < 2; ++i) {
+      const StridedConv& l = n->sh[i];
+      const ConvLayer cl = add_conv(n, "conv" + std::to_string(i), l.k, l.cin, l.cout);
+      n->sh_w[i] = cl.w; n->sh_b[i] = cl.b;
+    }
   }
   n->logical_params = 0;
-  for (const ParamInfo& p : n->params) n->logical_params += p.size;
-  add_param(n, "entropy_cost_param", {});
+  for (const ParamInfo& p : n->params.list) n->logical_params += p.size;
+  n->params.add("entropy_cost_param", {});
   *out = n;
   return SEEDRL_OK;
 }
 
 extern "C" void seedrl_net_destroy(seedrl_net* net) { delete net; }
 extern "C" int seedrl_net_num_param_tensors(const seedrl_net* net) {
-  return net ? (int)net->params.size() - 1 : 0;
+  return net ? (int)net->params.list.size() - 1 : 0;
 }
 extern "C" size_t seedrl_net_num_params(const seedrl_net* net) { return net ? net->logical_params : 0; }
-extern "C" size_t seedrl_net_arena_floats(const seedrl_net* net) { return net ? net->arena_floats : 0; }
+extern "C" size_t seedrl_net_arena_floats(const seedrl_net* net) { return net ? net->params.arena_floats : 0; }
 extern "C" int seedrl_net_set_lstm_mode(seedrl_net* net, int mode) {
   SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 2, "mode must be 0 (per-step launches), 1 (persistent, CTA = 2 units) or 2 (persistent, CTA = batch tile x 16 units)");
   net->lstm_mode = mode;
@@ -458,15 +404,8 @@ extern "C" int seedrl_net_set_conv_mode(seedrl_net* net, int mode) {
 
 extern "C" int seedrl_net_param_info(const seedrl_net* net, int index, char* name_buf,
                                      size_t name_buf_len, int64_t* dims, size_t* offset) {
-  if (!net || index < 0 || index >= (int)net->params.size()) return -1;
-  const ParamInfo& p = net->params[index];
-  if (name_buf && name_buf_len) {
-    strncpy(name_buf, p.name.c_str(), name_buf_len - 1);
-    name_buf[name_buf_len - 1] = 0;
-  }
-  if (dims) for (int i = 0; i < 4; ++i) dims[i] = p.dims[i];
-  if (offset) *offset = p.offset;
-  return p.rank;
+  const ParamInfo* p = net ? net->params.info(index, name_buf, name_buf_len, dims, offset) : nullptr;
+  return p ? p->rank : -1;
 }
 
 extern "C" size_t seedrl_net_workspace_bytes(const seedrl_net* net, int T1, int B) {
@@ -475,8 +414,8 @@ extern "C" size_t seedrl_net_workspace_bytes(const seedrl_net* net, int T1, int 
 }
 
 // ---- forward --------------------------------------------------------------------
-static int torso_forward_deep(const seedrl_net* n, const float* prm, const Plan& pl,
-                              const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_forward_deep(const Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   const int N = pl.N;
   const void* in = obs;
   int in_mode = IN_U8;
@@ -488,20 +427,20 @@ static int torso_forward_deep(const seedrl_net* n, const float* prm, const Plan&
     float* c1 = W<float>(ws, b.c1); float* o1 = W<float>(ws, b.o1);
     // _Stack.__call__, dmlab/networks.py:46-60
     if (s == 0 && generic_first(n))
-      SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, P(n, prm, k.conv.w), P(n, prm, k.conv.b), a0,
+      SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, c.P(k.conv.w), c.P(k.conv.b), a0,
                                     st));
     else
-      SEEDRL_TRY(run_conv(n, ws, pl, k.cin, k.c, in_mode, N, k.hin, k.win, in, P(n, prm, k.conv.w),
-                          P(n, prm, k.conv.b), nullptr, nullptr, a0, 0, st));
+      SEEDRL_TRY(run_conv(c, k.cin, k.c, in_mode, N, k.hin, k.win, in, c.P(k.conv.w),
+                          c.P(k.conv.b), nullptr, nullptr, a0, 0));
     SEEDRL_TRY(maxpool3s2_forward(N, k.hin, k.win, k.c, a0, p, W<uint8_t>(ws, b.idx), st));
-    SEEDRL_TRY(run_conv(n, ws, pl, k.c, k.c, IN_RELU, N, k.hout, k.wout, p, P(n, prm, k.r00.w),
-                        P(n, prm, k.r00.b), nullptr, nullptr, c0, 0, st));
-    SEEDRL_TRY(run_conv(n, ws, pl, k.c, k.c, IN_RELU, N, k.hout, k.wout, c0, P(n, prm, k.r01.w),
-                        P(n, prm, k.r01.b), nullptr, p, o0, 0, st));
-    SEEDRL_TRY(run_conv(n, ws, pl, k.c, k.c, IN_RELU, N, k.hout, k.wout, o0, P(n, prm, k.r10.w),
-                        P(n, prm, k.r10.b), nullptr, nullptr, c1, 0, st));
-    SEEDRL_TRY(run_conv(n, ws, pl, k.c, k.c, IN_RELU, N, k.hout, k.wout, c1, P(n, prm, k.r11.w),
-                        P(n, prm, k.r11.b), nullptr, o0, o1, 0, st));
+    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, p, c.P(k.r00.w),
+                        c.P(k.r00.b), nullptr, nullptr, c0, 0));
+    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, c0, c.P(k.r01.w),
+                        c.P(k.r01.b), nullptr, p, o0, 0));
+    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, o0, c.P(k.r10.w),
+                        c.P(k.r10.b), nullptr, nullptr, c1, 0));
+    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, c1, c.P(k.r11.w),
+                        c.P(k.r11.b), nullptr, o0, o1, 0));
     in = o1;
     in_mode = IN_F32;
   }
@@ -511,23 +450,19 @@ static int torso_forward_deep(const seedrl_net* n, const float* prm, const Plan&
 // conv_mode 3: the same _Stack schedule on plane tensors (conv_planes.cu).  The first conv reads the
 // uint8 frames with the staged wgmma kernel (bf16x3) and writes fp32 NHWC for the max-pool; from
 // there on every conv input is a TMA tile of an HBM-resident operand.
-static int planes_conv(const seedrl_net* n, void* ws, const Plan& pl, int cin, int cout, int N, int H, int Wd,
-                       const void* in, const float* w, int flip, const float* bias, const void* mask,
-                       const void* res, void* out_raw, void* out_relu, float* out_nhwc, cudaStream_t st) {
-  const void* wq = find_packed(w, flip);
-  if (!wq) {
-    void* scratch = W<void>(ws, pl.wq);
-    SEEDRL_TRY(conv3x3_tc_pack_weights(cin, cout, flip, 2, w, scratch, st));
-    wq = scratch;
-  }
-  PlaneConv c;
-  c.N = N; c.H = H; c.W = Wd; c.in = in; c.wq = wq; c.bias = bias; c.mask = mask; c.res = res;
-  c.out_raw = out_raw; c.out_relu = out_relu; c.out_nhwc = out_nhwc; c.err = W<int>(ws, pl.tcerr);
-  return convp_forward(cin, cout, c, st);
+static int planes_conv(const Call& c, int cin, int cout, int N, int H, int Wd, const void* in, const float* w,
+                       int flip, const float* bias, const void* mask, const void* res, void* out_raw, void* out_relu,
+                       float* out_nhwc) {
+  const void* wq;
+  SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, 2, &wq));
+  PlaneConv pc;
+  pc.N = N; pc.H = H; pc.W = Wd; pc.in = in; pc.wq = wq; pc.bias = bias; pc.mask = mask; pc.res = res;
+  pc.out_raw = out_raw; pc.out_relu = out_relu; pc.out_nhwc = out_nhwc; pc.err = c.ex.err;
+  return convp_forward(cin, cout, pc, c.ex.st);
 }
 
-static int torso_forward_planes(const seedrl_net* n, const float* prm, const Plan& pl,
-                                const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_forward_planes(const Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   const int N = pl.N;
   const void* prev = nullptr;
   const size_t ns = n->stacks.size();
@@ -544,85 +479,51 @@ static int torso_forward_planes(const seedrl_net* n, const float* prm, const Pla
                        "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
     if (s == 0 && conv0pool_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
       // first conv + bias + max-pool in one kernel: the full-resolution activation never reaches HBM
-      SEEDRL_TRY(conv0pool_forward(N, k.hin, k.win, first_c(n), obs, P(n, prm, k.conv.w), P(n, prm, k.conv.b), praw,
+      SEEDRL_TRY(conv0pool_forward(N, k.hin, k.win, first_c(n), obs, c.P(k.conv.w), c.P(k.conv.b), praw,
                                    prelu, W<uint8_t>(ws, b.idx), W<int>(ws, pl.tcerr), st));
     } else if (s == 0 && generic_first(n)) {
       return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv mode 3: the fused first layer takes frames up to 107 pixels wide");
     } else {
       if (s == 0)
-        SEEDRL_TRY(run_conv(n, ws, pl, k.cin, k.c, IN_U8, N, k.hin, k.win, obs, P(n, prm, k.conv.w),
-                            P(n, prm, k.conv.b), nullptr, nullptr, a0, 0, st));
+        SEEDRL_TRY(run_conv(c, k.cin, k.c, IN_U8, N, k.hin, k.win, obs, c.P(k.conv.w),
+                            c.P(k.conv.b), nullptr, nullptr, a0, 0));
       else
-        SEEDRL_TRY(planes_conv(n, ws, pl, k.cin, k.c, N, k.hin, k.win, prev, P(n, prm, k.conv.w), 0,
-                               P(n, prm, k.conv.b), nullptr, nullptr, nullptr, nullptr, a0, st));
+        SEEDRL_TRY(planes_conv(c, k.cin, k.c, N, k.hin, k.win, prev, c.P(k.conv.w), 0,
+                               c.P(k.conv.b), nullptr, nullptr, nullptr, nullptr, a0));
       SEEDRL_TRY(poolp_forward(N, k.hin, k.win, k.c, a0, praw, prelu, W<uint8_t>(ws, b.idx), st));
     }
     const int H = k.hout, Wd = k.wout, C = k.c;
     // res block 0: c0 = conv00(relu(p)); o0 = conv01(relu(c0)) + p        (networks.py:52-58)
-    SEEDRL_TRY(planes_conv(n, ws, pl, C, C, N, H, Wd, prelu, P(n, prm, k.r00.w), 0, P(n, prm, k.r00.b), nullptr,
-                           nullptr, nullptr, c0r, nullptr, st));
-    SEEDRL_TRY(planes_conv(n, ws, pl, C, C, N, H, Wd, c0r, P(n, prm, k.r01.w), 0, P(n, prm, k.r01.b), nullptr,
-                           praw, o0raw, o0relu, nullptr, st));
+    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, prelu, c.P(k.r00.w), 0, c.P(k.r00.b), nullptr,
+                           nullptr, nullptr, c0r, nullptr));
+    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, c0r, c.P(k.r01.w), 0, c.P(k.r01.b), nullptr,
+                           praw, o0raw, o0relu, nullptr));
     // res block 1: c1 = conv10(relu(o0)); o1 = conv11(relu(c1)) + o0
-    SEEDRL_TRY(planes_conv(n, ws, pl, C, C, N, H, Wd, o0relu, P(n, prm, k.r10.w), 0, P(n, prm, k.r10.b), nullptr,
-                           nullptr, nullptr, c1r, nullptr, st));
-    SEEDRL_TRY(planes_conv(n, ws, pl, C, C, N, H, Wd, c1r, P(n, prm, k.r11.w), 0, P(n, prm, k.r11.b), nullptr,
+    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, o0relu, c.P(k.r10.w), 0, c.P(k.r10.b), nullptr,
+                           nullptr, nullptr, c1r, nullptr));
+    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, c1r, c.P(k.r11.w), 0, c.P(k.r11.b), nullptr,
                            o0raw, last ? nullptr : W<void>(ws, b.o1p), nullptr,
-                           last ? W<float>(ws, b.o1) : nullptr, st));
+                           last ? W<float>(ws, b.o1) : nullptr));
     prev = W<void>(ws, b.o1p);
   }
   return SEEDRL_OK;
 }
 
-// Shallow net, tensor-core modes: layer 0 = conv 8x8/4 on the uint8 frames, layer 1 = conv 4x4/2 on a1.
-static bool shallow_gathered(const seedrl_net* n, int layer, int N, const void* x, ConvGather* cg) {
-  if (n->conv_mode < 1 || !gemm_tc_gather_enabled()) return false;
-  if (layer == 0)
-    return gemm_tc_supported(N * n->sh_h1 * n->sh_w1, 16, 64 * n->cfg.obs_c) &&
-           conv_gather_setup(x, 1, N, n->cfg.obs_h, n->cfg.obs_w, n->cfg.obs_c, 8, 4, cg);
-  return gemm_tc_supported(N * n->sh_h2 * n->sh_w2, 32, 256) && conv_gather_setup(x, 0, N, n->sh_h1, n->sh_w1, 16, 4, 2, cg);
-}
-static int run_gemm_gather(const seedrl_net* n, void* ws, const Plan& pl, bool ta, int M, int N, int K,
-                           const ConvGather& cg, const float* B, int ldb, float* C, int ldc, const GemmEpi& e,
-                           cudaStream_t st) {
-  return gemm_tc(ta, false, n->conv_mode >= 2, M, N, K, nullptr, 0, B, ldb, C, ldc, e, W<float>(ws, pl.gemm_ws),
-                 gemm_tc_workspace_bytes(), W<int>(ws, pl.tcerr), st, &cg);
-}
-
-static int torso_forward_shallow(const seedrl_net* n, const float* prm, const Plan& pl,
-                                 const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_forward_shallow(const Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   const int N = pl.N;
   float* a1 = W<float>(ws, pl.sh_a1);
   float* a2 = W<float>(ws, pl.sh_a2);
   if (n->conv_mode >= 1 && n->cfg.obs_c % 4 == 0) {
-    // tensor-core modes: im2col + wgmma GEMM with bias + ReLU in the epilogue (the R2D2 body's path)
-    const int C = n->cfg.obs_c, K0 = 64 * C, K1 = 16 * 16;
-    float* col0 = W<float>(ws, pl.sh_col0); float* col1 = W<float>(ws, pl.sh_col1);
-    GemmEpi e = epi_none();
-    e.bias = P(n, prm, n->sh_c0b); e.relu = 1;
-    const int M0 = N * n->sh_h1 * n->sh_w1, M1 = N * n->sh_h2 * n->sh_w2;
-    // the im2col matrices are gathered inside the GEMM's operand staging where the geometry allows it
-    // (kernels.h ConvGather); otherwise materialised (and kept for the weight gradient)
-    ConvGather cg;
-    if (shallow_gathered(n, 0, N, obs, &cg)) {
-      SEEDRL_TRY(run_gemm_gather(n, ws, pl, false, M0, 16, K0, cg, P(n, prm, n->sh_c0w), 16, a1, 16, e, st));
-    } else {
-      SEEDRL_TRY(im2col_nhwc(N, n->cfg.obs_h, n->cfg.obs_w, C, 8, 4, 1, obs, col0, st));
-      SEEDRL_TRY(run_gemm(n, ws, pl, false, false, M0, 16, K0, col0, K0, P(n, prm, n->sh_c0w), 16, a1, 16, e, st));
-    }
-    e.bias = P(n, prm, n->sh_c1b);
-    if (shallow_gathered(n, 1, N, a1, &cg)) {
-      SEEDRL_TRY(run_gemm_gather(n, ws, pl, false, M1, 32, K1, cg, P(n, prm, n->sh_c1w), 32, a2, 32, e, st));
-    } else {
-      SEEDRL_TRY(im2col_nhwc(N, n->sh_h1, n->sh_w1, 16, 4, 2, 0, a1, col1, st));
-      SEEDRL_TRY(run_gemm(n, ws, pl, false, false, M1, 32, K1, col1, K1, P(n, prm, n->sh_c1w), 32, a2, 32, e, st));
-    }
-    return SEEDRL_OK;
+    // tensor-core modes: the R2D2 body's im2col + GEMM layers (strided_conv.cu)
+    SEEDRL_TRY(n->sh[0].forward(c.ex, N, true, obs, c.P(n->sh_w[0]), c.P(n->sh_b[0]), W<float>(ws, pl.sh_col0), a1,
+                                16));
+    return n->sh[1].forward(c.ex, N, false, a1, c.P(n->sh_w[1]), c.P(n->sh_b[1]), W<float>(ws, pl.sh_col1), a2, 32);
   }
   SEEDRL_TRY(convgen_forward(N, n->cfg.obs_h, n->cfg.obs_w, n->cfg.obs_c, 16, 8, 4, 1, obs,
-                             P(n, prm, n->sh_c0w), P(n, prm, n->sh_c0b), 1, a1, st));
-  SEEDRL_TRY(convgen_forward(N, n->sh_h1, n->sh_w1, 16, 32, 4, 2, 0, a1, P(n, prm, n->sh_c1w),
-                             P(n, prm, n->sh_c1b), 1, a2, st));
+                             c.P(n->sh_w[0]), c.P(n->sh_b[0]), 1, a1, st));
+  SEEDRL_TRY(convgen_forward(N, n->sh[0].hout, n->sh[0].wout, 16, 32, 4, 2, 0, a1, c.P(n->sh_w[1]),
+                             c.P(n->sh_b[1]), 1, a2, st));
   return SEEDRL_OK;
 }
 
@@ -638,6 +539,7 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   const Plan pl = make_plan(n, T1, B);
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
+  Call c(n, pl, prm, nullptr, ws, st);
   const int N = pl.N, A = n->cfg.num_actions, CI = n->core_in;
   // bounded-wait error flag of the wgmma / persistent kernels: cleared here, set by any kernel of
   // this forward or the matching backward, read back by seedrl_net_check_error
@@ -645,21 +547,13 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   const float* flat_src;
   int flat_relu;
   if (n->cfg.net == SEEDRL_NET_DEEP) {
-    StepCtx ctx;
-    ctx.wb = WgradBatch{nullptr, 0, 0, 0, {}};
-    PadScope pad(n, prm, pl, observation, ws, st);
-    SEEDRL_TRY(pad.rc);
-    observation = pad.obs;
-    SEEDRL_TRY(pack_all_weights(n, prm, ws, pl, 0, &ctx, st));
-    t_ctx = &ctx;
-    const int rc_t = n->conv_mode == 3 ? torso_forward_planes(n, prm, pl, observation, ws, st)
-                                       : torso_forward_deep(n, prm, pl, observation, ws, st);
-    t_ctx = nullptr;
-    SEEDRL_TRY(rc_t);
+    SEEDRL_TRY(pad_first_layer(c, &observation));
+    SEEDRL_TRY(pack_all_weights(c, 0));
+    SEEDRL_TRY(n->conv_mode == 3 ? torso_forward_planes(c, observation) : torso_forward_deep(c, observation));
     flat_src = W<float>(ws, pl.st.back().o1);
     flat_relu = 1;                         // tf.nn.relu before Flatten, networks.py:105
   } else {
-    SEEDRL_TRY(torso_forward_shallow(n, prm, pl, observation, ws, st));
+    SEEDRL_TRY(torso_forward_shallow(c, observation));
     flat_src = W<float>(ws, pl.sh_a2);
     flat_relu = 0;                         // already relu'd
   }
@@ -671,33 +565,33 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   float* c0buf = W<float>(ws, pl.c0buf);
   // Dense(256) + relu written straight into the first 256 columns of the core input
   GemmEpi e = epi_none();
-  e.bias = P(n, prm, n->p_dense_b); e.relu = 1; e.a_relu = flat_relu;
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, false, N, kHidden, n->flat, flat_src, n->flat, P(n, prm, n->p_dense_w),
-                   kHidden, xc, CI, e, st));
+  e.bias = c.P(n->p_dense_b); e.relu = 1; e.a_relu = flat_relu;
+  SEEDRL_TRY(c.ex.gemm(false, false, N, kHidden, n->flat, flat_src, n->flat, c.P(n->p_dense_w),
+                   kHidden, xc, CI, e));
   SEEDRL_TRY(core_input_tail(N, kHidden, A, reward, prev_actions, xc, st));
   // input projection for all T at once: z = xc W + b
   e = epi_none();
-  e.bias = P(n, prm, n->p_core_b);
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, false, N, 4 * kHidden, CI, xc, CI, P(n, prm, n->p_core_w), 4 * kHidden, z,
-                   4 * kHidden, e, st));
+  e.bias = c.P(n->p_core_b);
+  SEEDRL_TRY(c.ex.gemm(false, false, N, 4 * kHidden, CI, xc, CI, c.P(n->p_core_w), 4 * kHidden, z,
+                   4 * kHidden, e));
   SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)B * kHidden * 4, cudaMemcpyDeviceToDevice, st));
   GemmEpi eacc = epi_none();
   eacc.accumulate = 1;
   if (n->lstm_mode == 2) {
     // one kernel for the whole recurrence, CTA = (batch tile, 16 units) (lstm_tiled.cu)
-    SEEDRL_TRY(lstm_forward_tiled(kHidden, T1, B, P(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
+    SEEDRL_TRY(lstm_forward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
                                   W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   } else if (n->lstm_mode == 1) {
     // one cooperative kernel for the whole recurrence (lstm_persistent.cu)
-    SEEDRL_TRY(lstm_forward_persistent(kHidden, T1, B, P(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
+    SEEDRL_TRY(lstm_forward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
                                        W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   } else {
     SEEDRL_TRY(lstm_mask_state(B, kHidden, done, h0, hp, st));
   }
   for (int t = 0; t < T1 && n->lstm_mode == 0; ++t) {
     float* zt = z + (size_t)t * B * 4 * kHidden;
-    SEEDRL_TRY(run_gemm(n, ws, pl, false, false, B, 4 * kHidden, kHidden, hp + (size_t)t * B * kHidden, kHidden,
-                     P(n, prm, n->p_core_u), 4 * kHidden, zt, 4 * kHidden, eacc, st));
+    SEEDRL_TRY(c.ex.gemm(false, false, B, 4 * kHidden, kHidden, hp + (size_t)t * B * kHidden, kHidden,
+                     c.P(n->p_core_u), 4 * kHidden, zt, 4 * kHidden, eacc));
     const bool last = (t + 1 == T1);
     SEEDRL_TRY(lstm_pointwise_fwd(B, kHidden, zt, t == 0 ? c0buf : cs + (size_t)(t - 1) * B * kHidden,
                                   done + (size_t)t * B, last ? nullptr : done + (size_t)(t + 1) * B,
@@ -706,12 +600,12 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   }
   // heads, networks.py:116-118
   e = epi_none();
-  e.bias = P(n, prm, n->p_pol_b);
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, false, N, A, kHidden, hs, kHidden, P(n, prm, n->p_pol_w), A, policy_logits,
-                   A, e, st));
-  e.bias = P(n, prm, n->p_base_b);
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, false, N, 1, kHidden, hs, kHidden, P(n, prm, n->p_base_w), 1, baseline, 1,
-                   e, st));
+  e.bias = c.P(n->p_pol_b);
+  SEEDRL_TRY(c.ex.gemm(false, false, N, A, kHidden, hs, kHidden, c.P(n->p_pol_w), A, policy_logits,
+                   A, e));
+  e.bias = c.P(n->p_base_b);
+  SEEDRL_TRY(c.ex.gemm(false, false, N, 1, kHidden, hs, kHidden, c.P(n->p_base_w), 1, baseline, 1,
+                   e));
   if (h_out)
     SEEDRL_CUDA(cudaMemcpyAsync(h_out, hs + (size_t)(T1 - 1) * B * kHidden, (size_t)B * kHidden * 4,
                                 cudaMemcpyDeviceToDevice, st));
@@ -721,50 +615,39 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   return SEEDRL_OK;
 }
 
-// Reads back the device-side error flag of the last forward/backward that used this workspace
-// (set when a bounded mbarrier / grid-barrier wait of a wgmma or persistent kernel expired, i.e.
-// the results are garbage).  Synchronises `stream`.
 extern "C" int seedrl_net_check_error(const seedrl_net* n, int T1, int B, void* ws, size_t ws_bytes,
                                       seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(n && ws && T1 >= 1 && B >= 1, "bad arguments");
   const Plan pl = make_plan(n, T1, B);
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
-  int flag = 0;
-  SEEDRL_CUDA(cudaMemcpyAsync(&flag, W<int>(ws, pl.tcerr), sizeof(int), cudaMemcpyDeviceToHost,
-                              (cudaStream_t)stream));
-  SEEDRL_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  if (flag != 0)
-    return set_error(SEEDRL_ERR_INTERNAL,
-                     "a tensor-core / persistent kernel timed out on a barrier: results of this step are invalid");
-  return SEEDRL_OK;
+  return read_error_flag(W<int>(ws, pl.tcerr), (cudaStream_t)stream, "step");
 }
 
 // ---- backward -------------------------------------------------------------------
-static int conv_bwd(const seedrl_net* n, const float* prm, float* grd, const ConvLayer& l, int N,
-                    int H, int Wd, const void* x, int x_mode, const float* dy, const float* dmask,
-                    const float* dres, float* dx, void* ws, const Plan& pl, cudaStream_t st) {
+static int conv_bwd(Call& c, const ConvLayer& l, int N, int H, int Wd, const void* x, int x_mode, const float* dy,
+                    const float* dmask, const float* dres, float* dx) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   // weight + bias gradient
   if (n->conv_mode >= 1 && conv3x3_wgrad_tc_supported(l.cin, l.cout, x_mode)) {
     SEEDRL_TRY(conv3x3_wgrad_tc(l.cin, l.cout, x_mode, n->conv_mode >= 2, N, H, Wd, x, dy,
-                                G(n, grd, l.w), G(n, grd, l.b), W<float>(ws, pl.partial),
-                                conv3x3_wgrad_partial_bytes(), W<int>(ws, pl.tcerr),
-                                t_ctx ? &t_ctx->wb : nullptr, st));
+                                c.G(l.w), c.G(l.b), W<float>(ws, pl.partial),
+                                conv3x3_wgrad_partial_bytes(), c.ex.err, &c.wb, st));
   } else {
-    SEEDRL_TRY(conv3x3_wgrad(l.cin, l.cout, x_mode, N, H, Wd, x, dy, G(n, grd, l.w), G(n, grd, l.b),
+    SEEDRL_TRY(conv3x3_wgrad(l.cin, l.cout, x_mode, N, H, Wd, x, dy, c.G(l.w), c.G(l.b),
                              W<float>(ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
   }
   if (dx) {  // data gradient = conv with flipped, transposed weights
     g_conv_cat = PC_CONV_DGRAD;
-    const int rc = run_conv(n, ws, pl, l.cout, l.cin, IN_F32, N, H, Wd, dy, P(n, prm, l.w), nullptr,
-                            dmask, dres, dx, 1, st);
+    const int rc = run_conv(c, l.cout, l.cin, IN_F32, N, H, Wd, dy, c.P(l.w), nullptr,
+                            dmask, dres, dx, 1);
     g_conv_cat = PC_CONV_FWD;
     SEEDRL_TRY(rc);
   }
   return SEEDRL_OK;
 }
 
-static int torso_backward_deep(const seedrl_net* n, const float* prm, float* grd, const Plan& pl,
-                               const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_backward_deep(Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   // On entry gA holds d loss / d o1 of the last stack.
   const int N = pl.N;
   float* gA = W<float>(ws, pl.gA); float* gB = W<float>(ws, pl.gB);
@@ -776,42 +659,40 @@ static int torso_backward_deep(const seedrl_net* n, const float* prm, float* grd
     const float* o0 = W<float>(ws, b.o0); const float* c1 = W<float>(ws, b.c1);
     const int H = k.hout, Wd = k.wout;
     // block 1: o1 = conv11(relu(c1)) + o0 ; c1 = conv10(relu(o0))
-    SEEDRL_TRY(conv_bwd(n, prm, grd, k.r11, N, H, Wd, c1, IN_RELU, gA, c1, nullptr, gB, ws, pl, st));
-    SEEDRL_TRY(conv_bwd(n, prm, grd, k.r10, N, H, Wd, o0, IN_RELU, gB, o0, gA, gC, ws, pl, st));
+    SEEDRL_TRY(conv_bwd(c, k.r11, N, H, Wd, c1, IN_RELU, gA, c1, nullptr, gB));
+    SEEDRL_TRY(conv_bwd(c, k.r10, N, H, Wd, o0, IN_RELU, gB, o0, gA, gC));
     // block 0: o0 = conv01(relu(c0)) + p ; c0 = conv00(relu(p))
-    SEEDRL_TRY(conv_bwd(n, prm, grd, k.r01, N, H, Wd, c0, IN_RELU, gC, c0, nullptr, gB, ws, pl, st));
-    SEEDRL_TRY(conv_bwd(n, prm, grd, k.r00, N, H, Wd, p, IN_RELU, gB, p, gC, gA, ws, pl, st));
+    SEEDRL_TRY(conv_bwd(c, k.r01, N, H, Wd, c0, IN_RELU, gC, c0, nullptr, gB));
+    SEEDRL_TRY(conv_bwd(c, k.r00, N, H, Wd, p, IN_RELU, gB, p, gC, gA));
     // max-pool, then the stack's first conv
     SEEDRL_TRY(maxpool3s2_backward(N, k.hin, k.win, k.c, gA, W<uint8_t>(ws, b.idx), gF, st));
     const void* x = s == 0 ? (const void*)obs : (const void*)W<float>(ws, pl.st[s - 1].o1);
     if (s == 0 && generic_first(n))
-      SEEDRL_TRY(conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, G(n, grd, k.conv.w), G(n, grd, k.conv.b),
+      SEEDRL_TRY(conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, c.G(k.conv.w), c.G(k.conv.b),
                                   W<float>(ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
     else
-      SEEDRL_TRY(conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, x, s == 0 ? IN_U8 : IN_F32, gF, nullptr,
-                          nullptr, s == 0 ? nullptr : gA, ws, pl, st));
+      SEEDRL_TRY(conv_bwd(c, k.conv, N, k.hin, k.win, x, s == 0 ? IN_U8 : IN_F32, gF, nullptr,
+                          nullptr, s == 0 ? nullptr : gA));
   }
   return SEEDRL_OK;
 }
 
 // conv_mode 3 backward: every gradient between the Dense layer and the first conv is a plane tensor.
-static int planes_conv_bwd(const seedrl_net* n, const float* prm, float* grd, const ConvLayer& l, int N, int H,
-                           int Wd, const void* x, const void* dy, const void* dmask, const void* dres,
-                           void* dx, void* ws, const Plan& pl, cudaStream_t st) {
-  SEEDRL_TRY(wgradp(l.cin, l.cout, N, H, Wd, x, dy, G(n, grd, l.w), G(n, grd, l.b), W<int>(ws, pl.tcerr),
-                    t_ctx ? &t_ctx->wb : nullptr, st));
+static int planes_conv_bwd(Call& c, const ConvLayer& l, int N, int H, int Wd, const void* x, const void* dy,
+                           const void* dmask, const void* dres, void* dx) {
+  SEEDRL_TRY(wgradp(l.cin, l.cout, N, H, Wd, x, dy, c.G(l.w), c.G(l.b), c.ex.err, &c.wb, c.ex.st));
   if (dx) {
     g_conv_cat = PC_CONV_DGRAD;
-    const int rc = planes_conv(n, ws, pl, l.cout, l.cin, N, H, Wd, dy, P(n, prm, l.w), 1, nullptr, dmask, dres,
-                               dx, nullptr, nullptr, st);
+    const int rc = planes_conv(c, l.cout, l.cin, N, H, Wd, dy, c.P(l.w), 1, nullptr, dmask, dres,
+                               dx, nullptr, nullptr);
     g_conv_cat = PC_CONV_FWD;
     SEEDRL_TRY(rc);
   }
   return SEEDRL_OK;
 }
 
-static int torso_backward_planes(const seedrl_net* n, const float* prm, float* grd, const Plan& pl,
-                                 const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_backward_planes(Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   // On entry gA (fp32 NHWC) holds d loss / d o1 of the last stack.
   const int N = pl.N;
   void* g1 = W<void>(ws, pl.gP1); void* g2 = W<void>(ws, pl.gP2); void* g3 = W<void>(ws, pl.gP3);
@@ -827,80 +708,65 @@ static int torso_backward_planes(const seedrl_net* n, const float* prm, float* g
     const void* prelu = W<void>(ws, b.prelu); const void* c0r = W<void>(ws, b.c0r);
     const void* o0relu = W<void>(ws, b.o0relu); const void* c1r = W<void>(ws, b.c1r);
     // block 1: o1 = conv11(relu(c1)) + o0 ; c1 = conv10(relu(o0))
-    SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r11, N, H, Wd, c1r, g1, c1r, nullptr, g2, ws, pl, st));
-    SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r10, N, H, Wd, o0relu, g2, o0relu, g1, g3, ws, pl, st));
+    SEEDRL_TRY(planes_conv_bwd(c, k.r11, N, H, Wd, c1r, g1, c1r, nullptr, g2));
+    SEEDRL_TRY(planes_conv_bwd(c, k.r10, N, H, Wd, o0relu, g2, o0relu, g1, g3));
     // block 0: o0 = conv01(relu(c0)) + p ; c0 = conv00(relu(p))
-    SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r01, N, H, Wd, c0r, g3, c0r, nullptr, g2, ws, pl, st));
-    SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.r00, N, H, Wd, prelu, g2, prelu, g3, g1, ws, pl, st));
+    SEEDRL_TRY(planes_conv_bwd(c, k.r01, N, H, Wd, c0r, g3, c0r, nullptr, g2));
+    SEEDRL_TRY(planes_conv_bwd(c, k.r00, N, H, Wd, prelu, g2, prelu, g3, g1));
     // max-pool, then the stack's first conv
-    if (s == 0 && t_ctx && first_wgrad_pooled_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
+    if (s == 0 && first_wgrad_pooled_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
       // no gradient flows into the frames: the weight gradient is taken straight from the pooled
       // gradient and the pool's arg-max taps (conv_first.cu), the full-resolution tensor never exists
-      SEEDRL_TRY(first_wgrad_pooled(N, k.hin, k.win, first_c(n), obs, g1, W<uint8_t>(ws, b.idx), G(n, grd, k.conv.w),
-                                    G(n, grd, k.conv.b), &t_ctx->wb, st));
+      SEEDRL_TRY(first_wgrad_pooled(N, k.hin, k.win, first_c(n), obs, g1, W<uint8_t>(ws, b.idx), c.G(k.conv.w),
+                                    c.G(k.conv.b), &c.wb, st));
     } else if (s == 0 && generic_first(n)) {
       return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
                        "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
     } else if (s == 0) {
       SEEDRL_TRY(poolp_backward(N, k.hin, k.win, k.c, g1, W<uint8_t>(ws, b.idx), nullptr, gF, st));
-      SEEDRL_TRY(conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, obs, IN_U8, gF, nullptr, nullptr, nullptr, ws, pl,
-                          st));
+      SEEDRL_TRY(conv_bwd(c, k.conv, N, k.hin, k.win, obs, IN_U8, gF, nullptr, nullptr, nullptr));
     } else {
       SEEDRL_TRY(poolp_backward(N, k.hin, k.win, k.c, g1, W<uint8_t>(ws, b.idx), gfp, nullptr, st));
-      SEEDRL_TRY(planes_conv_bwd(n, prm, grd, k.conv, N, k.hin, k.win, W<void>(ws, pl.st[s - 1].o1p), gfp, nullptr,
-                                 nullptr, g1, ws, pl, st));
+      SEEDRL_TRY(planes_conv_bwd(c, k.conv, N, k.hin, k.win, W<void>(ws, pl.st[s - 1].o1p), gfp, nullptr,
+                                 nullptr, g1));
     }
   }
   return SEEDRL_OK;
 }
 
-static int torso_backward_shallow(const seedrl_net* n, const float* prm, float* grd, const Plan& pl,
-                                  const uint8_t* obs, void* ws, cudaStream_t st) {
+static int torso_backward_shallow(Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   // On entry gA holds d loss / d a2 (already masked by a2 > 0).
   const int N = pl.N;
   float* gA = W<float>(ws, pl.gA); float* gB = W<float>(ws, pl.gB);
   const float* a1 = W<float>(ws, pl.sh_a1);
   if (n->conv_mode >= 1 && n->cfg.obs_c % 4 == 0) {
-    const int C = n->cfg.obs_c, K0 = 64 * C, K1 = 16 * 16;
-    const int M1 = N * n->sh_h2 * n->sh_w2, M0 = N * n->sh_h1 * n->sh_w1;
-    float* col0 = W<float>(ws, pl.sh_col0); float* col1 = W<float>(ws, pl.sh_col1);
-    const GemmEpi e0 = epi_none();
-    ConvGather cg;
-    if (shallow_gathered(n, 1, N, a1, &cg))
-      SEEDRL_TRY(run_gemm_gather(n, ws, pl, true, K1, 32, M1, cg, gA, 32, G(n, grd, n->sh_c1w), 32, e0, st));
-    else
-      SEEDRL_TRY(run_gemm(n, ws, pl, true, false, K1, 32, M1, col1, K1, gA, 32, G(n, grd, n->sh_c1w), 32, e0, st));
-    SEEDRL_TRY(colsum(M1, 32, gA, 32, G(n, grd, n->sh_c1b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
-    SEEDRL_TRY(run_gemm(n, ws, pl, false, true, M1, K1, 32, gA, 32, P(n, prm, n->sh_c1w), 32, col1, K1, e0, st));
-    SEEDRL_TRY(col2im_nhwc(N, n->sh_h1, n->sh_w1, 16, 4, 2, col1, a1, gB, st));
-    if (shallow_gathered(n, 0, N, obs, &cg))
-      SEEDRL_TRY(run_gemm_gather(n, ws, pl, true, K0, 16, M0, cg, gB, 16, G(n, grd, n->sh_c0w), 16, e0, st));
-    else
-      SEEDRL_TRY(run_gemm(n, ws, pl, true, false, K0, 16, M0, col0, K0, gB, 16, G(n, grd, n->sh_c0w), 16, e0, st));
-    SEEDRL_TRY(colsum(M0, 16, gB, 16, G(n, grd, n->sh_c0b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
-    return SEEDRL_OK;
+    const StridedConv &l0 = n->sh[0], &l1 = n->sh[1];
+    float* col1 = W<float>(ws, pl.sh_col1);
+    SEEDRL_TRY(l1.wgrad(c.ex, N, false, a1, col1, gA, c.G(n->sh_w[1]), 32, c.G(n->sh_b[1])));
+    SEEDRL_TRY(l1.dgrad(c.ex, N, gA, c.P(n->sh_w[1]), col1, a1, gB));
+    return l0.wgrad(c.ex, N, true, obs, W<float>(ws, pl.sh_col0), gB, c.G(n->sh_w[0]), 16, c.G(n->sh_b[0]));
   }
-  SEEDRL_TRY(convgen_wgrad(N, n->sh_h1, n->sh_w1, 16, 32, 4, 2, 0, a1, gA, G(n, grd, n->sh_c1w),
-                           G(n, grd, n->sh_c1b), W<float>(ws, pl.partial),
+  SEEDRL_TRY(convgen_wgrad(N, n->sh[0].hout, n->sh[0].wout, 16, 32, 4, 2, 0, a1, gA, c.G(n->sh_w[1]),
+                           c.G(n->sh_b[1]), W<float>(ws, pl.partial),
                            conv3x3_wgrad_partial_bytes(), st));
-  SEEDRL_TRY(convgen_dgrad(N, n->sh_h1, n->sh_w1, 16, 32, 4, 2, gA, P(n, prm, n->sh_c1w), a1, gB, st));
+  SEEDRL_TRY(convgen_dgrad(N, n->sh[0].hout, n->sh[0].wout, 16, 32, 4, 2, gA, c.P(n->sh_w[1]), a1, gB, st));
   SEEDRL_TRY(convgen_wgrad(N, n->cfg.obs_h, n->cfg.obs_w, n->cfg.obs_c, 16, 8, 4, 1, obs, gB,
-                           G(n, grd, n->sh_c0w), G(n, grd, n->sh_c0b), W<float>(ws, pl.partial),
+                           c.G(n->sh_w[0]), c.G(n->sh_b[0]), W<float>(ws, pl.partial),
                            conv3x3_wgrad_partial_bytes(), st));
   return SEEDRL_OK;
 }
 
-extern "C" int seedrl_net_backward(const seedrl_net* n, const float* prm, int T1, int B,
-                                   const int64_t* prev_actions, const float* reward,
-                                   const uint8_t* done, const uint8_t* observation,
-                                   const float* dlogits, const float* dbaseline, float* grd,
-                                   void* ws, size_t ws_bytes, seedrl_stream_t stream) {
+// seedrl_net_backward; head_ready (may be null) is recorded once the first arena bucket's gradients are final.
+static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, const uint8_t* done,
+                        const uint8_t* observation, const float* dlogits, const float* dbaseline, float* grd,
+                        void* ws, size_t ws_bytes, cudaEvent_t head_ready, cudaStream_t st) {
   SEEDRL_CHECK_ARG(n && prm && done && observation && dlogits && dbaseline && grd && ws,
                    "null pointer");
-  (void)prev_actions; (void)reward;
   const Plan pl = make_plan(n, T1, B);
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
-  cudaStream_t st = (cudaStream_t)stream;
+  Call c(n, pl, prm, grd, ws, st);
+  c.head_ready = head_ready;
   const int N = pl.N, A = n->cfg.num_actions, CI = n->core_in;
   float* xc = W<float>(ws, pl.xc); float* z = W<float>(ws, pl.z);
   float* hp = W<float>(ws, pl.hp); float* cs = W<float>(ws, pl.cs);
@@ -909,25 +775,25 @@ extern "C" int seedrl_net_backward(const seedrl_net* n, const float* prm, int T1
   float* dhrec = W<float>(ws, pl.dhrec); float* dd = W<float>(ws, pl.dd);
   float* dcb[2] = {W<float>(ws, pl.dc0), W<float>(ws, pl.dc1)};
   // padding floats and the entropy_cost_param slot must not carry garbage into Adam / all-reduce
-  SEEDRL_CUDA(cudaMemsetAsync(grd, 0, n->arena_floats * sizeof(float), st));
+  SEEDRL_CUDA(cudaMemsetAsync(grd, 0, n->params.arena_floats * sizeof(float), st));
 
   // heads
   GemmEpi e = epi_none();
-  SEEDRL_TRY(run_gemm(n, ws, pl, true, false, kHidden, A, N, hs, kHidden, dlogits, A, G(n, grd, n->p_pol_w), A, e, st));
-  SEEDRL_TRY(colsum(N, A, dlogits, A, G(n, grd, n->p_pol_b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
-  SEEDRL_TRY(run_gemm(n, ws, pl, true, false, kHidden, 1, N, hs, kHidden, dbaseline, 1, G(n, grd, n->p_base_w), 1, e, st));
-  SEEDRL_TRY(colsum(N, 1, dbaseline, 1, G(n, grd, n->p_base_b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, true, N, kHidden, A, dlogits, A, P(n, prm, n->p_pol_w), A, dhs, kHidden, e, st));
+  SEEDRL_TRY(c.ex.gemm(true, false, kHidden, A, N, hs, kHidden, dlogits, A, c.G(n->p_pol_w), A, e));
+  SEEDRL_TRY(c.ex.colsum(N, A, dlogits, A, c.G(n->p_pol_b)));
+  SEEDRL_TRY(c.ex.gemm(true, false, kHidden, 1, N, hs, kHidden, dbaseline, 1, c.G(n->p_base_w), 1, e));
+  SEEDRL_TRY(c.ex.colsum(N, 1, dbaseline, 1, c.G(n->p_base_b)));
+  SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, A, dlogits, A, c.P(n->p_pol_w), A, dhs, kHidden, e));
   GemmEpi eacc = epi_none();
   eacc.accumulate = 1;
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, true, N, kHidden, 1, dbaseline, 1, P(n, prm, n->p_base_w), 1, dhs, kHidden,
-                   eacc, st));
+  SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, 1, dbaseline, 1, c.P(n->p_base_w), 1, dhs, kHidden,
+                   eacc));
   // BPTT
   if (n->lstm_mode == 2)
-    SEEDRL_TRY(lstm_backward_tiled(kHidden, T1, B, P(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
+    SEEDRL_TRY(lstm_backward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                    W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   if (n->lstm_mode == 1)
-    SEEDRL_TRY(lstm_backward_persistent(kHidden, T1, B, P(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
+    SEEDRL_TRY(lstm_backward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                         W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   for (int t = T1 - 1; t >= 0 && n->lstm_mode == 0; --t) {
     const bool last = (t + 1 == T1);
@@ -938,54 +804,58 @@ extern "C" int seedrl_net_backward(const seedrl_net* n, const float* prm, int T1
                                   last ? nullptr : dhrec, last ? nullptr : dcb[(t + 1) & 1],
                                   dz + (size_t)t * B * 4 * kHidden, dcb[t & 1], st));
     if (t > 0)
-      SEEDRL_TRY(run_gemm(n, ws, pl, false, true, B, kHidden, 4 * kHidden, dz + (size_t)t * B * 4 * kHidden,
-                       4 * kHidden, P(n, prm, n->p_core_u), 4 * kHidden, dhrec, kHidden, e, st));
+      SEEDRL_TRY(c.ex.gemm(false, true, B, kHidden, 4 * kHidden, dz + (size_t)t * B * 4 * kHidden,
+                       4 * kHidden, c.P(n->p_core_u), 4 * kHidden, dhrec, kHidden, e));
   }
-  SEEDRL_TRY(run_gemm(n, ws, pl, true, false, kHidden, 4 * kHidden, N, hp, kHidden, dz, 4 * kHidden,
-                   G(n, grd, n->p_core_u), 4 * kHidden, e, st));
-  SEEDRL_TRY(run_gemm(n, ws, pl, true, false, CI, 4 * kHidden, N, xc, CI, dz, 4 * kHidden, G(n, grd, n->p_core_w),
-                   4 * kHidden, e, st));
-  SEEDRL_TRY(colsum(N, 4 * kHidden, dz, 4 * kHidden, G(n, grd, n->p_core_b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
+  SEEDRL_TRY(c.ex.gemm(true, false, kHidden, 4 * kHidden, N, hp, kHidden, dz, 4 * kHidden,
+                   c.G(n->p_core_u), 4 * kHidden, e));
+  SEEDRL_TRY(c.ex.gemm(true, false, CI, 4 * kHidden, N, xc, CI, dz, 4 * kHidden, c.G(n->p_core_w),
+                   4 * kHidden, e));
+  SEEDRL_TRY(c.ex.colsum(N, 4 * kHidden, dz, 4 * kHidden, c.G(n->p_core_b)));
   // d dense_out = (dz W[:256,:]^T) * (dense_out > 0)
   GemmEpi em = epi_none();
   em.mask = xc; em.ldm = CI;
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, true, N, kHidden, 4 * kHidden, dz, 4 * kHidden, P(n, prm, n->p_core_w),
-                   4 * kHidden, dd, kHidden, em, st));
+  SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, 4 * kHidden, dz, 4 * kHidden, c.P(n->p_core_w),
+                   4 * kHidden, dd, kHidden, em));
   // Dense(256)
   const float* flat_src = n->cfg.net == SEEDRL_NET_DEEP ? W<float>(ws, pl.st.back().o1)
                                                         : W<float>(ws, pl.sh_a2);
   GemmEpi ea = epi_none();
   ea.a_relu = n->cfg.net == SEEDRL_NET_DEEP ? 1 : 0;
-  SEEDRL_TRY(run_gemm(n, ws, pl, true, false, n->flat, kHidden, N, flat_src, n->flat, dd, kHidden,
-                   G(n, grd, n->p_dense_w), kHidden, ea, st));
-  SEEDRL_TRY(colsum(N, kHidden, dd, kHidden, G(n, grd, n->p_dense_b), st, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes()));
+  SEEDRL_TRY(c.ex.gemm(true, false, n->flat, kHidden, N, flat_src, n->flat, dd, kHidden,
+                   c.G(n->p_dense_w), kHidden, ea));
+  SEEDRL_TRY(c.ex.colsum(N, kHidden, dd, kHidden, c.G(n->p_dense_b)));
   // every gradient of the arena's first bucket (heads, Dense, LSTM: floats [0, seedrl_net_grad_split))
   // is final here -- the conv torso's backward below only writes the second bucket
-  if (t_head_ready) SEEDRL_CUDA(cudaEventRecord((cudaEvent_t)t_head_ready, st));
+  if (c.head_ready) SEEDRL_CUDA(cudaEventRecord(c.head_ready, st));
   GemmEpi ef = epi_none();
   ef.mask = flat_src; ef.ldm = n->flat;
-  SEEDRL_TRY(run_gemm(n, ws, pl, false, true, N, n->flat, kHidden, dd, kHidden, P(n, prm, n->p_dense_w), kHidden,
-                   W<float>(ws, pl.gA), n->flat, ef, st));
+  SEEDRL_TRY(c.ex.gemm(false, true, N, n->flat, kHidden, dd, kHidden, c.P(n->p_dense_w), kHidden,
+                   W<float>(ws, pl.gA), n->flat, ef));
   if (n->cfg.net == SEEDRL_NET_DEEP) {
-    StepCtx ctx;
-    ctx.wb = WgradBatch{W<float>(ws, pl.partial_all), kPartialAllBytes / sizeof(float), 0, 0, {}};
-    PadScope pad(n, prm, pl, observation, ws, st);
-    SEEDRL_TRY(pad.rc);
-    observation = pad.obs;
-    SEEDRL_TRY(pack_all_weights(n, prm, ws, pl, 1, &ctx, st));
-    t_ctx = &ctx;
-    int rc_t = n->conv_mode == 3 ? torso_backward_planes(n, prm, grd, pl, observation, ws, st)
-                                 : torso_backward_deep(n, prm, grd, pl, observation, ws, st);
-    t_ctx = nullptr;
-    if (rc_t == SEEDRL_OK) rc_t = wgrad_reduce_batch(&ctx.wb, st);
-    if (rc_t == SEEDRL_OK && pad.active) {        // padded [3,3,4,16] gradient -> the [3,3,3,16] parameter slot
-      unpad_dw0_kernel<<<ceil_div(9 * 3 * 16, 128), 128, 0, st>>>(16, W<float>(ws, pl.dw0pad),
-                                                                   grd + n->params[n->stacks[0].conv.w].offset);
+    c.wb = WgradBatch{W<float>(ws, pl.partial_all), kPartialAllBytes / sizeof(float), 0, 0, {}};
+    SEEDRL_TRY(pad_first_layer(c, &observation));
+    SEEDRL_TRY(pack_all_weights(c, 1));
+    SEEDRL_TRY(n->conv_mode == 3 ? torso_backward_planes(c, observation) : torso_backward_deep(c, observation));
+    SEEDRL_TRY(wgrad_reduce_batch(&c.wb, st));
+    if (c.dw0_pad) {        // padded [3,3,4,16] gradient -> the [3,3,3,16] parameter slot
+      unpad_dw0_kernel<<<ceil_div(9 * 3 * 16, 128), 128, 0, st>>>(16, c.dw0_pad,
+                                                                   grd + n->params.offset(n->stacks[0].conv.w));
       count_launch(PC_MISC, st);
     }
-    return rc_t;
+    return SEEDRL_OK;
   }
-  return torso_backward_shallow(n, prm, grd, pl, observation, ws, st);
+  return torso_backward_shallow(c, observation);
+}
+
+extern "C" int seedrl_net_backward(const seedrl_net* n, const float* prm, int T1, int B,
+                                   const int64_t* prev_actions, const float* reward,
+                                   const uint8_t* done, const uint8_t* observation,
+                                   const float* dlogits, const float* dbaseline, float* grd,
+                                   void* ws, size_t ws_bytes, seedrl_stream_t stream) {
+  (void)prev_actions; (void)reward;
+  return net_backward(n, prm, T1, B, done, observation, dlogits, dbaseline, grd, ws, ws_bytes, nullptr,
+                      (cudaStream_t)stream);
 }
 
 // Data-parallel overlap (SURVEY 8e: the one exchange step): same as seedrl_net_backward, and
@@ -999,16 +869,14 @@ extern "C" int seedrl_net_backward_overlap(const seedrl_net* n, const float* prm
                                            const uint8_t* observation, const float* dlogits, const float* dbaseline,
                                            float* grd, void* ws, size_t ws_bytes, void* head_ready_event,
                                            seedrl_stream_t stream) {
-  t_head_ready = head_ready_event;
-  const int rc = seedrl_net_backward(n, prm, T1, B, prev_actions, reward, done, observation, dlogits, dbaseline, grd,
-                                     ws, ws_bytes, stream);
-  t_head_ready = nullptr;
-  return rc;
+  (void)prev_actions; (void)reward;
+  return net_backward(n, prm, T1, B, done, observation, dlogits, dbaseline, grd, ws, ws_bytes,
+                      (cudaEvent_t)head_ready_event, (cudaStream_t)stream);
 }
 extern "C" size_t seedrl_net_grad_split(const seedrl_net* n) {
   if (!n) return 0;
-  const int first_conv = n->cfg.net == SEEDRL_NET_DEEP ? n->stacks[0].conv.w : n->sh_c0w;
-  return n->params[first_conv].offset;
+  const int first_conv = n->cfg.net == SEEDRL_NET_DEEP ? n->stacks[0].conv.w : n->sh_w[0];
+  return n->params.offset(first_conv);
 }
 
 // ---- single-kernel test hooks (exported so the GPU parity tests can localise a
@@ -1071,10 +939,6 @@ extern "C" int seedrl_debug_colsum(int M, int N, const float* X, int ld, float* 
   return colsum(M, N, X, ld, out, (cudaStream_t)stream, ws, ws_bytes);
 }
 
-// wgmma conv test hook: packs fp32 HWIO weights (optionally flipped/transposed for the
-// data-gradient) into `wq_scratch` (>= 2*9*max(cin,16)*cout*2 bytes) and runs the tensor-core conv.
-// `variant` bit0/bit1 swap LBO/SBO of the A/B descriptors (bring-up aid); *error_flag is
-// set to 1 by the kernel if its bounded mbarrier wait expires.
 // Host evaluation of the tall-image position -> pixel maps the conv kernels use (multiply-high
 // division): which = 0 padded-input position, 1 output position.  No GPU involved.
 extern "C" int seedrl_debug_conv_pixels(int N, int H, int W, int which, int start, int count, int* out) {
@@ -1100,8 +964,6 @@ extern "C" int seedrl_debug_conv3x3_wgrad_tc(int cin, int cout, int in_mode, int
   return conv3x3_wgrad_tc(cin, cout, in_mode, split, N, H, W, x, dy, dw, db, partial, partial_bytes,
                           error_flag, nullptr, (cudaStream_t)stream);
 }
-// Bench knob: output positions per tile of the tensor-core forward / data-gradient kernel
-// (the largest of 512/256/128 not above `mt` that keeps >= 2 CTAs per SM is used; default 512).
 extern "C" int seedrl_debug_conv0pool(int N, int H, int W, const uint8_t* frames, const float* w, const float* bias,
                                       void* praw, void* prelu, uint8_t* idx, int* err, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(frames && w && bias && praw && prelu && idx && err, "null pointer");
@@ -1132,12 +994,18 @@ extern "C" int seedrl_debug_set_gemm_bk(int bk) {
   gemm_tc_set_bk(bk);
   return SEEDRL_OK;
 }
+// Bench knob: output positions per tile of the tensor-core forward / data-gradient kernel
+// (the largest of 512/256/128 not above `mt` that keeps >= 2 CTAs per SM is used; default 512).
 extern "C" int seedrl_debug_set_conv_tile(int mt) {
   SEEDRL_CHECK_ARG(mt == 128 || mt == 256 || mt == 512, "tile must be 128, 256 or 512");
   conv3x3_tc_set_tile(mt);
   return SEEDRL_OK;
 }
 
+// wgmma conv test hook: packs fp32 HWIO weights (optionally flipped/transposed for the
+// data-gradient) into `wq_scratch` (>= 2*9*max(cin,16)*cout*2 bytes) and runs the tensor-core conv.
+// `variant` bit0/bit1 swap LBO/SBO of the A/B descriptors (bring-up aid); *error_flag is
+// set to 1 by the kernel if its bounded mbarrier wait expires.
 extern "C" int seedrl_debug_conv3x3_tc(int cin, int cout, int in_mode, int split, int N, int H, int W,
                                        const void* in, const float* w, const float* bias,
                                        const float* mask, const float* res, float* out, int flip,
