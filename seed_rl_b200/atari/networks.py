@@ -75,9 +75,13 @@ class DuelingLSTMDQNNet(object):
   dueling value / advantage heads, greedy action.  Parameters live in one flat fp32 HBM arena
   (Keras layouts, tf.Module variable order)."""
 
-  def __init__(self, num_actions, observation_shape, stack_size=1, seed=0, device=None, gemm_mode='tc3'):
+  def __init__(self, num_actions, observation_shape, stack_size=1, seed=0, device=None, gemm_mode='tc3',
+               lstm_mode='tiled'):
     """gemm_mode: 'tc3' = wgmma bf16x3 (fp32-faithful) for every contraction (convolutions as
-    im2col GEMMs, Dense, LSTM projection, heads); 'simt' = fp32 CUDA cores."""
+    im2col GEMMs, Dense, LSTM projection, heads); 'simt' = fp32 CUDA cores.  lstm_mode: how the
+    recurrent products of the LSTM core are computed: 'tiled' = one persistent kernel each way on
+    fp32 CUDA cores, 'tc3' = the same recurrence on wgmma with bf16x3 operands, 'persistent' = the
+    first persistent form."""
     L = _lib.lib()
     self._num_actions = int(num_actions)
     self._observation_shape = tuple(int(x) for x in observation_shape)
@@ -97,6 +101,11 @@ class DuelingLSTMDQNNet(object):
       raise ValueError("gemm_mode must be 'simt' or 'tc3'")
     self.gemm_mode = gemm_mode
     _lib.check(L.seedrl_r2d2_net_set_mode(h, modes[gemm_mode]))
+    lstm_modes = {'persistent': 1, 'tiled': 2, 'tc3': 3}
+    if lstm_mode not in lstm_modes:
+      raise ValueError("lstm_mode must be 'tiled', 'tc3' (the tiled recurrence on wgmma bf16x3) or 'persistent'")
+    self.lstm_mode = lstm_mode
+    _lib.check(L.seedrl_r2d2_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
     self._n_tensors = L.seedrl_r2d2_net_num_param_tensors(h)
     self.arena_floats = int(L.seedrl_r2d2_net_arena_floats(h))
     self.num_params = int(L.seedrl_r2d2_net_num_params(h))

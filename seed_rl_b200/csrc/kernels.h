@@ -228,4 +228,13 @@ int lstm_backward_tiled(int H, int T1, int B, const float* U, const uint8_t* don
                         const float* cs, const float* c0, const float* dhs, float* dz, unsigned int* counter,
                         int* err, cudaStream_t st);
 
+// lstm_tc.cu: the same recurrence with the recurrent products on wgmma in bf16x3, CTA = (64-row batch
+// tile, 16 hidden units); same arguments and workspace as the tiled form
+int lstm_forward_tc(int H, int T1, int B, const float* U, const uint8_t* done, float* z, const float* h0,
+                    const float* c0, float* hs, float* cs, float* hp, unsigned int* counter, int* err,
+                    cudaStream_t st);
+int lstm_backward_tc(int H, int T1, int B, const float* U, const uint8_t* done, const float* gates,
+                     const float* cs, const float* c0, const float* dhs, float* dz, unsigned int* counter,
+                     int* err, cudaStream_t st);
+
 }  // namespace seedrl

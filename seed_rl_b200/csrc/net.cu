@@ -34,7 +34,8 @@ struct seedrl_net {
   seedrl::StridedConv sh[2];               // shallow: conv 8x8/4 -> 16, conv 4x4/2 -> 32
   int sh_w[2], sh_b[2];                    // their param indices
   int flat;                                // conv features fed to Dense(256)
-  int lstm_mode = 2;                       // 2 = tiled persistent kernels (lstm_tiled.cu), 1 = first persistent form, 0 = per-step launches
+  int lstm_mode = 2;                       // 2 = tiled persistent kernels (lstm_tiled.cu), 1 = first persistent form, 0 = per-step launches,
+                                           // 3 = tiled on wgmma bf16x3 (lstm_tc.cu)
   int conv_mode = 0;                       // 0 = fp32 SIMT, 1 = wgmma bf16, 2 = wgmma bf16x3 (fp32-faithful)
   int core_in;                             // 256 + 1 + A
 };
@@ -385,7 +386,7 @@ extern "C" int seedrl_net_num_param_tensors(const seedrl_net* net) {
 extern "C" size_t seedrl_net_num_params(const seedrl_net* net) { return net ? net->logical_params : 0; }
 extern "C" size_t seedrl_net_arena_floats(const seedrl_net* net) { return net ? net->params.arena_floats : 0; }
 extern "C" int seedrl_net_set_lstm_mode(seedrl_net* net, int mode) {
-  SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 2, "mode must be 0 (per-step launches), 1 (persistent, CTA = 2 units) or 2 (persistent, CTA = batch tile x 16 units)");
+  SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 3, "mode must be 0 (per-step launches), 1 (persistent, CTA = 2 units), 2 (persistent, CTA = batch tile x 16 units) or 3 (as 2 on wgmma bf16x3)");
   net->lstm_mode = mode;
   return SEEDRL_OK;
 }
@@ -581,6 +582,10 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
     // one kernel for the whole recurrence, CTA = (batch tile, 16 units) (lstm_tiled.cu)
     SEEDRL_TRY(lstm_forward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
                                   W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  } else if (n->lstm_mode == 3) {
+    // the same recurrence with the recurrent products on the tensor cores (lstm_tc.cu)
+    SEEDRL_TRY(lstm_forward_tc(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
+                               W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   } else if (n->lstm_mode == 1) {
     // one cooperative kernel for the whole recurrence (lstm_persistent.cu)
     SEEDRL_TRY(lstm_forward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
@@ -792,6 +797,9 @@ static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, co
   if (n->lstm_mode == 2)
     SEEDRL_TRY(lstm_backward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                    W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  if (n->lstm_mode == 3)
+    SEEDRL_TRY(lstm_backward_tc(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
+                                W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   if (n->lstm_mode == 1)
     SEEDRL_TRY(lstm_backward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                         W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));

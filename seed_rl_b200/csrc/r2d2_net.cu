@@ -22,7 +22,8 @@ constexpr int kRH = 512;                 // LSTMCell(512), Dense(512) (networks.
 struct seedrl_r2d2_net {
   int A, H, W, C;
   int mode;                               // 0 = fp32 SIMT GEMMs, 2 = wgmma bf16x3
-  int lstm_mode = 2;                      // 2 = tiled persistent LSTM (lstm_tiled.cu), 1 = first persistent form
+  int lstm_mode = 2;                      // 2 = tiled persistent LSTM (lstm_tiled.cu), 1 = first persistent form,
+                                          // 3 = tiled on wgmma bf16x3 (lstm_tc.cu)
   seedrl::ParamTable params;
   size_t logical_params;
   seedrl::StridedConv conv[3];
@@ -188,7 +189,8 @@ extern "C" int seedrl_r2d2_net_set_mode(seedrl_r2d2_net* net, int mode) {
   return SEEDRL_OK;
 }
 extern "C" int seedrl_r2d2_net_set_lstm_mode(seedrl_r2d2_net* net, int mode) {
-  SEEDRL_CHECK_ARG(net && (mode == 1 || mode == 2), "mode must be 1 (persistent) or 2 (tiled persistent)");
+  SEEDRL_CHECK_ARG(net && mode >= 1 && mode <= 3,
+                   "mode must be 1 (persistent), 2 (tiled persistent) or 3 (tiled persistent on wgmma bf16x3)");
   net->lstm_mode = mode;
   return SEEDRL_OK;
 }
@@ -248,6 +250,9 @@ extern "C" int seedrl_r2d2_net_forward(const seedrl_r2d2_net* n, const float* pr
   if (n->lstm_mode == 2)
     SEEDRL_TRY(lstm_forward_tiled(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
                                   W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  else if (n->lstm_mode == 3)
+    SEEDRL_TRY(lstm_forward_tc(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
+                               W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   else
     SEEDRL_TRY(lstm_forward_persistent(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
                                        W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
@@ -322,6 +327,9 @@ extern "C" int seedrl_r2d2_net_backward(const seedrl_r2d2_net* n, const float* p
   if (n->lstm_mode == 2)
     SEEDRL_TRY(lstm_backward_tiled(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                    W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  else if (n->lstm_mode == 3)
+    SEEDRL_TRY(lstm_backward_tc(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
+                                W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
   else
     SEEDRL_TRY(lstm_backward_persistent(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
                                         W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));

@@ -36,7 +36,9 @@ class _CudaAgent(object):
     """conv_mode selects the arithmetic of every contraction (3x3 convs, Dense, LSTM input
     projection, policy head): 'simt' = fp32 CUDA cores (the 2e-3 parity path), 'tc' = wgmma
     tensor cores with bf16 operands and fp32 accumulation, 'tc3' = wgmma with bf16x3 split
-    operands (fp32-faithful)."""
+    operands (fp32-faithful).  lstm_mode selects how the recurrent products of the LSTM core are
+    computed: 'tiled' = one persistent kernel each way on fp32 CUDA cores, 'tc3' = the same
+    recurrence on wgmma with bf16x3 operands, 'persistent' / 'stepwise' = earlier forms."""
     self._num_actions = int(num_actions)
     self._obs_shape = tuple(int(x) for x in obs_shape)
     if self._NET == _lib.NET_DEEP and (len(self._obs_shape) != 3 or not 1 <= self._obs_shape[2] <= 16):
@@ -55,9 +57,10 @@ class _CudaAgent(object):
       raise ValueError("conv_mode 'tc3p' is built for the deep net")
     self.conv_mode = conv_mode
     _lib.check(L.seedrl_net_set_conv_mode(h, modes[conv_mode]))
-    lstm_modes = {'stepwise': 0, 'persistent': 1, 'tiled': 2}
+    lstm_modes = {'stepwise': 0, 'persistent': 1, 'tiled': 2, 'tc3': 3}
     if lstm_mode not in lstm_modes:
-      raise ValueError("lstm_mode must be 'tiled', 'persistent' or 'stepwise'")
+      raise ValueError("lstm_mode must be 'tiled', 'tc3' (the tiled recurrence on wgmma bf16x3), "
+                       "'persistent' or 'stepwise'")
     self.lstm_mode = lstm_mode
     _lib.check(L.seedrl_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
     self._n_tensors = L.seedrl_net_num_param_tensors(h)
