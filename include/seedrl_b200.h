@@ -256,6 +256,14 @@ int seedrl_store_append_field(uint8_t* state, const int32_t* index,
 int seedrl_store_advance(int32_t* index, const int32_t* env_ids, int n,
                          int full_length, int32_t* completed_ids,
                          int32_t* num_completed, seedrl_stream_t stream);
+/* Same, for a batch that mixes training and eval environments: rows whose env id is >= id_limit
+ * are neither advanced nor reported (the store has rows for ids < id_limit only); completed ids
+ * keep env_ids order among the rows that are kept.  A CUDA graph has a fixed batch, so it cannot
+ * drop the eval rows on the host as agents/r2d2/learner.py:792-803 does. */
+int seedrl_store_advance_limit(int32_t* index, const int32_t* env_ids, int n,
+                               int full_length, int32_t* completed_ids,
+                               int32_t* num_completed, int32_t id_limit,
+                               seedrl_stream_t stream);
 /* For each completed env: copy its full unroll rows to `unrolls`
  * ([n_completed, full_length, row_bytes], env-major like the reference, or
  * time-major [full_length, n_completed, row_bytes] if time_major != 0, which
@@ -281,6 +289,10 @@ typedef struct seedrl_row_job {
 } seedrl_row_job;
 int seedrl_rows_multi(const seedrl_row_job* jobs, int njobs, const int32_t* env_ids, int n,
                       const int32_t* index, seedrl_stream_t stream);
+/* Same, with append jobs (mode 2) skipping the rows whose env id is >= id_limit; gather and
+ * scatter jobs move every row.  seedrl_rows_multi is this with id_limit = INT32_MAX. */
+int seedrl_rows_multi_limit(const seedrl_row_job* jobs, int njobs, const int32_t* env_ids, int n,
+                            const int32_t* index, int32_t id_limit, seedrl_stream_t stream);
 /* Zero-copy minibatch assembly (SURVEY 8(f) rank 2; replaces the queue-element copy, tf.stack and
  * make_time_major of agents/vtrace/learner.py:418-432): like seedrl_store_gather_field with
  * time_major = 1, but unroll i lands in column col0 + i of the caller's batch tensor
@@ -401,6 +413,17 @@ int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_train, const fl
                              const float* importance_weights, float gamma, int n_steps, float eta,
                              float value_rescaling_eps, float* loss, float* priorities, float* dq,
                              void* scratch, seedrl_stream_t stream);
+/* <- agents/r2d2/learner.py:155-177 (apply_epsilon_greedy) on the device.  actions int32 [N]: the
+ *   greedy actions on entry, the chosen ones on exit; envs_epsilon float32 [num_envs] (the table of
+ *   get_envs_epsilon, :129-152), read at env_ids[n].  Row n draws
+ *   r = Philox4x32-10(counter = (c lo, c hi, n, 0), key = (seed lo, seed hi)) with c = *counter_dev;
+ *   it explores iff (r.x >> 8) * 2^-24 < epsilon, and then takes action (r.y * A) >> 32 (64-bit
+ *   product).  *counter_dev is then incremented by one (a second launch), so the call is capturable
+ *   in a CUDA graph and draws fresh numbers on every replay.  The reference draws from TF's global
+ *   generator: same distribution, different stream. */
+int seedrl_r2d2_epsilon_greedy(int N, int A, const int32_t* env_ids, const float* envs_epsilon,
+                               uint64_t seed, uint64_t* counter_dev, int32_t* actions,
+                               seedrl_stream_t stream);
 /* <- common/utils.py:327-352 (PrioritizedReplay.sample, priority_exp != 0): prob_i =
  *   prio_i^alpha / sum over the first `limit` slots; index_j = inverse CDF of uniforms[j] in
  *   [0,1) (the reference draws with tf.random.categorical: same distribution, different

@@ -39,8 +39,9 @@ class RowJob(ctypes.Structure):
 ROW_GATHER, ROW_SCATTER, ROW_APPEND = 0, 1, 2
 
 
-def rows_multi(jobs, env_ids_i32, index=None):
-  """jobs: list of (table tensor, rows tensor, mode).  One launch (seedrl_rows_multi)."""
+def rows_multi(jobs, env_ids_i32, index=None, id_limit=None):
+  """jobs: list of (table tensor, rows tensor, mode).  One launch (seedrl_rows_multi; with
+  id_limit, seedrl_rows_multi_limit: append jobs skip the rows whose env id is >= id_limit)."""
   n = int(env_ids_i32.numel())
   arr = (RowJob * len(jobs))()
   for k, (table, rows, mode) in enumerate(jobs):
@@ -48,7 +49,11 @@ def rows_multi(jobs, env_ids_i32, index=None):
     if rows.numel() * rows.element_size() != n * rb or rows.dtype != table.dtype or not rows.is_contiguous():
       raise ValueError('rows_multi: rows do not match the table (job %d)' % k)
     arr[k] = RowJob(table.data_ptr(), rows.data_ptr(), rb, mode, table.shape[1] if mode == ROW_APPEND else 0)
-  check(lib().seedrl_rows_multi(arr, len(jobs), ptr(env_ids_i32), n, ptr(index), stream_ptr()))
+  if id_limit is None:
+    check(lib().seedrl_rows_multi(arr, len(jobs), ptr(env_ids_i32), n, ptr(index), stream_ptr()))
+  else:
+    check(lib().seedrl_rows_multi_limit(arr, len(jobs), ptr(env_ids_i32), n, ptr(index), int(id_limit),
+                                        stream_ptr()))
 
 
 class NetConfig(ctypes.Structure):
@@ -101,8 +106,10 @@ SIGNATURES = {
     'seedrl_net_check_error': (c_int, [P, c_int, c_int, P, c_size_t, P]),
     'seedrl_store_append_field': (c_int, [P, P, P, c_int, c_int, c_size_t, P, P]),
     'seedrl_store_advance': (c_int, [P, P, c_int, c_int, P, P, P]),
+    'seedrl_store_advance_limit': (c_int, [P, P, c_int, c_int, P, P, ctypes.c_int32, P]),
     'seedrl_store_gather_field': (c_int, [P, P, c_int, c_int, c_size_t, c_int, c_int, P, P]),
     'seedrl_rows_multi': (c_int, [P, c_int, P, c_int, P, P]),
+    'seedrl_rows_multi_limit': (c_int, [P, c_int, P, c_int, P, ctypes.c_int32, P]),
     'seedrl_store_gather_field_into': (c_int, [P, P, c_int, c_int, c_size_t, c_int, P, c_int, c_int, P]),
     'seedrl_store_finish': (c_int, [P, P, c_int, c_int, P]),
     'seedrl_store_reset': (c_int, [P, P, P, c_int, c_int, c_size_t, c_int, P]),
@@ -138,6 +145,7 @@ SIGNATURES = {
     'seedrl_r2d2_loss_scratch_bytes': (c_size_t, [c_int, c_int, c_int]),
     'seedrl_r2d2_loss_fwd_bwd': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, c_float, c_int, c_float, c_float,
                                          P, P, P, P, P]),
+    'seedrl_r2d2_epsilon_greedy': (c_int, [c_int, c_int, P, P, c_u64, P, P, P]),
     'seedrl_replay_sample': (c_int, [c_int, P, c_float, c_float, c_int, P, P, P, P, P]),
     'seedrl_clip_scratch_bytes': (c_size_t, []),
     'seedrl_clip_by_global_norm': (c_int, [c_size_t, P, c_float, P, P, P]),

@@ -59,6 +59,10 @@ _define(flags.DEFINE_float, 'value_function_rescaling_epsilon', 1e-3, 'Epsilon u
 _define(flags.DEFINE_integer, 'n_steps', 5, 'n-step returns: how far ahead we look for computing the Bellman targets.')
 _define(flags.DEFINE_float, 'discounting', .997, 'Discounting factor.')
 _define(flags.DEFINE_float, 'eval_epsilon', 1e-3, 'Epsilon (as in epsilon-greedy) used for evaluation.')
+_define(flags.DEFINE_bool, 'inference_cuda_graph', False,
+        'Replay the device side of every full inference batch as one CUDA graph, with epsilon-greedy '
+        'drawn on the device from Philox (a different random stream than the torch generator of the '
+        'default path, so the explored actions differ).')
 
 AgentOutput = collections.namedtuple('AgentOutput', 'action q_values')
 
@@ -118,6 +122,22 @@ def apply_epsilon_greedy(actions, env_ids, num_training_envs, num_eval_envs, eva
   random_actions = torch.randint(0, num_actions, [B], dtype=torch.int32, device=actions.device, generator=generator)
   probs = torch.rand([B], device=actions.device, generator=generator)
   return torch.where(probs < eps, random_actions, actions)
+
+
+def device_epsilon_greedy(actions, env_ids_i32, envs_epsilon, num_actions, seed, counter):
+  """apply_epsilon_greedy in place, capturable in a CUDA graph (seedrl_r2d2_epsilon_greedy):
+  actions int32 [B] (greedy on entry), envs_epsilon float32 [num_envs] (the get_envs_epsilon table),
+  counter an int64 device scalar: the Philox offset, incremented by the call.  Draws from a
+  different random stream than apply_epsilon_greedy, with the same distribution."""
+  for t, dt, name in ((actions, torch.int32, 'actions'), (env_ids_i32, torch.int32, 'env_ids'),
+                      (envs_epsilon, torch.float32, 'envs_epsilon'), (counter, torch.int64, 'counter')):
+    if not (t.is_cuda and t.dtype == dt and t.is_contiguous()):
+      raise ValueError('%s must be a contiguous CUDA %s tensor' % (name, dt))
+  if env_ids_i32.numel() != actions.numel():
+    raise ValueError('env_ids and actions must have the same length')
+  _lib.check(_lib.lib().seedrl_r2d2_epsilon_greedy(
+      int(actions.numel()), int(num_actions), _lib.ptr(env_ids_i32), _lib.ptr(envs_epsilon),
+      int(seed) & 0xFFFFFFFFFFFFFFFF, _lib.ptr(counter), _lib.ptr(actions), _lib.stream_ptr()))
 
 
 def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target_agent_output, env_outputs,

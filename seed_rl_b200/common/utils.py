@@ -162,9 +162,11 @@ class UnrollStore(object):
       return self._complete_unrolls_into(nc, into, on_placed)
     return self._complete_unrolls(nc)
 
-  def device_append(self, ids_i32, flat_values):
+  def device_append(self, ids_i32, flat_values, id_limit=None):
     """The device half of `append` (:187-194): every field of the step into its ring row (ONE
-    launch) + the index advance / completed-id compaction.  No host work: capturable in a CUDA graph."""
+    launch) + the index advance / completed-id compaction.  No host work: capturable in a CUDA graph.
+    id_limit: rows whose env id is >= id_limit are skipped (a fixed-size batch that also carries
+    environments the store has no rows for); feed `host_advance` only the ids below it."""
     L = _lib.lib()
     n = int(ids_i32.numel())
     st = _lib.stream_ptr()
@@ -175,16 +177,25 @@ class UnrollStore(object):
         raise ValueError('Batch dimension must equal the number of environments in store %s.'
                          % self.name)
       keep.append(v)
+    if id_limit is not None and len(keep) > 16:
+      raise ValueError('device_append with id_limit takes at most 16 fields (store %s has %d)'
+                       % (self.name, len(keep)))
     if n and len(keep) <= 16:
-      _lib.rows_multi([(s, v, _lib.ROW_APPEND) for s, v in zip(self._state, keep)], ids_i32, index=self._index)
+      _lib.rows_multi([(s, v, _lib.ROW_APPEND) for s, v in zip(self._state, keep)], ids_i32, index=self._index,
+                      id_limit=id_limit)
     else:
       for i, (s, v) in enumerate(zip(self._state, keep)):
         _lib.check(L.seedrl_store_append_field(
             _lib.ptr(s), _lib.ptr(self._index), _lib.ptr(ids_i32), n, self._full_length,
             self._row_bytes(i), _lib.ptr(v), st))
-    _lib.check(L.seedrl_store_advance(
-        _lib.ptr(self._index), _lib.ptr(ids_i32), n, self._full_length,
-        _lib.ptr(self._completed), _lib.ptr(self._ncomp), st))        # :194
+    if id_limit is None:
+      _lib.check(L.seedrl_store_advance(
+          _lib.ptr(self._index), _lib.ptr(ids_i32), n, self._full_length,
+          _lib.ptr(self._completed), _lib.ptr(self._ncomp), st))      # :194
+    else:
+      _lib.check(L.seedrl_store_advance_limit(
+          _lib.ptr(self._index), _lib.ptr(ids_i32), n, self._full_length,
+          _lib.ptr(self._completed), _lib.ptr(self._ncomp), int(id_limit), st))
 
   def host_advance(self, host_ids):
     """The host half: which of these environments complete an unroll with this step (a pure
@@ -196,6 +207,10 @@ class UnrollStore(object):
     done_host = hid[pos]
     self._host_index[done_host] = 1 + self._num_overlapping_steps     # :254-255
     return done_host, pos
+
+  def complete(self, nc):
+    """Gathers the `nc` unrolls completed by the last device_append: (completed env ids, unrolls)."""
+    return self._complete_unrolls(nc)
 
   def complete_into(self, nc, into, on_placed=None):
     """Gathers the `nc` unrolls completed by the last device_append into `into`."""

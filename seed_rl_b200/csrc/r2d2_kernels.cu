@@ -6,6 +6,8 @@
 //   replay_sample_kernel       common/utils.py:327-352    p_i ~ prio_i^alpha, inverse-CDF draw,
 //                              importance weights normalised by their max
 //   global-norm clip           tf.clip_by_global_norm, learner.py:608 (clip_norm = 40)
+//   r2d2_epsilon_greedy_kernel agents/r2d2/learner.py:155-177  epsilon-greedy on the device, Philox
+//                              offset from a device counter (CUDA-graph replays)
 //
 // Parity: tests/test_gpu_r2d2.py against oracle/r2d2_oracle.py / oracle/r2d2_learner_oracle.py (frame
 // stacking and replay indices bit-exact, loss / priorities / dq within fp32 rounding), on an H100.
@@ -104,6 +106,25 @@ __global__ void clip_scale_kernel(size_t n, float* __restrict__ g, const float* 
     g[i] *= sc;
 }
 
+// ---------------------------------------------------------------------------------------
+// Epsilon-greedy: row n draws r = philox4x32_10((counter lo, counter hi, n, 0), seed); it explores
+// iff (r.x >> 8) * 2^-24 < epsilon(env), with the uniform action (r.y * A) >> 32.  The formulas are
+// part of the interface: tests restate them in numpy bit for bit.
+__global__ void r2d2_epsilon_greedy_kernel(int N, int A, const int32_t* __restrict__ env_ids,
+                                           const float* __restrict__ envs_epsilon, uint64_t seed,
+                                           const uint64_t* __restrict__ counter, int32_t* __restrict__ actions) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  const uint64_t c = *counter;
+  const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)n, 0u),
+                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+  if ((float)(r.x >> 8) * 5.9604644775390625e-8f < envs_epsilon[env_ids[n]])
+    actions[n] = (int32_t)(((uint64_t)r.y * (uint64_t)A) >> 32);
+}
+
+// a separate one-thread launch, so that no block of the draw can see the incremented counter
+__global__ void r2d2_bump_counter_kernel(uint64_t* counter) { *counter += 1; }
+
 }  // namespace seedrl
 
 using namespace seedrl;
@@ -160,6 +181,24 @@ extern "C" int seedrl_replay_sample(int limit, const float* priorities, float pr
                                                             importance_sampling_exp, num_samples, uniforms,
                                                             indices, weights, probs_out);
   count_launch(PC_MISC, (cudaStream_t)stream);
+  SEEDRL_CHECK_LAUNCH();
+  return SEEDRL_OK;
+}
+
+extern "C" int seedrl_r2d2_epsilon_greedy(int N, int A, const int32_t* env_ids, const float* envs_epsilon,
+                                          uint64_t seed, uint64_t* counter_dev, int32_t* actions,
+                                          seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(N >= 0 && A >= 1, "need N >= 0, A >= 1");
+  SEEDRL_CHECK_ARG(env_ids && envs_epsilon && counter_dev && actions, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (N > 0) {
+    r2d2_epsilon_greedy_kernel<<<ceil_div(N, 128), 128, 0, st>>>(N, A, env_ids, envs_epsilon, seed, counter_dev,
+                                                                  actions);
+    count_launch(PC_MISC, st);
+    SEEDRL_CHECK_LAUNCH();
+  }
+  r2d2_bump_counter_kernel<<<1, 1, 0, st>>>(counter_dev);
+  count_launch(PC_MISC, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
 }

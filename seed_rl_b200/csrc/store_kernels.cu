@@ -33,11 +33,12 @@ __global__ void store_append_kernel(uint8_t* state, const int32_t* __restrict__ 
            row_bytes);
 }
 
-// index[env]++ ; completed ids compacted in env_ids order (utils.py:194,229-233).
+// index[env]++ ; completed ids compacted in env_ids order (utils.py:194,229-233).  Rows whose env id
+// is >= id_limit (eval environments, which have no store rows) are skipped.
 // Single CTA: n is an inference batch (<= a few thousand).
 __global__ void store_advance_kernel(int32_t* index, const int32_t* __restrict__ env_ids, int n,
                                      int full_length, int32_t* __restrict__ completed_ids,
-                                     int32_t* __restrict__ num_completed) {
+                                     int32_t* __restrict__ num_completed, int id_limit) {
   __shared__ int s_base;
   __shared__ int s_warp[32];
   if (threadIdx.x == 0) s_base = 0;
@@ -46,8 +47,7 @@ __global__ void store_advance_kernel(int32_t* index, const int32_t* __restrict__
   for (int j0 = 0; j0 < n; j0 += blockDim.x) {
     const int j = j0 + threadIdx.x;
     int flag = 0, env = 0;
-    if (j < n) {
-      env = env_ids[j];
+    if (j < n && (env = env_ids[j]) < id_limit) {
       const int v = index[env] + 1;
       index[env] = v;
       flag = (v == full_length);
@@ -114,10 +114,11 @@ __global__ void store_zero_rows_kernel(uint8_t* state, const int32_t* __restrict
 // agents/vtrace/learner.py:381-403): block (j, f) moves row j of job f.
 //   mode 0  gather   rows[j]  = table[env_ids[j]]                      (Aggregator.read, utils.py:504-516)
 //   mode 1  scatter  table[env_ids[j]] = rows[j]                       (Aggregator.replace, :519-543)
-//   mode 2  append   table[env_ids[j], index[env_ids[j]]] = rows[j]    (UnrollStore.append, :187-190)
+//   mode 2  append   table[env_ids[j], index[env_ids[j]]] = rows[j]    (UnrollStore.append, :187-190),
+//                    skipped for env ids >= id_limit
 struct RowJobs { seedrl_row_job job[SEEDRL_MAX_ROW_JOBS]; };
 __global__ void rows_multi_kernel(const __grid_constant__ RowJobs t, const int32_t* __restrict__ env_ids,
-                                  const int32_t* __restrict__ index) {
+                                  const int32_t* __restrict__ index, int id_limit) {
   const seedrl_row_job jb = t.job[blockIdx.y];
   const int j = blockIdx.x;
   const int env = env_ids[j];
@@ -128,6 +129,7 @@ __global__ void rows_multi_kernel(const __grid_constant__ RowJobs t, const int32
   } else if (jb.mode == 1) {
     copy_row(table + (size_t)env * jb.row_bytes, rows + (size_t)j * jb.row_bytes, jb.row_bytes);
   } else {
+    if (env >= id_limit) return;
     const int ti = index[env];
     if (ti < 0 || ti >= jb.full_length) return;
     copy_row(table + ((size_t)env * jb.full_length + ti) * jb.row_bytes, rows + (size_t)j * jb.row_bytes,
@@ -139,20 +141,26 @@ __global__ void rows_multi_kernel(const __grid_constant__ RowJobs t, const int32
 
 using namespace seedrl;
 
-extern "C" int seedrl_rows_multi(const seedrl_row_job* jobs, int njobs, const int32_t* env_ids, int n,
-                                 const int32_t* index, seedrl_stream_t stream) {
+extern "C" int seedrl_rows_multi_limit(const seedrl_row_job* jobs, int njobs, const int32_t* env_ids, int n,
+                                       const int32_t* index, int32_t id_limit, seedrl_stream_t stream) {
   if (n == 0 || njobs == 0) return SEEDRL_OK;
   SEEDRL_CHECK_ARG(jobs && env_ids && n > 0 && njobs > 0 && njobs <= SEEDRL_MAX_ROW_JOBS, "bad argument");
+  SEEDRL_CHECK_ARG(id_limit >= 0, "id_limit must be >= 0");
   RowJobs t;
   for (int i = 0; i < njobs; ++i) {
     SEEDRL_CHECK_ARG(jobs[i].table && jobs[i].rows && jobs[i].mode >= 0 && jobs[i].mode <= 2, "bad job");
     SEEDRL_CHECK_ARG(jobs[i].mode != 2 || (index && jobs[i].full_length > 0), "append job needs index");
     t.job[i] = jobs[i];
   }
-  rows_multi_kernel<<<dim3(n, njobs), 128, 0, (cudaStream_t)stream>>>(t, env_ids, index);
+  rows_multi_kernel<<<dim3(n, njobs), 128, 0, (cudaStream_t)stream>>>(t, env_ids, index, id_limit);
   count_launch(PC_MISC, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
+}
+
+extern "C" int seedrl_rows_multi(const seedrl_row_job* jobs, int njobs, const int32_t* env_ids, int n,
+                                 const int32_t* index, seedrl_stream_t stream) {
+  return seedrl_rows_multi_limit(jobs, njobs, env_ids, n, index, INT32_MAX, stream);
 }
 
 extern "C" int seedrl_store_append_field(uint8_t* state, const int32_t* index, const int32_t* env_ids,
@@ -168,15 +176,23 @@ extern "C" int seedrl_store_append_field(uint8_t* state, const int32_t* index, c
   return SEEDRL_OK;
 }
 
-extern "C" int seedrl_store_advance(int32_t* index, const int32_t* env_ids, int n, int full_length,
-                                    int32_t* completed_ids, int32_t* num_completed,
-                                    seedrl_stream_t stream) {
+extern "C" int seedrl_store_advance_limit(int32_t* index, const int32_t* env_ids, int n, int full_length,
+                                          int32_t* completed_ids, int32_t* num_completed, int32_t id_limit,
+                                          seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(index && env_ids && completed_ids && num_completed && n >= 0, "bad argument");
+  SEEDRL_CHECK_ARG(id_limit >= 0, "id_limit must be >= 0");
   store_advance_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(index, env_ids, n, full_length,
-                                                            completed_ids, num_completed);
+                                                            completed_ids, num_completed, id_limit);
   count_launch(PC_MISC, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
+}
+
+extern "C" int seedrl_store_advance(int32_t* index, const int32_t* env_ids, int n, int full_length,
+                                    int32_t* completed_ids, int32_t* num_completed,
+                                    seedrl_stream_t stream) {
+  return seedrl_store_advance_limit(index, env_ids, n, full_length, completed_ids, num_completed, INT32_MAX,
+                                    stream);
 }
 
 extern "C" int seedrl_store_gather_field(uint8_t* state, const int32_t* completed_ids,

@@ -101,21 +101,8 @@ __global__ void categorical_logprob_entropy_kernel(int N, int A, const float* __
   }
 }
 
-// Philox4x32-10 (Salmon et al. 2011), counter = (offset, row, block-of-4, 0).
-__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
-  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-  for (int i = 0; i < 10; ++i) {
-    const uint32_t hi0 = __umulhi(M0, ctr.x), lo0 = M0 * ctr.x;
-    const uint32_t hi1 = __umulhi(M1, ctr.z), lo1 = M1 * ctr.z;
-    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-    key.x += W0;
-    key.y += W1;
-  }
-  return ctr;
-}
-
-// one thread per row (A is small); first max wins ties like np.argmax.
+// one thread per row (A is small); first max wins ties like np.argmax.  Philox counter =
+// (offset lo, offset hi, row, block of 4 actions), key = seed (philox4x32_10, common.cuh).
 __global__ void categorical_sample_kernel(int N, int A, const float* __restrict__ logits,
                                           const float* __restrict__ noise, uint64_t seed,
                                           uint64_t offset, const uint64_t* __restrict__ offset_dev,
