@@ -18,11 +18,10 @@ import time
 
 from absl import flags
 from absl import logging
-import numpy as np
 import torch
 
-from seed_rl_b200 import _lib
 from seed_rl_b200.agents.vtrace import learner as learner_lib
+from seed_rl_b200.common import inference_host
 from seed_rl_b200.common import utils
 from seed_rl_b200.common.parametric_distribution import get_parametric_distribution_for_action_space
 from seed_rl_b200.dmlab import networks
@@ -32,8 +31,10 @@ FLAGS = flags.FLAGS
 Unroll = learner_lib.Unroll
 
 
-class InferenceHost(object):
+class InferenceHost(inference_host.InferenceHostBase):
   """Everything `create_host` builds in the reference (learner.py:314-413) for one GPU."""
+
+  algorithm = 'VTRACE'
 
   def __init__(self, agent, num_envs, unroll_length, inference_batch_size, obs_shape,
                num_action_repeats=1, device='cuda', info_queue=None, training_batch_size=None,
@@ -41,238 +42,46 @@ class InferenceHost(object):
     """training_batch_size: when given, completed unrolls are gathered straight into the columns
     of preallocated time-major training batches (`self.assembler`, utils.BatchAssembler: zero-copy
     minibatch assembly); otherwise they go through the reference's capacity-1 `unroll_queue` of
-    single unrolls and `dequeue_batch` stacks them."""
-    self.agent = agent
-    self.device = torch.device(device)
-    self.N = inference_batch_size
-    self.num_action_repeats = num_action_repeats
+    single unrolls and `dequeue_batch` stacks them.  cuda_graph: replay the device side of every
+    full batch as one CUDA graph (default: with the assembler); it needs the assembler."""
     TS = utils.TensorSpec
-    self.env_output_specs = utils.EnvOutput(
-        TS([], 'float32', 'reward'), TS([], 'bool', 'done'),
-        TS(list(obs_shape), 'uint8', 'observation'), TS([], 'bool', 'abandoned'),
-        TS([], 'int32', 'episode_step'))
-    action_specs = TS([], 'int64', 'action')
-    A = agent._num_actions
     agent_output_specs = networks.AgentOutput(
-        TS([], 'int64', 'action'), TS([A], 'float32', 'policy_logits'), TS([], 'float32', 'baseline'))
+        TS([], 'int64', 'action'), TS([agent._num_actions], 'float32', 'policy_logits'),
+        TS([], 'float32', 'baseline'))
     agent_state_specs = (TS([networks.LSTM_UNITS], 'float32', 'h'), TS([networks.LSTM_UNITS], 'float32', 'c'))
+    # CUDA-graph replay of the device side of a full inference batch: gather -> T=1 forward ->
+    # sample -> write-back -> store append are ~40 small dependent launches whose CPU issue cost,
+    # not their GPU time, bounded the step.
+    use_graph = bool(training_batch_size) and (cuda_graph is None or bool(cuda_graph))
     # time_major=True: completed unrolls come out as [T+1, n, ...] (no make_time_major pass)
-    self.store = utils.UnrollStore(num_envs, unroll_length,
-                                   (action_specs, self.env_output_specs, agent_output_specs),
-                                   device=device, time_major=True)
-    # run ids / episode stats feed host-side logging only -> host tables (learner.py:321-324)
-    self.env_run_ids = np.zeros([num_envs], np.int64)
-    self.env_infos = [np.zeros([num_envs], np.int64), np.zeros([num_envs], np.float32),
-                      np.zeros([num_envs], np.float32)]
-    self.first_agent_states = utils.Aggregator(num_envs, agent_state_specs, 'first_agent_states', device)
-    self.agent_states = utils.Aggregator(num_envs, agent_state_specs, 'agent_states', device)
-    self.actions = utils.Aggregator(num_envs, action_specs, 'actions', device)
+    super(InferenceHost, self).__init__(
+        agent, num_envs, inference_batch_size, obs_shape, 'int64', agent_state_specs, agent_output_specs,
+        unroll_length, time_major=True, num_action_repeats=num_action_repeats, device=device,
+        info_queue=info_queue, use_graph=use_graph)
     self.unroll_specs = Unroll(agent_state_specs, *self.store.unroll_specs)
     self.unroll_queue = utils.StructuredFIFOQueue(1, self.unroll_specs)      # capacity 1, :336
     self.assembler = None
     if training_batch_size:
-      self.assembler = utils.BatchAssembler((action_specs, self.env_output_specs, agent_output_specs),
-                                            agent_state_specs, unroll_length + 1, training_batch_size,
-                                            slots=2, device=device)
-    self.info_queue = info_queue
-    N = self.N
-    self.inference_specs = (
-        TS([N], 'int32', 'env_id'), TS([N], 'int64', 'run_id'),
-        utils.map_structure(lambda s: TS([N] + list(s.shape), s.dtype, s.name), self.env_output_specs),
-        TS([N], 'float32', 'raw_reward'))
-    self.output_specs = TS([N], 'int64', 'action')
-    self.stream = torch.cuda.Stream(device=self.device) if self.device.type == 'cuda' else None
-    # CUDA-graph replay of the device side of a full inference batch (default with the assembler):
-    # gather -> T=1 forward -> sample -> write-back -> store append are ~40 small dependent launches
-    # whose CPU issue cost, not their GPU time, bounded the step.
-    self.use_graph = bool(cuda_graph if cuda_graph is not None else (self.assembler is not None))
-    self._graph = None
+      self.assembler = utils.BatchAssembler(self.store._specs, agent_state_specs, unroll_length + 1,
+                                            training_batch_size, slots=2, device=device)
 
-    @grpc.function(self.inference_specs, self.output_specs)
-    def inference(env_ids, run_ids, env_outputs, raw_rewards):
-      return self._inference(env_ids, run_ids, env_outputs, raw_rewards)
-    self.inference = inference
+  def _policy(self, ids32, prev_actions, env_outputs, prev_states, counter):
+    return self.agent(prev_actions, env_outputs, prev_states, is_training=False, rng_counter=counter)
 
-  # ---- CUDA-graph path ---------------------------------------------------------------------------
-  def _device_step(self, ids32, env_dev, rng_counter):
-    """Everything of one inference batch that runs on the device (learner.py:381-403), on static
-    buffers: captured once, replayed per batch."""
-    n = int(ids32.numel())
-    prev_actions = torch.empty([n], dtype=torch.int64, device=self.device)
-    prev_states = tuple(torch.empty([n, networks.LSTM_UNITS], dtype=torch.float32, device=self.device)
-                        for _ in range(2))
-    _lib.rows_multi([(self.actions._state[0], prev_actions, _lib.ROW_GATHER),
-                     (self.agent_states._state[0], prev_states[0], _lib.ROW_GATHER),
-                     (self.agent_states._state[1], prev_states[1], _lib.ROW_GATHER)], ids32)
-    agent_outputs, curr_states = self.agent(prev_actions, env_dev, prev_states, is_training=False,
-                                            rng_counter=rng_counter)
-    self.store.device_append(ids32, utils.flatten((prev_actions, env_dev, agent_outputs)))
-    _lib.rows_multi([(self.agent_states._state[0], curr_states[0].contiguous(), _lib.ROW_SCATTER),
-                     (self.agent_states._state[1], curr_states[1].contiguous(), _lib.ROW_SCATTER),
-                     (self.actions._state[0], agent_outputs.action.contiguous(), _lib.ROW_SCATTER)], ids32)
-    return prev_states, agent_outputs
+  def _completed_unrolls(self, nc):
+    """Into the next columns of the assembler, or (:394-399) one queue item per unroll."""
+    if self.assembler is None:
+      completed_ids, unrolls = self.store.complete(nc)
+      first = self.first_agent_states.read(completed_ids)
+      # [T+1, nc, ...] -> [nc, T+1, ...]: the queue splits the batch along dim 0 into single unrolls
+      return completed_ids, Unroll(first, *utils.map_structure(lambda t: t.transpose(0, 1), unrolls))
 
-  def _build_graph(self):
-    N, dev = self.N, self.device
-    dt = utils.as_torch_dtype
-    self._g_ids = torch.zeros([N], dtype=torch.int32, device=dev)
-    self._g_env = utils.EnvOutput(*(torch.zeros([N] + list(s.shape), dtype=dt(s.dtype), device=dev)
-                                    for s in self.env_output_specs))
-    self._g_pin = [torch.zeros_like(t, device='cpu').pin_memory() for t in (self._g_ids,) + tuple(self._g_env)]
-    self._g_counter = torch.zeros([], dtype=torch.int64, device=dev)
-    with torch.cuda.stream(self.stream):
-      self._g_ids.copy_(torch.arange(N, dtype=torch.int32))       # distinct ids for the warm-up / capture
-      # warm-up on scratch copies of the mutable tables is not needed: the capture run below does
-      # not execute, and the one eager warm-up is undone by restoring the tables it touches
-      saved = [t.clone() for t in self.actions._state + self.agent_states._state + self.store._state] + \
-              [self.store._index.clone()]
-      self._device_step(self._g_ids, self._g_env, self._g_counter)   # eager: lazy inits (func attributes, workspaces)
-      for t, sv in zip(self.actions._state + self.agent_states._state + self.store._state + [self.store._index], saved):
-        t.copy_(sv)
-      self._g_counter.zero_()
-      self.stream.synchronize()
-      g = torch.cuda.CUDAGraph()
-      # thread_local: the learner thread may allocate / launch on its own stream during the capture
-      with torch.cuda.graph(g, stream=self.stream, capture_error_mode='thread_local'):
-        self._g_prev_states, self._g_out = self._device_step(self._g_ids, self._g_env, self._g_counter)
-      self._g_actions_pin = torch.zeros([N], dtype=torch.int64).pin_memory()
-    self._graph = g
-
-  def _inference_graph(self, env_ids, run_ids, env_outputs, raw_rewards):
-    """reference learner.py:351-405 with the device side as one graph replay."""
-    reward, done = np.asarray(env_outputs.reward), np.asarray(env_outputs.done)
-    previous = self.env_run_ids[env_ids]
-    self.env_run_ids[env_ids] = run_ids
-    reset_ids = env_ids[previous != run_ids]
-    if np.asarray(env_outputs.abandoned).any():                         # :368-370
-      raise ValueError('Abandoned done states are not supported in VTRACE.')
-    utils._check_no_duplicates(None, env_ids, 'inference batch')
-    with torch.cuda.stream(self.stream):
-      if self._graph is None:
-        self._build_graph()
-      if reset_ids.size:                                                # :353-366 (rare: eager)
-        logging.info('Environment ids needing reset: %s', reset_ids)
-        for t in self.env_infos:
-          t[reset_ids] = 0
-        self.store.reset(reset_ids)
-        init = self.agent.initial_state(len(reset_ids))
-        self.first_agent_states.replace(reset_ids, init)
-        self.agent_states.replace(reset_ids, init)
-        self.actions.reset(reset_ids)
-      self.env_infos[1][env_ids] += reward                              # :373-378
-      self.env_infos[2][env_ids] += np.asarray(raw_rewards)
-      done_ids = env_ids[done]
-      if self.info_queue is not None and done_ids.size:
-        self.info_queue.enqueue_many(tuple(torch.as_tensor(t[done_ids]) for t in self.env_infos))
-      for t in self.env_infos:
-        t[done_ids] = 0
-      self.env_infos[0][env_ids] += self.num_action_repeats
-      # inputs: host arrays -> pinned staging -> the graph's static device buffers
-      srcs = (env_ids.astype(np.int32),) + tuple(np.asarray(x) for x in env_outputs)
-      for pin, dst, src in zip(self._g_pin, (self._g_ids,) + tuple(self._g_env), srcs):
-        t = torch.from_numpy(np.ascontiguousarray(src))
-        if t.numel() >= 65536 and t.is_pinned():
-          dst.copy_(t, non_blocking=True)        # the batcher's slabs are pinned: DMA straight from them
-        else:
-          pin.numpy()[...] = src                 # small fields / pageable memory: own pinned staging
-          dst.copy_(pin, non_blocking=True)
-      self._graph.replay()
-      # completed unrolls (known on the host) -> columns of the training batch; first agent states
-      done_host, pos = self.store.host_advance(env_ids)
-      if done_host.size:
-        pos_dev = torch.as_tensor(pos.astype(np.int64)).to(self.device, non_blocking=True)
-        def on_placed(slot, col0, ids):
-          first = self.first_agent_states.read(ids.to(torch.int64))
-          for dst, src in zip(self.assembler._states[slot], first):
-            dst[col0:col0 + int(ids.numel())].copy_(src)
-        completed_ids, _ = self.store.complete_into(int(done_host.size), self.assembler, on_placed)
-        # the state the next unroll starts from = the state this step started from (:400-401)
-        self.first_agent_states.replace(completed_ids, tuple(s.index_select(0, pos_dev) for s in self._g_prev_states),
-                                        check_unique=False)
-      self._g_actions_pin.copy_(self._g_out.action, non_blocking=True)
-      self.stream.synchronize()
-    return self._g_actions_pin.numpy().copy()
-
-  def _inference(self, env_ids, run_ids, env_outputs, raw_rewards):
-    """reference learner.py:351-405."""
-    env_ids = np.asarray(env_ids); run_ids = np.asarray(run_ids)
-    if self.use_graph and self.assembler is not None and len(env_ids) == self.N:
-      return self._inference_graph(env_ids, run_ids, env_outputs, raw_rewards)
-    reward, done = np.asarray(env_outputs.reward), np.asarray(env_outputs.done)
-    # Reset the environments that had their first run or crashed (:353-366).
-    previous = self.env_run_ids[env_ids]
-    self.env_run_ids[env_ids] = run_ids
-    reset_ids = env_ids[previous != run_ids]
-    with torch.cuda.stream(self.stream):
-      if reset_ids.size:
-        logging.info('Environment ids needing reset: %s', reset_ids)
-        for t in self.env_infos:
-          t[reset_ids] = 0
-        self.store.reset(reset_ids)
-        init = self.agent.initial_state(len(reset_ids))
-        self.first_agent_states.replace(reset_ids, init)
-        self.agent_states.replace(reset_ids, init)
-        self.actions.reset(reset_ids)
-      if np.asarray(env_outputs.abandoned).any():                       # :368-370
-        raise ValueError('Abandoned done states are not supported in VTRACE.')
-      # Update steps and return (:373-378).
-      self.env_infos[1][env_ids] += reward
-      self.env_infos[2][env_ids] += np.asarray(raw_rewards)
-      done_ids = env_ids[done]
-      if self.info_queue is not None and done_ids.size:
-        self.info_queue.enqueue_many(tuple(torch.as_tensor(t[done_ids]) for t in self.env_infos))
-      for t in self.env_infos:
-        t[done_ids] = 0
-      self.env_infos[0][env_ids] += self.num_action_repeats
-      # Inference (:381-390): one H2D copy per field, T=1 forward on the GPU.
-      ids_dev = torch.as_tensor(env_ids.astype(np.int64)).to(self.device, non_blocking=True)
-      ids32 = ids_dev.to(torch.int32)
-      env_dev = utils.EnvOutput(*(torch.as_tensor(np.asarray(x)).to(self.device, non_blocking=True)
-                                  for x in env_outputs))
-      # previous action + recurrent state of these environments: ONE gather launch (:381-383)
-      n = int(ids32.numel())
-      prev_actions = torch.empty([n], dtype=torch.int64, device=self.device)
-      prev_states = tuple(torch.empty([n, networks.LSTM_UNITS], dtype=torch.float32, device=self.device)
-                          for _ in range(2))
-      _lib.rows_multi([(self.actions._state[0], prev_actions, _lib.ROW_GATHER),
-                       (self.agent_states._state[0], prev_states[0], _lib.ROW_GATHER),
-                       (self.agent_states._state[1], prev_states[1], _lib.ROW_GATHER)], ids32)
-      agent_outputs, curr_states = self.agent(prev_actions, env_dev, prev_states, is_training=False)
-      # Append to the unroll store, enqueue completed unrolls (:394-399).
-      pending = []
-      if self.assembler is not None:
-        def on_placed(slot, col0, ids):
-          first = self.first_agent_states.read(ids.to(torch.int64))
-          for dst, src in zip(self.assembler._states[slot], first):
-            dst[col0:col0 + int(ids.numel())].copy_(src)
-        completed_ids, placed = self.store.append(env_ids, (prev_actions, env_dev, agent_outputs),
-                                                  check_duplicates=True, into=self.assembler,
-                                                  on_placed=on_placed)
-        n_done = 0
-        if placed:
-          self.first_agent_states.replace(completed_ids, self.agent_states.read(completed_ids), check_unique=False)
-      else:
-        completed_ids, unrolls = self.store.append(env_ids, (prev_actions, env_dev, agent_outputs),
-                                                   check_duplicates=True)
-        n_done = int(completed_ids.numel())
-      if n_done:
-        first = self.first_agent_states.read(completed_ids)
-        flat = utils.flatten(unrolls)
-        for i in range(n_done):     # one queue element per unroll, as in the reference
-          u = utils.pack_sequence_as(self.store._specs, [f[:, i] for f in flat])
-          pending.append(Unroll((first[0][i], first[1][i]), *u))
-        self.first_agent_states.replace(completed_ids, self.agent_states.read(completed_ids), check_unique=False)
-      # Update current state (:402-403) and return the actions (:405).
-      # (ids are unique: UnrollStore.append checked them)  ONE scatter launch
-      _lib.rows_multi([(self.agent_states._state[0], curr_states[0].contiguous(), _lib.ROW_SCATTER),
-                       (self.agent_states._state[1], curr_states[1].contiguous(), _lib.ROW_SCATTER),
-                       (self.actions._state[0], agent_outputs.action.contiguous(), _lib.ROW_SCATTER)], ids32)
-      out = agent_outputs.action.cpu()       # D2H + sync of this stream
-    # The unrolls were produced on self.stream, which the blocking copy above has drained: only
-    # now are they handed to the learner thread (which consumes them on another stream).
-    for u in pending:
-      self.unroll_queue.enqueue(u)
-    return out.numpy()
+    def on_placed(slot, col0, ids):
+      first = self.first_agent_states.read(ids.to(torch.int64))
+      for dst, src in zip(self.assembler._states[slot], first):
+        dst[col0:col0 + int(ids.numel())].copy_(src)
+    completed_ids, _ = self.store.complete_into(nc, self.assembler, on_placed)
+    return completed_ids, None
 
 
 def dequeue_batch(unroll_queue, batch_size):

@@ -145,9 +145,8 @@ class UnrollStore(object):
     s = self._state[i]
     return int(s[0, 0].numel()) * s.element_size()
 
-  def append(self, env_ids, values, check_duplicates=True, into=None, on_placed=None):
-    """Appends values; returns (completed env ids int64 [n], completed unrolls) -- or, with
-    `into` (a BatchAssembler), (completed env ids, [(slot, first column, count)])."""
+  def append(self, env_ids, values, check_duplicates=True):
+    """Appends values; returns (completed env ids int64 [n], completed unrolls)."""
     ids, host = _ids_to_device(env_ids, self._device)
     if check_duplicates:
       _check_no_duplicates(ids, host, 'store %s' % self.name)
@@ -158,9 +157,7 @@ class UnrollStore(object):
       nc = int(self.host_advance(host)[0].size)
     else:
       self._host_index = None          # ids live on the device only: fall back to reading the counter
-    if into is not None:
-      return self._complete_unrolls_into(nc, into, on_placed)
-    return self._complete_unrolls(nc)
+    return self.complete(nc)
 
   def device_append(self, ids_i32, flat_values, id_limit=None):
     """The device half of `append` (:187-194): every field of the step into its ring row (ONE
@@ -208,21 +205,32 @@ class UnrollStore(object):
     self._host_index[done_host] = 1 + self._num_overlapping_steps     # :254-255
     return done_host, pos
 
-  def complete(self, nc):
+  def complete(self, nc=None):
     """Gathers the `nc` unrolls completed by the last device_append: (completed env ids, unrolls)."""
-    return self._complete_unrolls(nc)
-
-  def complete_into(self, nc, into, on_placed=None):
-    """Gathers the `nc` unrolls completed by the last device_append into `into`."""
-    return self._complete_unrolls_into(nc, into, on_placed)
-
-  def _complete_unrolls_into(self, nc, into, on_placed=None):
-    """Gathers the completed unrolls straight into free columns of `into` (a BatchAssembler): no
-    per-unroll tensors, no stack, no transpose.  Returns (completed env ids, [(slot, col0, n)])."""
     L = _lib.lib()
     st = _lib.stream_ptr()
     if nc is None:
-      nc = int(self._ncomp.item())
+      nc = int(self._ncomp.item())      # device-resident ids: the one host sync that sizes the outputs
+    done_ids = self._completed[:nc]
+    unrolls = []
+    for i, s in enumerate(self._state):
+      tail = list(s.shape[2:])
+      shape = ([self._full_length, nc] if self._time_major else [nc, self._full_length]) + tail
+      u = torch.empty(shape, dtype=s.dtype, device=self._device)
+      _lib.check(L.seedrl_store_gather_field(
+          _lib.ptr(s), _lib.ptr(done_ids), nc, self._full_length, self._row_bytes(i),
+          self._num_overlapping_steps, 1 if self._time_major else 0, _lib.ptr(u), st))
+      unrolls.append(u)
+    _lib.check(L.seedrl_store_finish(_lib.ptr(self._index), _lib.ptr(done_ids), nc,
+                                     self._num_overlapping_steps, st))
+    return done_ids.to(torch.int64), pack_sequence_as(self._specs, unrolls)
+
+  def complete_into(self, nc, into, on_placed=None):
+    """Gathers the `nc` unrolls completed by the last device_append straight into free columns of
+    `into` (a BatchAssembler): no per-unroll tensors, no stack, no transpose.  Returns (completed
+    env ids, [(slot, col0, n)])."""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
     done_ids = self._completed[:nc]
     placed, start = [], 0
     while start < nc:
@@ -241,25 +249,6 @@ class UnrollStore(object):
     _lib.check(L.seedrl_store_finish(_lib.ptr(self._index), _lib.ptr(done_ids), nc,
                                      self._num_overlapping_steps, st))
     return done_ids.to(torch.int64), placed
-
-  def _complete_unrolls(self, nc=None):
-    L = _lib.lib()
-    st = _lib.stream_ptr()
-    if nc is None:
-      nc = int(self._ncomp.item())      # device-resident ids: the one host sync that sizes the outputs
-    done_ids = self._completed[:nc]
-    unrolls = []
-    for i, s in enumerate(self._state):
-      tail = list(s.shape[2:])
-      shape = ([self._full_length, nc] if self._time_major else [nc, self._full_length]) + tail
-      u = torch.empty(shape, dtype=s.dtype, device=self._device)
-      _lib.check(L.seedrl_store_gather_field(
-          _lib.ptr(s), _lib.ptr(done_ids), nc, self._full_length, self._row_bytes(i),
-          self._num_overlapping_steps, 1 if self._time_major else 0, _lib.ptr(u), st))
-      unrolls.append(u)
-    _lib.check(L.seedrl_store_finish(_lib.ptr(self._index), _lib.ptr(done_ids), nc,
-                                     self._num_overlapping_steps, st))
-    return done_ids.to(torch.int64), pack_sequence_as(self._specs, unrolls)
 
   def reset(self, env_ids):
     """Reset after actor preemption (reference utils.py:198-225)."""
@@ -283,7 +272,7 @@ class UnrollStore(object):
 class BatchAssembler(object):
   """Zero-copy minibatch assembly (SURVEY 8(f) rank 2).  Holds `slots` preallocated time-major
   training batches ([T+1, B, ...] per field of the unroll specs, plus the [B, ...] first agent
-  states); the inference thread's UnrollStore.append(..., into=self) gathers every completed
+  states); the inference thread's UnrollStore.complete_into(nc, self) gathers every completed
   unroll straight into the next free column.  A full slot is handed to the learner (`get`), which
   returns it with `release(slot)` once its step is enqueued.  Replaces the reference's
   capacity-1 queue of single unrolls + tf.stack + make_time_major (agents/vtrace/learner.py:336,
