@@ -537,6 +537,23 @@ int seedrl_debug_strided_conv(int op, int mode, int gather, int in_u8, int N, in
                               const float* dy, const float* mask, float* out, int ldo, float* dbias,
                               float* col, size_t col_bytes, float* ws, size_t ws_bytes, int* error_flag,
                               int* gathered, seedrl_stream_t stream);
+/* The LSTM recurrence alone, making exactly the calls the networks make (csrc/lstm.cu
+ * lstm_recurrence_forward / _backward): Keras LSTMCell(H), H = 256 or 512, with done-resets, over T1 steps.
+ * mode is the network's lstm_mode: 0 per-step GEMM + pointwise kernels, H = 256 only (gemm_mode 0: fp32 SIMT
+ * GEMM, 2: bf16x3 wgmma GEMM; modes 1-3 ignore it), 1 persistent, 2 tiled, 3 tiled on wgmma bf16x3.
+ *   forward:  z [T1,B,4H] holds x W + b on entry and the activated gates (i,f,g,o) on exit; hs, cs, hp [T1,B,H]
+ *             (hp[t] = h[t-1] with step t's resets applied); h0, c0 [B,H]; U [H,4H]; done [T1,B].
+ *   backward: dz [T1,B,4H] = d loss / d(x W + b) from the forward's gates and cs and dhs = d loss / d hs.
+ * ws: seedrl_debug_lstm_workspace_bytes(mode, H, T1, B) bytes.  *error_flag is set (never cleared) when a
+ * bounded barrier wait expires.  An H other than 256 / 512 (256 in mode 0) or a batch the mode cannot take
+ * returns SEEDRL_ERR_INVALID_ARGUMENT with nothing launched. */
+size_t seedrl_debug_lstm_workspace_bytes(int mode, int H, int T1, int B);
+int seedrl_debug_lstm_forward(int mode, int gemm_mode, int H, int T1, int B, const float* U, const uint8_t* done,
+                              float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
+                              void* ws, size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
+int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, const float* U, const uint8_t* done,
+                               const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
+                               void* ws, size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
 
 /* ---- plane-tensor convolution path (conv_mode 3) test hooks: single kernels of
  * csrc/conv_planes.cu, so the GPU parity tests can localise a failure.  Not on the product path. */

@@ -189,6 +189,11 @@ SIGNATURES = {
     'seedrl_debug_strided_conv':
         (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P,
                  c_int, P, P, c_size_t, P, c_size_t, P, ctypes.POINTER(c_int), P]),
+    'seedrl_debug_lstm_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'seedrl_debug_lstm_forward':
+        (c_int, [c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P, P]),
+    'seedrl_debug_lstm_backward':
+        (c_int, [c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, c_size_t, P, P]),
 }
 
 _lib = None

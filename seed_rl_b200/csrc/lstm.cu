@@ -1,0 +1,118 @@
+// The LSTM recurrence of one network call, in each lstm_mode: the one place that dispatches on the mode
+// (net.cu and r2d2_net.cu call it), and its C-ABI test hook, which makes the same calls.
+#include "schedule.h"
+
+namespace seedrl {
+
+int lstm_recurrence_forward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
+                            float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
+                            unsigned int* counter) {
+  cudaStream_t st = ex.st;
+  // one kernel for the whole recurrence, CTA = (batch tile, 16 units) (lstm_tiled.cu)
+  if (mode == 2) return lstm_forward_tiled(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
+  // the same recurrence with the recurrent products on the tensor cores (lstm_tc.cu)
+  if (mode == 3) return lstm_forward_tc(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
+  // one cooperative kernel for the whole recurrence (lstm_persistent.cu)
+  if (mode == 1) return lstm_forward_persistent(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
+  // mode 0: per step, z[t] += hp[t] U on the caller's GEMM, then the pointwise cell update
+  SEEDRL_TRY(lstm_mask_state(B, H, done, h0, hp, st));
+  GemmEpi eacc = epi_none();
+  eacc.accumulate = 1;
+  for (int t = 0; t < T1; ++t) {
+    float* zt = z + (size_t)t * B * 4 * H;
+    SEEDRL_TRY(ex.gemm(false, false, B, 4 * H, H, hp + (size_t)t * B * H, H, U, 4 * H, zt, 4 * H, eacc));
+    const bool last = (t + 1 == T1);
+    SEEDRL_TRY(lstm_pointwise_fwd(B, H, zt, t == 0 ? c0 : cs + (size_t)(t - 1) * B * H, done + (size_t)t * B,
+                                  last ? nullptr : done + (size_t)(t + 1) * B, cs + (size_t)t * B * H,
+                                  hs + (size_t)t * B * H, last ? nullptr : hp + (size_t)(t + 1) * B * H, st));
+  }
+  return SEEDRL_OK;
+}
+
+int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
+                             const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
+                             float* dhrec, float* const dc[2], unsigned int* counter) {
+  cudaStream_t st = ex.st;
+  if (mode == 2) return lstm_backward_tiled(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
+  if (mode == 3) return lstm_backward_tc(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
+  if (mode == 1) return lstm_backward_persistent(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
+  SEEDRL_CHECK_ARG(dhrec && dc && dc[0] && dc[1], "lstm mode 0: the BPTT needs dh_rec and two dc buffers");
+  for (int t = T1 - 1; t >= 0; --t) {
+    const bool last = (t + 1 == T1);
+    const size_t o = (size_t)t * B * H;
+    SEEDRL_TRY(lstm_pointwise_bwd(B, H, gates + (size_t)t * B * 4 * H, cs + o, t == 0 ? c0 : cs + o - (size_t)B * H,
+                                  done + (size_t)t * B, last ? nullptr : done + (size_t)(t + 1) * B, dhs + o,
+                                  last ? nullptr : dhrec, last ? nullptr : dc[(t + 1) & 1],
+                                  dz + (size_t)t * B * 4 * H, dc[t & 1], st));
+    if (t > 0)
+      SEEDRL_TRY(ex.gemm(false, true, B, H, 4 * H, dz + (size_t)t * B * 4 * H, 4 * H, U, 4 * H, dhrec, H,
+                         epi_none()));
+  }
+  return SEEDRL_OK;
+}
+
+// Workspace of the test hook: the barrier counters, then (mode 0) dh_rec, the two dc buffers and the
+// GEMM's split-K partials.
+struct DebugLstmPlan {
+  size_t counter, dhrec, dc[2], gemm_ws, total;
+};
+static DebugLstmPlan debug_lstm_plan(int mode, int H, int B) {
+  DebugLstmPlan p;
+  Bump b;
+  p.counter = b.take(256);
+  p.dhrec = p.dc[0] = p.dc[1] = p.gemm_ws = 0;
+  if (mode == 0) {
+    p.dhrec = b.take((size_t)B * H * 4);
+    p.dc[0] = b.take((size_t)B * H * 4);
+    p.dc[1] = b.take((size_t)B * H * 4);
+    p.gemm_ws = b.take(gemm_tc_workspace_bytes());
+  }
+  p.total = b.off;
+  return p;
+}
+
+}  // namespace seedrl
+
+using namespace seedrl;
+
+extern "C" size_t seedrl_debug_lstm_workspace_bytes(int mode, int H, int T1, int B) {
+  if (mode < 0 || mode > 3 || H < 1 || T1 < 1 || B < 1) return 0;
+  return debug_lstm_plan(mode, H, B).total;
+}
+
+// A batch a mode cannot take is refused by its launcher, before anything is launched.
+static int debug_lstm_check(int mode, int gemm_mode, int H, int T1, int B, size_t ws_bytes) {
+  SEEDRL_CHECK_ARG(mode >= 0 && mode <= 3, "lstm mode must be 0..3");
+  SEEDRL_CHECK_ARG(gemm_mode == 0 || gemm_mode == 2, "gemm_mode must be 0 (fp32 SIMT) or 2 (wgmma bf16x3)");
+  SEEDRL_CHECK_ARG(H == 256 || H == 512, "lstm: hidden size must be 256 or 512");
+  SEEDRL_CHECK_ARG(mode != 0 || H == 256, "lstm mode 0 runs at H = 256 only (the IMPALA core)");
+  SEEDRL_CHECK_ARG(T1 >= 1 && B >= 1 && (size_t)T1 * B * 4 * H < ((size_t)1 << 31), "bad T1 / B");
+  SEEDRL_CHECK_ARG(ws_bytes >= debug_lstm_plan(mode, H, B).total, "workspace too small");
+  return SEEDRL_OK;
+}
+
+extern "C" int seedrl_debug_lstm_forward(int mode, int gemm_mode, int H, int T1, int B, const float* U,
+                                         const uint8_t* done, float* z, const float* h0, const float* c0, float* hs,
+                                         float* cs, float* hp, void* ws, size_t ws_bytes, int* error_flag,
+                                         seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(U && done && z && h0 && c0 && hs && cs && hp && ws && error_flag, "null pointer");
+  SEEDRL_TRY(debug_lstm_check(mode, gemm_mode, H, T1, B, ws_bytes));
+  const DebugLstmPlan pl = debug_lstm_plan(mode, H, B);
+  const GemmExec ex{gemm_mode, false, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes(), error_flag,
+                    (cudaStream_t)stream};
+  return lstm_recurrence_forward(mode, ex, H, T1, B, U, done, z, h0, c0, hs, cs, hp, W<unsigned int>(ws, pl.counter));
+}
+
+extern "C" int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, const float* U,
+                                          const uint8_t* done, const float* gates, const float* cs, const float* c0,
+                                          const float* dhs, float* dz, void* ws, size_t ws_bytes, int* error_flag,
+                                          seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(U && done && gates && cs && c0 && dhs && dz && ws && error_flag, "null pointer");
+  SEEDRL_TRY(debug_lstm_check(mode, gemm_mode, H, T1, B, ws_bytes));
+  const DebugLstmPlan pl = debug_lstm_plan(mode, H, B);
+  const GemmExec ex{gemm_mode, false, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes(), error_flag,
+                    (cudaStream_t)stream};
+  float* const dc[2] = {W<float>(ws, pl.dc[0]), W<float>(ws, pl.dc[1])};
+  return lstm_recurrence_backward(mode, ex, H, T1, B, U, done, gates, cs, c0, dhs, dz, W<float>(ws, pl.dhrec), dc,
+                                  W<unsigned int>(ws, pl.counter));
+}

@@ -576,33 +576,8 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   SEEDRL_TRY(c.ex.gemm(false, false, N, 4 * kHidden, CI, xc, CI, c.P(n->p_core_w), 4 * kHidden, z,
                    4 * kHidden, e));
   SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)B * kHidden * 4, cudaMemcpyDeviceToDevice, st));
-  GemmEpi eacc = epi_none();
-  eacc.accumulate = 1;
-  if (n->lstm_mode == 2) {
-    // one kernel for the whole recurrence, CTA = (batch tile, 16 units) (lstm_tiled.cu)
-    SEEDRL_TRY(lstm_forward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                                  W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  } else if (n->lstm_mode == 3) {
-    // the same recurrence with the recurrent products on the tensor cores (lstm_tc.cu)
-    SEEDRL_TRY(lstm_forward_tc(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                               W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  } else if (n->lstm_mode == 1) {
-    // one cooperative kernel for the whole recurrence (lstm_persistent.cu)
-    SEEDRL_TRY(lstm_forward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                                       W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  } else {
-    SEEDRL_TRY(lstm_mask_state(B, kHidden, done, h0, hp, st));
-  }
-  for (int t = 0; t < T1 && n->lstm_mode == 0; ++t) {
-    float* zt = z + (size_t)t * B * 4 * kHidden;
-    SEEDRL_TRY(c.ex.gemm(false, false, B, 4 * kHidden, kHidden, hp + (size_t)t * B * kHidden, kHidden,
-                     c.P(n->p_core_u), 4 * kHidden, zt, 4 * kHidden, eacc));
-    const bool last = (t + 1 == T1);
-    SEEDRL_TRY(lstm_pointwise_fwd(B, kHidden, zt, t == 0 ? c0buf : cs + (size_t)(t - 1) * B * kHidden,
-                                  done + (size_t)t * B, last ? nullptr : done + (size_t)(t + 1) * B,
-                                  cs + (size_t)t * B * kHidden, hs + (size_t)t * B * kHidden,
-                                  last ? nullptr : hp + (size_t)(t + 1) * B * kHidden, st));
-  }
+  SEEDRL_TRY(lstm_recurrence_forward(n->lstm_mode, c.ex, kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs,
+                                     cs, hp, W<unsigned int>(ws, pl.counter)));
   // heads, networks.py:116-118
   e = epi_none();
   e.bias = c.P(n->p_pol_b);
@@ -794,27 +769,8 @@ static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, co
   SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, 1, dbaseline, 1, c.P(n->p_base_w), 1, dhs, kHidden,
                    eacc));
   // BPTT
-  if (n->lstm_mode == 2)
-    SEEDRL_TRY(lstm_backward_tiled(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                   W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  if (n->lstm_mode == 3)
-    SEEDRL_TRY(lstm_backward_tc(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  if (n->lstm_mode == 1)
-    SEEDRL_TRY(lstm_backward_persistent(kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                        W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  for (int t = T1 - 1; t >= 0 && n->lstm_mode == 0; --t) {
-    const bool last = (t + 1 == T1);
-    const size_t o = (size_t)t * B * kHidden;
-    SEEDRL_TRY(lstm_pointwise_bwd(B, kHidden, z + (size_t)t * B * 4 * kHidden, cs + o,
-                                  t == 0 ? c0buf : cs + o - (size_t)B * kHidden, done + (size_t)t * B,
-                                  last ? nullptr : done + (size_t)(t + 1) * B, dhs + o,
-                                  last ? nullptr : dhrec, last ? nullptr : dcb[(t + 1) & 1],
-                                  dz + (size_t)t * B * 4 * kHidden, dcb[t & 1], st));
-    if (t > 0)
-      SEEDRL_TRY(c.ex.gemm(false, true, B, kHidden, 4 * kHidden, dz + (size_t)t * B * 4 * kHidden,
-                       4 * kHidden, c.P(n->p_core_u), 4 * kHidden, dhrec, kHidden, e));
-  }
+  SEEDRL_TRY(lstm_recurrence_backward(n->lstm_mode, c.ex, kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs,
+                                      dz, dhrec, dcb, W<unsigned int>(ws, pl.counter)));
   SEEDRL_TRY(c.ex.gemm(true, false, kHidden, 4 * kHidden, N, hp, kHidden, dz, 4 * kHidden,
                    c.G(n->p_core_u), 4 * kHidden, e));
   SEEDRL_TRY(c.ex.gemm(true, false, CI, 4 * kHidden, N, xc, CI, dz, 4 * kHidden, c.G(n->p_core_w),

@@ -247,15 +247,8 @@ extern "C" int seedrl_r2d2_net_forward(const seedrl_r2d2_net* n, const float* pr
   e.bias = RP(n, prm, n->p_core_b);
   SEEDRL_TRY(ex.gemm(false, false, N, 4 * kRH, CI, xc, CI, RP(n, prm, n->p_core_w), 4 * kRH, z, 4 * kRH, e));
   SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)B * kRH * 4, cudaMemcpyDeviceToDevice, st));
-  if (n->lstm_mode == 2)
-    SEEDRL_TRY(lstm_forward_tiled(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                                  W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  else if (n->lstm_mode == 3)
-    SEEDRL_TRY(lstm_forward_tc(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                               W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  else
-    SEEDRL_TRY(lstm_forward_persistent(kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs, hp,
-                                       W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  SEEDRL_TRY(lstm_recurrence_forward(n->lstm_mode, ex, kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs,
+                                     hp, W<unsigned int>(ws, pl.counter)));
   // dueling heads
   float* vh = W<float>(ws, pl.vh); float* ah = W<float>(ws, pl.ah);
   float* v = W<float>(ws, pl.v); float* adv = W<float>(ws, pl.adv);
@@ -323,16 +316,9 @@ extern "C" int seedrl_r2d2_net_backward(const seedrl_r2d2_net* n, const float* p
   // d core output
   SEEDRL_TRY(ex.gemm(false, true, N, kRH, 512, dah, 512, RP(n, prm, n->p_ah_w), 512, dhs, kRH, e0));
   SEEDRL_TRY(ex.gemm(false, true, N, kRH, 512, dvh, 512, RP(n, prm, n->p_vh_w), 512, dhs, kRH, eacc));
-  // BPTT
-  if (n->lstm_mode == 2)
-    SEEDRL_TRY(lstm_backward_tiled(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                   W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  else if (n->lstm_mode == 3)
-    SEEDRL_TRY(lstm_backward_tc(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
-  else
-    SEEDRL_TRY(lstm_backward_persistent(kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs, dz,
-                                        W<unsigned int>(ws, pl.counter), W<int>(ws, pl.tcerr), st));
+  // BPTT (lstm_mode is 1..3 here, so no per-step scratch)
+  SEEDRL_TRY(lstm_recurrence_backward(n->lstm_mode, ex, kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs,
+                                      dz, nullptr, nullptr, W<unsigned int>(ws, pl.counter)));
   SEEDRL_TRY(ex.gemm(true, false, kRH, 4 * kRH, N, hp, kRH, dz, 4 * kRH, RG(n, grd, n->p_core_u), 4 * kRH, e0));
   SEEDRL_TRY(ex.gemm(true, false, CI, 4 * kRH, N, xc, CI, dz, 4 * kRH, RG(n, grd, n->p_core_w), 4 * kRH, e0));
   SEEDRL_TRY(ex.colsum(N, 4 * kRH, dz, 4 * kRH, RG(n, grd, n->p_core_b)));

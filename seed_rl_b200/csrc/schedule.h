@@ -95,6 +95,21 @@ struct GemmExec {
   }
 };
 
+// The LSTM recurrence of one call (lstm.cu), Keras LSTMCell(H) with done-resets over T1 steps, in lstm_mode
+// `mode`: 0 per-step launches (z[t] += hp[t] U and dh_rec = dZ[t] U^T on ex's GEMM, pointwise kernels),
+// 1 persistent (lstm_persistent.cu), 2 tiled (lstm_tiled.cu), 3 tiled on wgmma bf16x3 (lstm_tc.cu).
+//   forward   z [T1,B,4H]: x W + b in, activated gates out; hs, cs, hp [T1,B,H] (hp[t] = h[t-1] with step t's
+//             resets applied)
+//   backward  dz [T1,B,4H] from the forward's gates and cs and dhs [T1,B,H]; mode 0 also takes dh_rec [B,H] and
+//             two dc buffers [B,H] as scratch
+// counter: 64 barrier counters (256 B), reset by each launch; ex.err: the bounded-wait error flag.
+int lstm_recurrence_forward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
+                            float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
+                            unsigned int* counter);
+int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
+                             const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
+                             float* dhrec, float* const dc[2], unsigned int* counter);
+
 // Reads back the device-side error flag of the last forward/backward that used a workspace (set when
 // a bounded mbarrier / grid-barrier wait of a wgmma or persistent kernel expired, i.e. the results are
 // garbage).  Synchronises `st`.  `unit` names what the results belong to ("step", "unroll").
