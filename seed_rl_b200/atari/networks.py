@@ -11,13 +11,11 @@ All math runs in libseedrl_b200 (seedrl_r2d2_stack_frames, seedrl_r2d2_net_forwa
 _backward: csrc/r2d2_kernels.cu, csrc/r2d2_net.cu)."""
 import collections
 import ctypes
-import math
-import threading
 
-import numpy as np
 import torch
 
 from seed_rl_b200 import _lib
+from seed_rl_b200.common.cuda_net import CudaNet
 
 AgentOutput = collections.namedtuple('AgentOutput', 'action q_values')
 AgentState = collections.namedtuple('AgentState', 'core_state frame_stacking_state')
@@ -69,11 +67,12 @@ def stack_frames(frames, frame_stacking_state, done, stack_size):
   return out, new_state
 
 
-class DuelingLSTMDQNNet(object):
+class DuelingLSTMDQNNet(CudaNet):
   """reference atari/networks.py:221-340.  Conv 8x8/4 -> 32, 4x4/2 -> 64, 3x3/1 -> 64 ('valid',
   ReLU), Dense(512, ReLU), concat(reward, one_hot(prev_action)), LSTMCell(512) with done-resets,
   dueling value / advantage heads, greedy action.  Parameters live in one flat fp32 HBM arena
   (Keras layouts, tf.Module variable order)."""
+  _LIB = 'seedrl_r2d2_net'
 
   def __init__(self, num_actions, observation_shape, stack_size=1, seed=0, device=None, gemm_mode='tc3',
                lstm_mode='tiled'):
@@ -106,60 +105,13 @@ class DuelingLSTMDQNNet(object):
       raise ValueError("lstm_mode must be 'tiled', 'tc3' (the tiled recurrence on wgmma bf16x3) or 'persistent'")
     self.lstm_mode = lstm_mode
     _lib.check(L.seedrl_r2d2_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
-    self._n_tensors = L.seedrl_r2d2_net_num_param_tensors(h)
-    self.arena_floats = int(L.seedrl_r2d2_net_arena_floats(h))
-    self.num_params = int(L.seedrl_r2d2_net_num_params(h))
-    self.param_info = []
-    for i in range(self._n_tensors):
-      name = ctypes.create_string_buffer(128)
-      dims = (ctypes.c_int64 * 4)()
-      rank = ctypes.c_int()
-      off = ctypes.c_size_t()
-      _lib.check(L.seedrl_r2d2_net_param_info(h, i, name, 128, dims, ctypes.byref(rank), ctypes.byref(off)))
-      self.param_info.append((name.value.decode(), tuple(int(dims[k]) for k in range(rank.value)), int(off.value)))
-    self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
-    self.params = torch.zeros(self.arena_floats, dtype=torch.float32, device=self.device)
-    self.grads = torch.zeros_like(self.params)
-    self._init_parameters(seed)
-    self._workspaces = {}
-    self._lock = threading.Lock()
-    self._saved = None
+    self._setup(seed, device)
 
-  def __del__(self):
-    try:
-      if getattr(self, '_h', None):
-        _lib.lib().seedrl_r2d2_net_destroy(self._h)
-        self._h = None
-    except Exception:   # interpreter shutdown
-      pass
-
-  # ---- parameters ---------------------------------------------------------------
-  def _view(self, arena, i):
-    _, shape, off = self.param_info[i]
-    n = int(np.prod(shape)) if shape else 1
-    return arena[off:off + n].view(shape if shape else ())
-
-  @property
-  def trainable_variables(self):
-    return [self._view(self.params, i) for i in range(self._n_tensors)]
-
-  @property
-  def variable_names(self):
-    return [p[0] for p in self.param_info]
-
-  def named_parameters(self):
-    return collections.OrderedDict((self.param_info[i][0], self._view(self.params, i)) for i in range(self._n_tensors))
-
-  def named_gradients(self):
-    return collections.OrderedDict((self.param_info[i][0], self._view(self.grads, i)) for i in range(self._n_tensors))
-
-  def load_named_parameters(self, named):
-    mine = self.named_parameters()
-    for k, v in named.items():
-      t = torch.as_tensor(np.asarray(v, np.float32))
-      if tuple(t.shape) != tuple(mine[k].shape):
-        raise ValueError('shape mismatch for %s: %s vs %s' % (k, tuple(t.shape), tuple(mine[k].shape)))
-      mine[k].copy_(t)
+  def _param_rank(self, index, name_buf, dims, offset):
+    rank = ctypes.c_int()
+    _lib.check(_lib.lib().seedrl_r2d2_net_param_info(self._h, index, name_buf, len(name_buf), dims,
+                                                     ctypes.byref(rank), ctypes.byref(offset)))
+    return rank.value
 
   def assign_from(self, other):
     """update_target_agent (agents/r2d2/learner.py:535-544): target_var.assign(source_var)."""
@@ -167,47 +119,12 @@ class DuelingLSTMDQNNet(object):
       raise ValueError('Mismatch in number of net tensors')
     self.params.copy_(other.params)
 
-  def _init_parameters(self, seed):
-    """Keras defaults (TF 2.4.1): glorot_uniform kernels, zero biases, orthogonal recurrent
-    kernel, unit_forget_bias."""
-    rng = np.random.default_rng(seed)
-    for i in range(self._n_tensors):
-      name, shape, _ = self.param_info[i]
-      if name.endswith('bias'):
-        a = np.zeros(shape, np.float32)
-        if name == 'core/bias':
-          a[LSTM_UNITS:2 * LSTM_UNITS] = 1.0
-      elif name == 'core/recurrent_kernel':
-        q, r = np.linalg.qr(rng.normal(size=(shape[1], shape[0])))
-        a = (q * np.sign(np.diag(r))).T.astype(np.float32)
-      else:
-        rf = int(np.prod(shape[:-2])) if len(shape) > 2 else 1
-        lim = math.sqrt(6.0 / (shape[-2] * rf + shape[-1] * rf))
-        a = rng.uniform(-lim, lim, shape).astype(np.float32)
-      self._view(self.params, i).copy_(torch.from_numpy(a))
-
   # ---- protocol ---------------------------------------------------------------
   def initial_state(self, batch_size):
     z = torch.zeros([batch_size, LSTM_UNITS], dtype=torch.float32, device=self.device)
     return AgentState(core_state=(z, z.clone()),
                       frame_stacking_state=initial_frame_stacking_state(
                           self._stack_size, batch_size, self._observation_shape, device=self.device))
-
-  def _workspace(self, T, B):
-    key = (T, B, threading.get_ident())
-    with self._lock:
-      ws = self._workspaces.get(key)
-      if ws is None:
-        nbytes = int(_lib.lib().seedrl_r2d2_net_workspace_bytes(self._h, T, B))
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        self._workspaces[key] = ws
-    return ws
-
-  def check_errors(self):
-    if self._saved is None:
-      return
-    T, B, _, ws, _ = self._saved
-    _lib.check(_lib.lib().seedrl_r2d2_net_check_error(self._h, T, B, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()))
 
   def __call__(self, input_, agent_state, unroll=False, is_training=False):
     prev_actions, env_outputs = input_
@@ -229,13 +146,13 @@ class DuelingLSTMDQNNet(object):
     action = torch.empty([T, B], dtype=torch.int32, device=self.device)
     h = torch.empty_like(h0)
     c = torch.empty_like(c0)
-    ws = self._workspace(T, B)
+    ws = self.workspace(T, B)
     _lib.check(_lib.lib().seedrl_r2d2_net_forward(
         self._h, _lib.ptr(self.params), T, B, _lib.ptr(prev_actions), _lib.ptr(reward), _lib.ptr(done),
         _lib.ptr(stacked), _lib.ptr(h0), _lib.ptr(c0), _lib.ptr(q), _lib.ptr(action), _lib.ptr(h), _lib.ptr(c),
         _lib.ptr(ws), ws.numel(), _lib.stream_ptr()))
     if is_training:
-      self._saved = (T, B, done, ws, stacked)
+      self._saved = (T, B, ws, done, stacked)
     out = AgentOutput(action, q)
     if not unroll:
       out = AgentOutput(*(t.squeeze(0) for t in out))
@@ -245,7 +162,7 @@ class DuelingLSTMDQNNet(object):
     """d loss / d parameters of the last is_training unroll -> self.grads (overwritten)."""
     if self._saved is None:
       raise RuntimeError('backward() needs a preceding __call__(..., unroll=True, is_training=True)')
-    T, B, done, ws, stacked = self._saved
+    T, B, ws, done, stacked = self._saved
     dq = _lib.require_cuda(dq, torch.float32, 'dq')
     if tuple(dq.shape) != (T, B, self._num_actions):
       raise ValueError('dq must be [T, B, num_actions] of the training unroll')
@@ -253,9 +170,3 @@ class DuelingLSTMDQNNet(object):
         self._h, _lib.ptr(self.params), T, B, _lib.ptr(stacked), _lib.ptr(done), _lib.ptr(dq), _lib.ptr(self.grads),
         _lib.ptr(ws), ws.numel(), _lib.stream_ptr()))
     return self.grads
-
-  def state_dict(self):
-    return {'params': self.params.detach().cpu(), 'param_info': self.param_info}
-
-  def load_state_dict(self, d):
-    self.params.copy_(d['params'].to(self.device))

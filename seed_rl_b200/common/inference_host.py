@@ -150,6 +150,9 @@ class InferenceHostBase(object):
     # thread_local: other threads (the learner, other hosts) may launch on their streams meanwhile
     with torch.cuda.graph(g, stream=self.stream, capture_error_mode='thread_local'):
       self._g_prev_states, self._g_out = self._device_step(self._g_ids, self._g_env, self._g_counter)
+    # the agent's (1, N) workspace the graph captured: eager batches of other sizes may evict it from the
+    # agent's cache, and every replay still writes into it
+    self._g_workspace = self.agent.workspace(1, N)
     self._graph = g
 
   def _inference(self, env_ids, run_ids, env_outputs, raw_rewards):

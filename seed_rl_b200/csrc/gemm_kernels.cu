@@ -238,31 +238,6 @@ int colsum(int M, int N, const float* X, int ld, float* out, cudaStream_t st, fl
 }
 
 // ---------------------------------------------------------------------------
-// torso tail, dmlab/networks.py:111-114: core_in[n] = concat(dense_out[n] (256, already
-// relu'd), clip(reward[n], -1, 1), one_hot(prev_action[n], A)).
-__global__ void core_input_tail_kernel(int Nrows, int D, int A, const float* __restrict__ reward,
-                                       const int64_t* __restrict__ prev_action,
-                                       float* __restrict__ core_in /* [N, D+1+A] */) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int W = 1 + A;
-  if (i >= Nrows * W) return;
-  const int n = i / W, j = i - n * W;
-  float v;
-  if (j == 0) v = fminf(fmaxf(reward[n], -1.f), 1.f);
-  else v = (prev_action[n] == (int64_t)(j - 1)) ? 1.f : 0.f;
-  core_in[(size_t)n * (D + W) + D + j] = v;
-}
-
-int core_input_tail(int Nrows, int D, int A, const float* reward, const int64_t* prev_action,
-                    float* core_in, cudaStream_t st) {
-  const int n = Nrows * (1 + A);
-  core_input_tail_kernel<<<ceil_div(n, 256), 256, 0, st>>>(Nrows, D, A, reward, prev_action, core_in);
-  count_launch(PC_MISC, st);
-  SEEDRL_CHECK_LAUNCH();
-  return SEEDRL_OK;
-}
-
-// ---------------------------------------------------------------------------
 // LSTM.  Keras LSTMCell: z = x W + h U + b (gate order i,f,c,o), c' = s(f) c + s(i) tanh(g),
 // h' = s(o) tanh(c').  dmlab/networks.py:160-167: state is reset to zero where done[t]
 // BEFORE consuming step t.

@@ -199,8 +199,6 @@ bool gemm_tc_gather_enabled();
 int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, int lda, const float* B,
             int ldb, float* C, int ldc, const GemmEpi& e, float* ws, size_t ws_bytes, int* err,
             cudaStream_t st, const ConvGather* cg = nullptr);
-int core_input_tail(int Nrows, int D, int A, const float* reward, const int64_t* prev_action,
-                    float* core_in, cudaStream_t st);
 int lstm_mask_state(int B, int Hd, const uint8_t* done, const float* h_src, float* h_dst,
                     cudaStream_t st);
 int lstm_pointwise_fwd(int B, int Hd, float* z, const float* c_prev_src, const uint8_t* done_t,

@@ -51,6 +51,123 @@ int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B,
   return SEEDRL_OK;
 }
 
+// ---- the recurrent core of both nets ---------------------------------------------------------
+Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu,
+                 bool stepwise) {
+  Core k;
+  k.H = H; k.flat = flat; k.A = A; k.core_in = H + 1 + A;
+  k.clip_reward = clip_reward; k.flat_relu = flat_relu; k.stepwise = stepwise;
+  k.dense_w = t.add(dense + "/kernel", {flat, H});
+  k.dense_b = t.add(dense + "/bias", {H});
+  k.w = t.add("core/kernel", {k.core_in, 4 * H});
+  k.u = t.add("core/recurrent_kernel", {H, 4 * H});
+  k.b = t.add("core/bias", {4 * H});
+  return k;
+}
+
+CorePlan core_plan(const Core& k, Bump& b, int T1, int B) {
+  CorePlan p;
+  p.T1 = T1; p.B = B; p.N = T1 * B;
+  const size_t N = (size_t)p.N, H = (size_t)k.H, BH = (size_t)B * H * 4;
+  p.xc = b.take(N * k.core_in * 4);
+  p.z = b.take(N * 4 * H * 4);
+  p.hp = b.take(N * H * 4);
+  p.cs = b.take(N * H * 4);
+  p.hs = b.take(N * H * 4);
+  p.c0buf = b.take(BH);
+  p.dhs = b.take(N * H * 4);
+  p.dz = b.take(N * 4 * H * 4);
+  p.dhrec = p.dc[0] = p.dc[1] = 0;
+  if (k.stepwise) {
+    p.dhrec = b.take(BH);
+    p.dc[0] = b.take(BH);
+    p.dc[1] = b.take(BH);
+  }
+  p.dd = b.take(N * H * 4);
+  p.counter = b.take(256);
+  return p;
+}
+
+// core_in[n] = concat(dense_out[n] (D columns, already written), reward[n] (clipped to [-1, 1] if `clip`),
+// one_hot(prev_action[n], A))
+__global__ void core_input_tail_kernel(int Nrows, int D, int A, bool clip, const float* __restrict__ reward,
+                                       const int64_t* __restrict__ prev_action, float* __restrict__ core_in) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int Wd = 1 + A;
+  if (i >= Nrows * Wd) return;
+  const int n = i / Wd, j = i - n * Wd;
+  float v;
+  if (j == 0) v = clip ? fminf(fmaxf(reward[n], -1.f), 1.f) : reward[n];
+  else v = prev_action[n] == (int64_t)(j - 1) ? 1.f : 0.f;
+  core_in[(size_t)n * (D + Wd) + D + j] = v;
+}
+
+int core_forward(const Core& k, const ParamTable& t, const CorePlan& p, const GemmExec& ex, void* ws, const float* prm,
+                 const float* flat, const float* reward, const int64_t* prev_actions, const uint8_t* done,
+                 const float* h0, const float* c0) {
+  cudaStream_t st = ex.st;
+  const int N = p.N, H = k.H, CI = k.core_in;
+  float* xc = W<float>(ws, p.xc);
+  float* z = W<float>(ws, p.z);
+  float* c0buf = W<float>(ws, p.c0buf);
+  // Dense + ReLU written straight into the first H columns of the core input
+  GemmEpi e = epi_none();
+  e.bias = prm + t.offset(k.dense_b); e.relu = 1; e.a_relu = k.flat_relu;
+  SEEDRL_TRY(ex.gemm(false, false, N, H, k.flat, flat, k.flat, prm + t.offset(k.dense_w), H, xc, CI, e));
+  core_input_tail_kernel<<<ceil_div(N * (1 + k.A), 256), 256, 0, st>>>(N, H, k.A, k.clip_reward, reward,
+                                                                       prev_actions, xc);
+  count_launch(PC_MISC, st);
+  SEEDRL_CHECK_LAUNCH();
+  // input projection for all T at once: z = xc W + b
+  e = epi_none();
+  e.bias = prm + t.offset(k.b);
+  SEEDRL_TRY(ex.gemm(false, false, N, 4 * H, CI, xc, CI, prm + t.offset(k.w), 4 * H, z, 4 * H, e));
+  SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)p.B * H * 4, cudaMemcpyDeviceToDevice, st));
+  return lstm_recurrence_forward(k.lstm_mode, ex, H, p.T1, p.B, prm + t.offset(k.u), done, z, h0, c0buf,
+                                 W<float>(ws, p.hs), W<float>(ws, p.cs), W<float>(ws, p.hp),
+                                 W<unsigned int>(ws, p.counter));
+}
+
+int core_final_state(const Core& k, const CorePlan& p, cudaStream_t st, void* ws, float* h_out, float* c_out) {
+  const size_t last = (size_t)(p.T1 - 1) * p.B * k.H, bytes = (size_t)p.B * k.H * 4;
+  if (h_out)
+    SEEDRL_CUDA(cudaMemcpyAsync(h_out, W<float>(ws, p.hs) + last, bytes, cudaMemcpyDeviceToDevice, st));
+  if (c_out)
+    SEEDRL_CUDA(cudaMemcpyAsync(c_out, W<float>(ws, p.cs) + last, bytes, cudaMemcpyDeviceToDevice, st));
+  return SEEDRL_OK;
+}
+
+int core_backward(const Core& k, const ParamTable& t, const CorePlan& p, const GemmExec& ex, void* ws,
+                  const float* prm, float* grd, const uint8_t* done, const float* flat, float* dflat,
+                  cudaEvent_t head_ready) {
+  const int N = p.N, H = k.H, CI = k.core_in;
+  const float* xc = W<float>(ws, p.xc);
+  float* dz = W<float>(ws, p.dz);
+  float* dd = W<float>(ws, p.dd);
+  float* const dc[2] = {W<float>(ws, p.dc[0]), W<float>(ws, p.dc[1])};
+  const GemmEpi e = epi_none();
+  // BPTT (mode 0 needs the stepwise scratch; a net without it gets an error, not a crash)
+  SEEDRL_TRY(lstm_recurrence_backward(k.lstm_mode, ex, H, p.T1, p.B, prm + t.offset(k.u), done, W<float>(ws, p.z),
+                                      W<float>(ws, p.cs), W<float>(ws, p.c0buf), W<float>(ws, p.dhs), dz,
+                                      k.stepwise ? W<float>(ws, p.dhrec) : nullptr, k.stepwise ? dc : nullptr,
+                                      W<unsigned int>(ws, p.counter)));
+  SEEDRL_TRY(ex.gemm(true, false, H, 4 * H, N, W<float>(ws, p.hp), H, dz, 4 * H, grd + t.offset(k.u), 4 * H, e));
+  SEEDRL_TRY(ex.gemm(true, false, CI, 4 * H, N, xc, CI, dz, 4 * H, grd + t.offset(k.w), 4 * H, e));
+  SEEDRL_TRY(ex.colsum(N, 4 * H, dz, 4 * H, grd + t.offset(k.b)));
+  // d dense_out = (dz W[:H,:]^T) * (dense_out > 0)
+  GemmEpi em = epi_none();
+  em.mask = xc; em.ldm = CI;
+  SEEDRL_TRY(ex.gemm(false, true, N, H, 4 * H, dz, 4 * H, prm + t.offset(k.w), 4 * H, dd, H, em));
+  // Dense
+  GemmEpi ea = epi_none();
+  ea.a_relu = k.flat_relu;
+  SEEDRL_TRY(ex.gemm(true, false, k.flat, H, N, flat, k.flat, dd, H, grd + t.offset(k.dense_w), H, ea));
+  SEEDRL_TRY(ex.colsum(N, H, dd, H, grd + t.offset(k.dense_b)));
+  if (head_ready) SEEDRL_CUDA(cudaEventRecord(head_ready, ex.st));
+  em.mask = flat; em.ldm = k.flat;
+  return ex.gemm(false, true, N, k.flat, H, dd, H, prm + t.offset(k.dense_w), H, dflat, k.flat, em);
+}
+
 // Workspace of the test hook: the barrier counters, then (mode 0) dh_rec, the two dc buffers and the
 // GEMM's split-K partials.
 struct DebugLstmPlan {

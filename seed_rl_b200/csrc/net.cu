@@ -29,15 +29,12 @@ struct seedrl_net {
   seedrl_net_config cfg;
   seedrl::ParamTable params;               // network tensors, then entropy_cost_param
   size_t logical_params;
-  int p_base_w, p_base_b, p_dense_w, p_dense_b, p_core_w, p_core_u, p_core_b, p_pol_w, p_pol_b;
+  int p_base_w, p_base_b, p_pol_w, p_pol_b;
+  seedrl::Core core;                       // Dense(256) + LSTM(256); lstm_mode 0..3 (schedule.h)
   std::vector<seedrl::Stack> stacks;       // deep
   seedrl::StridedConv sh[2];               // shallow: conv 8x8/4 -> 16, conv 4x4/2 -> 32
   int sh_w[2], sh_b[2];                    // their param indices
-  int flat;                                // conv features fed to Dense(256)
-  int lstm_mode = 2;                       // 2 = tiled persistent kernels (lstm_tiled.cu), 1 = first persistent form, 0 = per-step launches,
-                                           // 3 = tiled on wgmma bf16x3 (lstm_tc.cu)
   int conv_mode = 0;                       // 0 = fp32 SIMT, 1 = wgmma bf16, 2 = wgmma bf16x3 (fp32-faithful)
-  int core_in;                             // 256 + 1 + A
 };
 
 namespace seedrl {
@@ -68,9 +65,9 @@ struct Plan {
   std::vector<StackBufs> st;
   size_t sh_a1, sh_a2;         // shallow conv outputs (post-relu)
   size_t sh_col0, sh_col1;     // shallow net, tensor-core modes: im2col matrices (kept for the backward)
-  size_t xc, z, hp, cs, hs, c0buf;
+  CorePlan core;
   // backward scratch
-  size_t dhs, dz, dhrec, dc0, dc1, dd, gA, gB, gC, gFull, wt, partial, wq, tcerr, counter, gemm_ws, wq_all, partial_all;
+  size_t gA, gB, gC, gFull, wt, partial, wq, tcerr, gemm_ws, wq_all, partial_all;
   size_t gP1, gP2, gP3, gFP;   // conv_mode 3: plane-tensor gradients (pooled resolution x3, full resolution)
   size_t obs4, w0pad, dw0pad;  // 3-channel frames: zero-padded frames / first-conv weights / their gradient
   size_t total;
@@ -125,18 +122,7 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
     pooled_max = a1 > a2 ? a1 : a2;
     full_max = 0;
   }
-  p.xc = b.take(N * n->core_in * 4);
-  p.z = b.take(N * 4 * kHidden * 4);
-  p.hp = b.take(N * kHidden * 4);
-  p.cs = b.take(N * kHidden * 4);
-  p.hs = b.take(N * kHidden * 4);
-  p.c0buf = b.take((size_t)B * kHidden * 4);
-  p.dhs = b.take(N * kHidden * 4);
-  p.dz = b.take(N * 4 * kHidden * 4);
-  p.dhrec = b.take((size_t)B * kHidden * 4);
-  p.dc0 = b.take((size_t)B * kHidden * 4);
-  p.dc1 = b.take((size_t)B * kHidden * 4);
-  p.dd = b.take(N * kHidden * 4);
+  p.core = core_plan(n->core, b, T1, B);
   p.obs4 = p.w0pad = p.dw0pad = 0;
   if (n->cfg.net == SEEDRL_NET_DEEP && n->cfg.obs_c == 3) {
     p.obs4 = b.take(N * n->cfg.obs_h * n->cfg.obs_w * 4);
@@ -161,16 +147,20 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
   p.wq_all = b.take((size_t)kMaxPackJobs * kPackSlotBytes);
   p.partial_all = b.take(kPartialAllBytes);
   p.tcerr = b.take(256);
-  p.counter = b.take(256);
   p.partial = b.take(conv3x3_wgrad_partial_bytes());
   p.total = b.off;
   return p;
 }
 
+// The torso's output, the flat features Dense(256) reads (the deep net's is ReLU'd as it is read).
+static const float* flat_features(const seedrl_net* n, const Plan& pl, void* ws) {
+  return W<float>(ws, n->cfg.net == SEEDRL_NET_DEEP ? pl.st.back().o1 : pl.sh_a2);
+}
+
 // State of one forward or backward call, passed down the schedule: the GEMM execution, the weights
-// pre-packed for this call, the deferred weight-gradient reductions, the head-ready event, and for
-// 3-channel frames the zero-padded first-conv weights and their gradient (pad_first_layer), which
-// stand in for that one parameter in P() / G().
+// pre-packed for this call, the deferred weight-gradient reductions, and for 3-channel frames the
+// zero-padded first-conv weights and their gradient (pad_first_layer), which stand in for that one
+// parameter in P() / G().
 struct Call {
   const seedrl_net* n;
   const Plan& pl;
@@ -180,7 +170,6 @@ struct Call {
   GemmExec ex;
   PackTable packed;
   WgradBatch wb;
-  cudaEvent_t head_ready = nullptr;  // recorded when the gradients of the first arena bucket are final
   int w0_index = -1;
   const float* w0_pad = nullptr;
   float* dw0_pad = nullptr;
@@ -318,7 +307,6 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
   seedrl_net* n = new seedrl_net();
   n->cfg = *cfg;
   const int A = cfg->num_actions;
-  n->core_in = kHidden + 1 + A;
   // tf.Module order: _baseline, _conv_to_linear, _core, _policy_logits, _stacks
   n->p_base_w = n->params.add("baseline/kernel", {kHidden, 1});
   n->p_base_b = n->params.add("baseline/bias", {1});
@@ -338,12 +326,9 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
     n->sh[1] = StridedConv(4, 2, 16, 32, n->sh[0].hout, n->sh[0].wout);
     flat = n->sh[1].hout * n->sh[1].wout * 32;
   }
-  n->flat = flat;
-  n->p_dense_w = n->params.add("conv_to_linear/kernel", {flat, kHidden});
-  n->p_dense_b = n->params.add("conv_to_linear/bias", {kHidden});
-  n->p_core_w = n->params.add("core/kernel", {n->core_in, 4 * kHidden});
-  n->p_core_u = n->params.add("core/recurrent_kernel", {kHidden, 4 * kHidden});
-  n->p_core_b = n->params.add("core/bias", {4 * kHidden});
+  // the reward is clipped (networks.py:111); the deep torso's output is ReLU'd as Dense reads it (:105), the
+  // shallow one's already is
+  n->core = core_create(n->params, "conv_to_linear", kHidden, flat, A, true, cfg->net == SEEDRL_NET_DEEP, true);
   n->p_pol_w = n->params.add("policy_logits/kernel", {kHidden, A});
   n->p_pol_b = n->params.add("policy_logits/bias", {A});
   if (cfg->net == SEEDRL_NET_DEEP) {
@@ -387,7 +372,7 @@ extern "C" size_t seedrl_net_num_params(const seedrl_net* net) { return net ? ne
 extern "C" size_t seedrl_net_arena_floats(const seedrl_net* net) { return net ? net->params.arena_floats : 0; }
 extern "C" int seedrl_net_set_lstm_mode(seedrl_net* net, int mode) {
   SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 3, "mode must be 0 (per-step launches), 1 (persistent, CTA = 2 units), 2 (persistent, CTA = batch tile x 16 units) or 3 (as 2 on wgmma bf16x3)");
-  net->lstm_mode = mode;
+  net->core.lstm_mode = mode;
   return SEEDRL_OK;
 }
 extern "C" int seedrl_net_set_conv_mode(seedrl_net* net, int mode) {
@@ -541,58 +526,29 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   Call c(n, pl, prm, nullptr, ws, st);
-  const int N = pl.N, A = n->cfg.num_actions, CI = n->core_in;
+  const int N = pl.N, A = n->cfg.num_actions;
   // bounded-wait error flag of the wgmma / persistent kernels: cleared here, set by any kernel of
   // this forward or the matching backward, read back by seedrl_net_check_error
   SEEDRL_CUDA(cudaMemsetAsync(W<int>(ws, pl.tcerr), 0, sizeof(int), st));
-  const float* flat_src;
-  int flat_relu;
   if (n->cfg.net == SEEDRL_NET_DEEP) {
     SEEDRL_TRY(pad_first_layer(c, &observation));
     SEEDRL_TRY(pack_all_weights(c, 0));
     SEEDRL_TRY(n->conv_mode == 3 ? torso_forward_planes(c, observation) : torso_forward_deep(c, observation));
-    flat_src = W<float>(ws, pl.st.back().o1);
-    flat_relu = 1;                         // tf.nn.relu before Flatten, networks.py:105
   } else {
     SEEDRL_TRY(torso_forward_shallow(c, observation));
-    flat_src = W<float>(ws, pl.sh_a2);
-    flat_relu = 0;                         // already relu'd
   }
-  float* xc = W<float>(ws, pl.xc);
-  float* z = W<float>(ws, pl.z);
-  float* hp = W<float>(ws, pl.hp);
-  float* cs = W<float>(ws, pl.cs);
-  float* hs = W<float>(ws, pl.hs);
-  float* c0buf = W<float>(ws, pl.c0buf);
-  // Dense(256) + relu written straight into the first 256 columns of the core input
-  GemmEpi e = epi_none();
-  e.bias = c.P(n->p_dense_b); e.relu = 1; e.a_relu = flat_relu;
-  SEEDRL_TRY(c.ex.gemm(false, false, N, kHidden, n->flat, flat_src, n->flat, c.P(n->p_dense_w),
-                   kHidden, xc, CI, e));
-  SEEDRL_TRY(core_input_tail(N, kHidden, A, reward, prev_actions, xc, st));
-  // input projection for all T at once: z = xc W + b
-  e = epi_none();
-  e.bias = c.P(n->p_core_b);
-  SEEDRL_TRY(c.ex.gemm(false, false, N, 4 * kHidden, CI, xc, CI, c.P(n->p_core_w), 4 * kHidden, z,
-                   4 * kHidden, e));
-  SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)B * kHidden * 4, cudaMemcpyDeviceToDevice, st));
-  SEEDRL_TRY(lstm_recurrence_forward(n->lstm_mode, c.ex, kHidden, T1, B, c.P(n->p_core_u), done, z, h0, c0buf, hs,
-                                     cs, hp, W<unsigned int>(ws, pl.counter)));
+  SEEDRL_TRY(core_forward(n->core, n->params, pl.core, c.ex, ws, prm, flat_features(n, pl, ws), reward, prev_actions,
+                          done, h0, c0));
+  const float* hs = W<float>(ws, pl.core.hs);
   // heads, networks.py:116-118
-  e = epi_none();
+  GemmEpi e = epi_none();
   e.bias = c.P(n->p_pol_b);
   SEEDRL_TRY(c.ex.gemm(false, false, N, A, kHidden, hs, kHidden, c.P(n->p_pol_w), A, policy_logits,
                    A, e));
   e.bias = c.P(n->p_base_b);
   SEEDRL_TRY(c.ex.gemm(false, false, N, 1, kHidden, hs, kHidden, c.P(n->p_base_w), 1, baseline, 1,
                    e));
-  if (h_out)
-    SEEDRL_CUDA(cudaMemcpyAsync(h_out, hs + (size_t)(T1 - 1) * B * kHidden, (size_t)B * kHidden * 4,
-                                cudaMemcpyDeviceToDevice, st));
-  if (c_out)
-    SEEDRL_CUDA(cudaMemcpyAsync(c_out, cs + (size_t)(T1 - 1) * B * kHidden, (size_t)B * kHidden * 4,
-                                cudaMemcpyDeviceToDevice, st));
-  return SEEDRL_OK;
+  return core_final_state(n->core, pl.core, st, ws, h_out, c_out);
 }
 
 extern "C" int seedrl_net_check_error(const seedrl_net* n, int T1, int B, void* ws, size_t ws_bytes,
@@ -746,14 +702,9 @@ static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, co
   const Plan pl = make_plan(n, T1, B);
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   Call c(n, pl, prm, grd, ws, st);
-  c.head_ready = head_ready;
-  const int N = pl.N, A = n->cfg.num_actions, CI = n->core_in;
-  float* xc = W<float>(ws, pl.xc); float* z = W<float>(ws, pl.z);
-  float* hp = W<float>(ws, pl.hp); float* cs = W<float>(ws, pl.cs);
-  float* hs = W<float>(ws, pl.hs); float* c0buf = W<float>(ws, pl.c0buf);
-  float* dhs = W<float>(ws, pl.dhs); float* dz = W<float>(ws, pl.dz);
-  float* dhrec = W<float>(ws, pl.dhrec); float* dd = W<float>(ws, pl.dd);
-  float* dcb[2] = {W<float>(ws, pl.dc0), W<float>(ws, pl.dc1)};
+  const int N = pl.N, A = n->cfg.num_actions;
+  const float* hs = W<float>(ws, pl.core.hs);
+  float* dhs = W<float>(ws, pl.core.dhs);
   // padding floats and the entropy_cost_param slot must not carry garbage into Adam / all-reduce
   SEEDRL_CUDA(cudaMemsetAsync(grd, 0, n->params.arena_floats * sizeof(float), st));
 
@@ -768,34 +719,11 @@ static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, co
   eacc.accumulate = 1;
   SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, 1, dbaseline, 1, c.P(n->p_base_w), 1, dhs, kHidden,
                    eacc));
-  // BPTT
-  SEEDRL_TRY(lstm_recurrence_backward(n->lstm_mode, c.ex, kHidden, T1, B, c.P(n->p_core_u), done, z, cs, c0buf, dhs,
-                                      dz, dhrec, dcb, W<unsigned int>(ws, pl.counter)));
-  SEEDRL_TRY(c.ex.gemm(true, false, kHidden, 4 * kHidden, N, hp, kHidden, dz, 4 * kHidden,
-                   c.G(n->p_core_u), 4 * kHidden, e));
-  SEEDRL_TRY(c.ex.gemm(true, false, CI, 4 * kHidden, N, xc, CI, dz, 4 * kHidden, c.G(n->p_core_w),
-                   4 * kHidden, e));
-  SEEDRL_TRY(c.ex.colsum(N, 4 * kHidden, dz, 4 * kHidden, c.G(n->p_core_b)));
-  // d dense_out = (dz W[:256,:]^T) * (dense_out > 0)
-  GemmEpi em = epi_none();
-  em.mask = xc; em.ldm = CI;
-  SEEDRL_TRY(c.ex.gemm(false, true, N, kHidden, 4 * kHidden, dz, 4 * kHidden, c.P(n->p_core_w),
-                   4 * kHidden, dd, kHidden, em));
-  // Dense(256)
-  const float* flat_src = n->cfg.net == SEEDRL_NET_DEEP ? W<float>(ws, pl.st.back().o1)
-                                                        : W<float>(ws, pl.sh_a2);
-  GemmEpi ea = epi_none();
-  ea.a_relu = n->cfg.net == SEEDRL_NET_DEEP ? 1 : 0;
-  SEEDRL_TRY(c.ex.gemm(true, false, n->flat, kHidden, N, flat_src, n->flat, dd, kHidden,
-                   c.G(n->p_dense_w), kHidden, ea));
-  SEEDRL_TRY(c.ex.colsum(N, kHidden, dd, kHidden, c.G(n->p_dense_b)));
-  // every gradient of the arena's first bucket (heads, Dense, LSTM: floats [0, seedrl_net_grad_split))
-  // is final here -- the conv torso's backward below only writes the second bucket
-  if (c.head_ready) SEEDRL_CUDA(cudaEventRecord(c.head_ready, st));
-  GemmEpi ef = epi_none();
-  ef.mask = flat_src; ef.ldm = n->flat;
-  SEEDRL_TRY(c.ex.gemm(false, true, N, n->flat, kHidden, dd, kHidden, c.P(n->p_dense_w), kHidden,
-                   W<float>(ws, pl.gA), n->flat, ef));
+  // BPTT, the core and Dense(256).  head_ready: every gradient of the arena's first bucket (heads, Dense,
+  // LSTM: floats [0, seedrl_net_grad_split)) is final before dflat -- the conv torso's backward below only
+  // writes the second bucket
+  SEEDRL_TRY(core_backward(n->core, n->params, pl.core, c.ex, ws, prm, grd, done, flat_features(n, pl, ws),
+                           W<float>(ws, pl.gA), head_ready));
   if (n->cfg.net == SEEDRL_NET_DEEP) {
     c.wb = WgradBatch{W<float>(ws, pl.partial_all), kPartialAllBytes / sizeof(float), 0, 0, {}};
     SEEDRL_TRY(pad_first_layer(c, &observation));

@@ -22,14 +22,12 @@ constexpr int kRH = 512;                 // LSTMCell(512), Dense(512) (networks.
 struct seedrl_r2d2_net {
   int A, H, W, C;
   int mode;                               // 0 = fp32 SIMT GEMMs, 2 = wgmma bf16x3
-  int lstm_mode = 2;                      // 2 = tiled persistent LSTM (lstm_tiled.cu), 1 = first persistent form,
-                                          // 3 = tiled on wgmma bf16x3 (lstm_tc.cu)
   seedrl::ParamTable params;
   size_t logical_params;
   seedrl::StridedConv conv[3];
   int conv_w[3], conv_b[3];               // param indices
-  int flat, core_in;
-  int p_ah_w, p_ah_b, p_a_w, p_dense_w, p_dense_b, p_core_w, p_core_u, p_core_b, p_vh_w, p_vh_b, p_v_w, p_v_b;
+  seedrl::Core core;                      // Dense(512) + LSTM(512); lstm_mode 1..3 (schedule.h)
+  int p_ah_w, p_ah_b, p_a_w, p_vh_w, p_vh_b, p_v_w, p_v_b;
 };
 
 namespace seedrl {
@@ -37,9 +35,10 @@ namespace seedrl {
 struct RPlan {
   size_t N;
   size_t col[3], act[3];                  // im2col matrices, post-ReLU conv outputs (NHWC)
-  size_t xc, z, hp, cs, hs, c0buf, vh, ah, v, adv;
-  size_t dv, dadv, dvh, dah, dhs, dz, dd, g[3];
-  size_t gemm_ws, tcerr, counter;
+  CorePlan core;
+  size_t vh, ah, v, adv;
+  size_t dv, dadv, dvh, dah, g[3];
+  size_t gemm_ws, tcerr;
   size_t total;
 };
 
@@ -54,12 +53,7 @@ static RPlan r_plan(const seedrl_r2d2_net* n, int T, int B) {
     p.act[i] = b.take(N * c.hout * c.wout * (size_t)c.cout * 4);
     p.g[i] = b.take(N * c.hout * c.wout * (size_t)c.cout * 4);
   }
-  p.xc = b.take(N * (size_t)n->core_in * 4);
-  p.z = b.take(N * 4 * kRH * 4);
-  p.hp = b.take(N * kRH * 4);
-  p.cs = b.take(N * kRH * 4);
-  p.hs = b.take(N * kRH * 4);
-  p.c0buf = b.take((size_t)B * kRH * 4);
+  p.core = core_plan(n->core, b, T, B);
   p.vh = b.take(N * kRH * 4);
   p.ah = b.take(N * kRH * 4);
   p.v = b.take(N * 4);
@@ -68,12 +62,8 @@ static RPlan r_plan(const seedrl_r2d2_net* n, int T, int B) {
   p.dadv = b.take(N * (size_t)n->A * 4);
   p.dvh = b.take(N * kRH * 4);
   p.dah = b.take(N * kRH * 4);
-  p.dhs = b.take(N * kRH * 4);
-  p.dz = b.take(N * 4 * kRH * 4);
-  p.dd = b.take(N * kRH * 4);
   p.gemm_ws = b.take(gemm_tc_workspace_bytes());
   p.tcerr = b.take(256);
-  p.counter = b.take(256);
   p.total = b.off;
   return p;
 }
@@ -86,17 +76,6 @@ static inline const float* RP(const seedrl_r2d2_net* n, const float* arena, int 
   return arena + n->params.offset(idx);
 }
 static inline float* RG(const seedrl_r2d2_net* n, float* arena, int idx) { return arena + n->params.offset(idx); }
-
-// _torso tail (networks.py:262-273): core_in[n] = concat(dense_out[n] (512, already ReLU'd),
-// reward[n] (NOT clipped, unlike ImpalaDeep), one_hot(prev_action[n], A)).
-__global__ void r2d2_core_tail_kernel(int Nrows, int D, int A, const float* __restrict__ reward,
-                                      const int64_t* __restrict__ prev_action, float* __restrict__ core_in) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int Wd = 1 + A;
-  if (i >= Nrows * Wd) return;
-  const int n = i / Wd, j = i - n * Wd;
-  core_in[(size_t)n * (D + Wd) + D + j] = j == 0 ? reward[n] : (prev_action[n] == (int64_t)(j - 1) ? 1.f : 0.f);
-}
 
 // _head (networks.py:275-288): q = value + advantage - mean(advantage); action = argmax_a q (first
 // maximum, tf.argmax).  Thread per row.
@@ -147,8 +126,6 @@ extern "C" int seedrl_r2d2_net_create(int num_actions, int obs_h, int obs_w, int
     const StridedConv& k = n->conv[i] = StridedConv(spec[i][1], spec[i][2], c, spec[i][0], h, w);
     h = k.hout; w = k.wout; c = k.cout;
   }
-  n->flat = h * w * c;
-  n->core_in = kRH + 1 + num_actions;
   ParamTable& t = n->params;
   // tf.Module attribute order: _advantage, _body, _core, _value
   n->p_ah_w = t.add("advantage/hidden/kernel", {kRH, 512});
@@ -160,11 +137,8 @@ extern "C" int seedrl_r2d2_net_create(int num_actions, int obs_h, int obs_w, int
     n->conv_w[i] = t.add(pre + "/kernel", {k.k, k.k, k.cin, k.cout});
     n->conv_b[i] = t.add(pre + "/bias", {k.cout});
   }
-  n->p_dense_w = t.add("body/dense/kernel", {n->flat, 512});
-  n->p_dense_b = t.add("body/dense/bias", {512});
-  n->p_core_w = t.add("core/kernel", {n->core_in, 4 * kRH});
-  n->p_core_u = t.add("core/recurrent_kernel", {kRH, 4 * kRH});
-  n->p_core_b = t.add("core/bias", {4 * kRH});
+  // _torso tail (networks.py:262-273): the reward is NOT clipped, unlike ImpalaDeep
+  n->core = core_create(t, "body/dense", kRH, h * w * c, num_actions, false, false, false);
   n->p_vh_w = t.add("value/hidden/kernel", {kRH, 512});
   n->p_vh_b = t.add("value/hidden/bias", {512});
   n->p_v_w = t.add("value/head/kernel", {512, 1});
@@ -191,7 +165,7 @@ extern "C" int seedrl_r2d2_net_set_mode(seedrl_r2d2_net* net, int mode) {
 extern "C" int seedrl_r2d2_net_set_lstm_mode(seedrl_r2d2_net* net, int mode) {
   SEEDRL_CHECK_ARG(net && mode >= 1 && mode <= 3,
                    "mode must be 1 (persistent), 2 (tiled persistent) or 3 (tiled persistent on wgmma bf16x3)");
-  net->lstm_mode = mode;
+  net->core.lstm_mode = mode;
   return SEEDRL_OK;
 }
 extern "C" int seedrl_r2d2_net_param_info(const seedrl_r2d2_net* net, int index, char* name_buf, size_t name_cap,
@@ -220,7 +194,7 @@ extern "C" int seedrl_r2d2_net_forward(const seedrl_r2d2_net* n, const float* pr
                    "unroll batch too large (GEMM row count)");
   cudaStream_t st = (cudaStream_t)stream;
   const GemmExec ex = r_exec(n, pl, ws, st);
-  const int N = (int)pl.N, A = n->A, CI = n->core_in;
+  const int N = (int)pl.N, A = n->A;
   SEEDRL_CUDA(cudaMemsetAsync(W<int>(ws, pl.tcerr), 0, sizeof(int), st));
   // ---- body: three convolutions as im2col + GEMM (bias + ReLU in the epilogue) ----------------
   const void* x = frames;
@@ -231,28 +205,14 @@ extern "C" int seedrl_r2d2_net_forward(const seedrl_r2d2_net* n, const float* pr
                          act, c.cout));
     x = act;
   }
-  float* xc = W<float>(ws, pl.xc); float* z = W<float>(ws, pl.z);
-  float* hp = W<float>(ws, pl.hp); float* cs = W<float>(ws, pl.cs); float* hs = W<float>(ws, pl.hs);
-  float* c0buf = W<float>(ws, pl.c0buf);
-  // Flatten (NHWC order) + Dense(512) + ReLU written into the first 512 columns of the core input
-  GemmEpi e = epi_none();
-  e.bias = RP(n, prm, n->p_dense_b); e.relu = 1;
-  SEEDRL_TRY(ex.gemm(false, false, N, kRH, n->flat, W<float>(ws, pl.act[2]), n->flat, RP(n, prm, n->p_dense_w), kRH,
-                     xc, CI, e));
-  r2d2_core_tail_kernel<<<ceil_div(N * (1 + A), 256), 256, 0, st>>>(N, kRH, A, reward, prev_actions, xc);
-  count_launch(PC_MISC, st);
-  SEEDRL_CHECK_LAUNCH();
-  // LSTM input projection for all T at once, then the persistent recurrence
-  e = epi_none();
-  e.bias = RP(n, prm, n->p_core_b);
-  SEEDRL_TRY(ex.gemm(false, false, N, 4 * kRH, CI, xc, CI, RP(n, prm, n->p_core_w), 4 * kRH, z, 4 * kRH, e));
-  SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)B * kRH * 4, cudaMemcpyDeviceToDevice, st));
-  SEEDRL_TRY(lstm_recurrence_forward(n->lstm_mode, ex, kRH, T, B, RP(n, prm, n->p_core_u), done, z, h0, c0buf, hs, cs,
-                                     hp, W<unsigned int>(ws, pl.counter)));
+  // Flatten (NHWC order) + Dense(512) + the LSTM core
+  SEEDRL_TRY(core_forward(n->core, n->params, pl.core, ex, ws, prm, W<float>(ws, pl.act[2]), reward, prev_actions, done,
+                          h0, c0));
+  const float* hs = W<float>(ws, pl.core.hs);
   // dueling heads
   float* vh = W<float>(ws, pl.vh); float* ah = W<float>(ws, pl.ah);
   float* v = W<float>(ws, pl.v); float* adv = W<float>(ws, pl.adv);
-  e = epi_none();
+  GemmEpi e = epi_none();
   e.bias = RP(n, prm, n->p_vh_b); e.relu = 1;
   SEEDRL_TRY(ex.gemm(false, false, N, 512, kRH, hs, kRH, RP(n, prm, n->p_vh_w), 512, vh, 512, e));
   e.bias = RP(n, prm, n->p_ah_b);
@@ -265,13 +225,7 @@ extern "C" int seedrl_r2d2_net_forward(const seedrl_r2d2_net* n, const float* pr
   dueling_fwd_kernel<<<ceil_div(N, 128), 128, 0, st>>>(N, A, v, adv, q_values, action);
   count_launch(PC_MISC, st);
   SEEDRL_CHECK_LAUNCH();
-  if (h_out)
-    SEEDRL_CUDA(cudaMemcpyAsync(h_out, hs + (size_t)(T - 1) * B * kRH, (size_t)B * kRH * 4, cudaMemcpyDeviceToDevice,
-                                st));
-  if (c_out)
-    SEEDRL_CUDA(cudaMemcpyAsync(c_out, cs + (size_t)(T - 1) * B * kRH, (size_t)B * kRH * 4, cudaMemcpyDeviceToDevice,
-                                st));
-  return SEEDRL_OK;
+  return core_final_state(n->core, pl.core, st, ws, h_out, c_out);
 }
 
 // Backward of the unroll whose forward last used `ws` (same T, B, frames).  grads = flat arena (overwritten).
@@ -283,14 +237,12 @@ extern "C" int seedrl_r2d2_net_backward(const seedrl_r2d2_net* n, const float* p
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const GemmExec ex = r_exec(n, pl, ws, st);
-  const int N = (int)pl.N, A = n->A, CI = n->core_in;
-  float* xc = W<float>(ws, pl.xc); float* z = W<float>(ws, pl.z);
-  float* hp = W<float>(ws, pl.hp); float* cs = W<float>(ws, pl.cs); float* hs = W<float>(ws, pl.hs);
-  float* c0buf = W<float>(ws, pl.c0buf);
+  const int N = (int)pl.N, A = n->A;
+  const float* hs = W<float>(ws, pl.core.hs);
   float* vh = W<float>(ws, pl.vh); float* ah = W<float>(ws, pl.ah);
   float* dv = W<float>(ws, pl.dv); float* dadv = W<float>(ws, pl.dadv);
   float* dvh = W<float>(ws, pl.dvh); float* dah = W<float>(ws, pl.dah);
-  float* dhs = W<float>(ws, pl.dhs); float* dz = W<float>(ws, pl.dz); float* dd = W<float>(ws, pl.dd);
+  float* dhs = W<float>(ws, pl.core.dhs);
   SEEDRL_CUDA(cudaMemsetAsync(grd, 0, n->params.arena_floats * sizeof(float), st));
   const GemmEpi e0 = epi_none();
   GemmEpi eacc = epi_none();
@@ -316,21 +268,9 @@ extern "C" int seedrl_r2d2_net_backward(const seedrl_r2d2_net* n, const float* p
   // d core output
   SEEDRL_TRY(ex.gemm(false, true, N, kRH, 512, dah, 512, RP(n, prm, n->p_ah_w), 512, dhs, kRH, e0));
   SEEDRL_TRY(ex.gemm(false, true, N, kRH, 512, dvh, 512, RP(n, prm, n->p_vh_w), 512, dhs, kRH, eacc));
-  // BPTT (lstm_mode is 1..3 here, so no per-step scratch)
-  SEEDRL_TRY(lstm_recurrence_backward(n->lstm_mode, ex, kRH, T, B, RP(n, prm, n->p_core_u), done, z, cs, c0buf, dhs,
-                                      dz, nullptr, nullptr, W<unsigned int>(ws, pl.counter)));
-  SEEDRL_TRY(ex.gemm(true, false, kRH, 4 * kRH, N, hp, kRH, dz, 4 * kRH, RG(n, grd, n->p_core_u), 4 * kRH, e0));
-  SEEDRL_TRY(ex.gemm(true, false, CI, 4 * kRH, N, xc, CI, dz, 4 * kRH, RG(n, grd, n->p_core_w), 4 * kRH, e0));
-  SEEDRL_TRY(ex.colsum(N, 4 * kRH, dz, 4 * kRH, RG(n, grd, n->p_core_b)));
-  // d dense_out = (dz W[:512,:]^T) * (dense_out > 0)
-  em.mask = xc; em.ldm = CI;
-  SEEDRL_TRY(ex.gemm(false, true, N, kRH, 4 * kRH, dz, 4 * kRH, RP(n, prm, n->p_core_w), 4 * kRH, dd, kRH, em));
-  const float* flat = W<float>(ws, pl.act[2]);
-  SEEDRL_TRY(ex.gemm(true, false, n->flat, kRH, N, flat, n->flat, dd, kRH, RG(n, grd, n->p_dense_w), kRH, e0));
-  SEEDRL_TRY(ex.colsum(N, kRH, dd, kRH, RG(n, grd, n->p_dense_b)));
-  em.mask = flat; em.ldm = n->flat;
-  SEEDRL_TRY(ex.gemm(false, true, N, n->flat, kRH, dd, kRH, RP(n, prm, n->p_dense_w), kRH, W<float>(ws, pl.g[2]),
-                     n->flat, em));
+  // BPTT, the core and Dense(512), down to d flat
+  SEEDRL_TRY(core_backward(n->core, n->params, pl.core, ex, ws, prm, grd, done, W<float>(ws, pl.act[2]),
+                           W<float>(ws, pl.g[2]), nullptr));
   // convolutions, last to first; the weight gradient reads the layer's input (gathered) or the im2col
   // matrix the forward kept
   for (int i = 2; i >= 0; --i) {

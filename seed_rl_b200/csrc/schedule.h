@@ -1,6 +1,6 @@
 // Pieces shared by the network schedules (net.cu: ImpalaDeep / shallow IMPALA net, r2d2_net.cu:
-// DuelingLSTMDQNNet): the parameter table, the workspace planner, the GEMM execution of one call and
-// the 'valid' strided convolution layer (strided_conv.cu).
+// DuelingLSTMDQNNet): the parameter table, the workspace planner, the GEMM execution of one call, the
+// recurrent core (lstm.cu) and the 'valid' strided convolution layer (strided_conv.cu).
 #pragma once
 #include <string.h>
 
@@ -109,6 +109,40 @@ int lstm_recurrence_forward(int mode, const GemmExec& ex, int H, int T1, int B, 
 int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
                              const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
                              float* dhrec, float* const dc[2], unsigned int* counter);
+
+// The recurrent core both nets share (lstm.cu): Dense(flat -> H) + ReLU, concat(that, reward,
+// one_hot(prev_action, A)) = the core input [N, core_in], then Keras LSTMCell(H) with done-resets.
+struct Core {
+  int H, flat, A, core_in;              // core_in = H + 1 + A
+  int dense_w, dense_b, w, u, b;        // parameter indices: Dense kernel / bias, core kernel / recurrent / bias
+  bool clip_reward;                     // reward clipped to [-1, 1] (ImpalaDeep, dmlab/networks.py:111)
+  bool flat_relu;                       // ReLU applied to the flat features as Dense reads them (ImpalaDeep)
+  bool stepwise;                        // the net offers lstm_mode 0: the plan carves its BPTT scratch
+  int lstm_mode = 2;
+};
+// Registers Dense (`dense` + "/kernel", "/bias"), then core/{kernel,recurrent_kernel,bias}.
+Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu,
+                 bool stepwise);
+
+// The core's buffers in a workspace of T1 x B frames (N = T1 * B rows): core input, gates, h[t-1], c, h, the
+// copy of c0, d h, d gates, (stepwise) dh_rec and two dc buffers, d dense_out, the LSTM barrier counters.
+struct CorePlan {
+  int T1, B, N;
+  size_t xc, z, hp, cs, hs, c0buf, dhs, dz, dhrec, dc[2], dd, counter;
+};
+CorePlan core_plan(const Core& k, Bump& b, int T1, int B);
+
+// Forward up to hs (ws + p.hs, [T1, B, H]) from the flat features [N, flat].
+int core_forward(const Core& k, const ParamTable& t, const CorePlan& p, const GemmExec& ex, void* ws, const float* prm,
+                 const float* flat, const float* reward, const int64_t* prev_actions, const uint8_t* done,
+                 const float* h0, const float* c0);
+// The final h and c of the last core_forward (either may be null).
+int core_final_state(const Core& k, const CorePlan& p, cudaStream_t st, void* ws, float* h_out, float* c_out);
+// Backward from d hs (ws + p.dhs) to the core and Dense gradients and dflat [N, flat] (masked by flat > 0);
+// head_ready (may be null) is recorded once every gradient but dflat is final.
+int core_backward(const Core& k, const ParamTable& t, const CorePlan& p, const GemmExec& ex, void* ws,
+                  const float* prm, float* grd, const uint8_t* done, const float* flat, float* dflat,
+                  cudaEvent_t head_ready);
 
 // Reads back the device-side error flag of the last forward/backward that used a workspace (set when
 // a bounded mbarrier / grid-barrier wait of a wgmma or persistent kernel expired, i.e. the results are

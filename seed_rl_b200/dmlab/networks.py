@@ -16,20 +16,21 @@ IMPALA-paper shallow net (not in the reference, SURVEY 0), same protocol.
 import collections
 import ctypes
 import math
-import threading
 
-import numpy as np
 import torch
 
 from seed_rl_b200 import _lib
+from seed_rl_b200.common.cuda_net import CudaNet
 
 AgentOutput = collections.namedtuple('AgentOutput', 'action policy_logits baseline')
 
 LSTM_UNITS = 256
 
 
-class _CudaAgent(object):
+class _CudaAgent(CudaNet):
   _NET = None
+  _LIB = 'seedrl_net'
+  _EXTRA_PARAMS = 1        # entropy_cost_param (learner.py:225-234)
 
   def __init__(self, num_actions, obs_shape=(84, 84, 4), seed=0, device=None, conv_mode='simt',
                lstm_mode='tiled'):
@@ -63,61 +64,12 @@ class _CudaAgent(object):
                        "'persistent' or 'stepwise'")
     self.lstm_mode = lstm_mode
     _lib.check(L.seedrl_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
-    self._n_tensors = L.seedrl_net_num_param_tensors(h)
-    self.arena_floats = int(L.seedrl_net_arena_floats(h))
-    self.num_params = int(L.seedrl_net_num_params(h))
-    self.param_info = []       # (name, shape, offset) incl. entropy_cost_param last
-    for i in range(self._n_tensors + 1):
-      name = ctypes.create_string_buffer(128)
-      dims = (ctypes.c_int64 * 4)()
-      off = ctypes.c_size_t()
-      rank = L.seedrl_net_param_info(h, i, name, 128, dims, ctypes.byref(off))
-      self.param_info.append((name.value.decode(), tuple(int(dims[k]) for k in range(rank)),
-                              int(off.value)))
-    self.device = torch.device(device if device is not None else
-                               ('cuda:%d' % torch.cuda.current_device()))
-    # flat arenas: params / grads (Adam slots live in the optimizer)
-    self.params = torch.zeros(self.arena_floats, dtype=torch.float32, device=self.device)
-    self.grads = torch.zeros_like(self.params)
-    self._init_parameters(seed)
-    # One activation workspace per (T1, B): the inference thread (T1=1, B=N, its own stream)
-    # and the learner thread (T1=T+1, B=batch) share this agent's parameters but never a
-    # workspace; backward() uses exactly the buffer its is_training forward filled.
-    self._workspaces = {}
-    self._lock = threading.Lock()
+    self._setup(seed, device)
     self._rng_offset = 0
     self._seed = seed
-    self._saved = None
 
-  def __del__(self):
-    try:
-      if getattr(self, '_h', None):
-        _lib.lib().seedrl_net_destroy(self._h)
-        self._h = None
-    except Exception:   # interpreter shutdown
-      pass
-
-  # ---- parameters ---------------------------------------------------------------
-  def _view(self, arena, i):
-    name, shape, off = self.param_info[i]
-    n = int(np.prod(shape)) if shape else 1
-    return arena[off:off + n].view(shape if shape else ())
-
-  @property
-  def trainable_variables(self):
-    return [self._view(self.params, i) for i in range(self._n_tensors)]
-
-  @property
-  def variable_names(self):
-    return [p[0] for p in self.param_info[:self._n_tensors]]
-
-  def named_parameters(self):
-    return collections.OrderedDict(
-        (self.param_info[i][0], self._view(self.params, i)) for i in range(self._n_tensors))
-
-  def named_gradients(self):
-    return collections.OrderedDict(
-        (self.param_info[i][0], self._view(self.grads, i)) for i in range(self._n_tensors + 1))
+  def _param_rank(self, index, name_buf, dims, offset):
+    return _lib.lib().seedrl_net_param_info(self._h, index, name_buf, len(name_buf), dims, ctypes.byref(offset))
 
   @property
   def entropy_cost_param(self):
@@ -127,65 +79,10 @@ class _CudaAgent(object):
   def entropy_cost_param_index(self):
     return self.param_info[self._n_tensors][2]
 
-  def load_named_parameters(self, named):
-    """Copies {name: array} (Keras layouts) into the arena."""
-    mine = self.named_parameters()
-    for k, v in named.items():
-      if k == 'entropy_cost_param':
-        self.entropy_cost_param.copy_(torch.as_tensor(np.asarray(v, np.float32)))
-        continue
-      t = torch.as_tensor(np.asarray(v, np.float32))
-      if tuple(t.shape) != tuple(mine[k].shape):
-        raise ValueError('shape mismatch for %s: %s vs %s' % (k, tuple(t.shape), tuple(mine[k].shape)))
-      mine[k].copy_(t)
-
-  def _init_parameters(self, seed):
-    """Keras defaults (TF 2.4.1): glorot_uniform kernels, zero biases, orthogonal
-    recurrent kernel, unit_forget_bias.  One-time host-side work."""
-    rng = np.random.default_rng(seed)
-    for i in range(self._n_tensors):
-      name, shape, _ = self.param_info[i]
-      if name.endswith('bias'):
-        a = np.zeros(shape, np.float32)
-        if name == 'core/bias':
-          a[LSTM_UNITS:2 * LSTM_UNITS] = 1.0
-      elif name == 'core/recurrent_kernel':
-        m = rng.normal(size=(shape[1], shape[0]))
-        q, r = np.linalg.qr(m)
-        a = (q * np.sign(np.diag(r))).T.astype(np.float32)
-      else:
-        rf = int(np.prod(shape[:-2])) if len(shape) > 2 else 1
-        lim = math.sqrt(6.0 / (shape[-2] * rf + shape[-1] * rf))
-        a = rng.uniform(-lim, lim, shape).astype(np.float32)
-      self._view(self.params, i).copy_(torch.from_numpy(a))
-
   # ---- protocol ---------------------------------------------------------------
   def initial_state(self, batch_size):
     z = torch.zeros([batch_size, LSTM_UNITS], dtype=torch.float32, device=self.device)
     return (z, z.clone())
-
-  def _workspace(self, T1, B):
-    key = (T1, B, threading.get_ident())
-    with self._lock:
-      ws = self._workspaces.get(key)
-      if ws is None:
-        nbytes = int(_lib.lib().seedrl_net_workspace_bytes(self._h, T1, B))
-        # drop this thread's buffers of other shapes first (a learner that changes batch size
-        # must not keep several multi-GB workspaces alive)
-        for k in [k for k in self._workspaces if k[2] == key[2] and k != key]:
-          del self._workspaces[k]
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        self._workspaces[key] = ws
-    return ws
-
-  def check_errors(self):
-    """Raises if a kernel of the last training forward/backward hit a bounded-wait timeout
-    (synchronises the current stream; call where the loss is read anyway)."""
-    if self._saved is None:
-      return
-    T1, B, ws = self._saved[0], self._saved[1], self._saved[-1]
-    _lib.check(_lib.lib().seedrl_net_check_error(self._h, T1, B, _lib.ptr(ws), ws.numel(),
-                                                 _lib.stream_ptr()))
 
   def _next_rng_offset(self):
     with self._lock:
@@ -218,7 +115,7 @@ class _CudaAgent(object):
     baseline = torch.empty([T1, B], dtype=torch.float32, device=self.device)
     h = torch.empty_like(h0)
     c = torch.empty_like(c0)
-    ws = self._workspace(T1, B)
+    ws = self.workspace(T1, B)
     L = _lib.lib()
     st = _lib.stream_ptr()
     _lib.check(L.seedrl_net_forward(
@@ -239,7 +136,7 @@ class _CudaAgent(object):
           _lib.ptr(action), st))
     action = action.view(T1, B)
     if is_training:
-      self._saved = (T1, B, prev_actions, reward, done, frame, ws)
+      self._saved = (T1, B, ws, prev_actions, reward, done, frame)
     out = AgentOutput(action, logits, baseline)
     if not unroll:
       out = AgentOutput(*(t.squeeze(0) for t in out))
@@ -251,7 +148,7 @@ class _CudaAgent(object):
     LSTM) are final -- before the convolution torso's backward -- for an overlapped all-reduce."""
     if self._saved is None:
       raise RuntimeError('backward() needs a preceding __call__(..., unroll=True, is_training=True)')
-    T1, B, prev_actions, reward, done, frame, ws = self._saved
+    T1, B, ws, prev_actions, reward, done, frame = self._saved
     L = _lib.lib()
     if head_ready_event is None:
       _lib.check(L.seedrl_net_backward(
@@ -278,12 +175,6 @@ class _CudaAgent(object):
 
   def entropy_cost(self):
     return torch.exp(self._entropy_mul * self.entropy_cost_param)
-
-  def state_dict(self):
-    return {'params': self.params.detach().cpu(), 'param_info': self.param_info}
-
-  def load_state_dict(self, d):
-    self.params.copy_(d['params'].to(self.device))
 
 
 class ImpalaDeep(_CudaAgent):

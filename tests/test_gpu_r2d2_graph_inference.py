@@ -1,6 +1,7 @@
 """GPU: R2D2 central inference as one CUDA-graph replay per batch (R2D2InferenceHost(cuda_graph=True)):
 the device epsilon-greedy kernel against a numpy restatement of its Philox draw, the eval-aware store
-append, bit-for-bit parity with the eager host in greedy mode, exploration statistics,
+append, bit-for-bit parity with the eager host in greedy mode (also with partial batches of two other
+sizes, through which the graph host keeps the workspace it captured), exploration statistics,
 reproducibility, two hosts sharing one agent, and the hand-off to the replay and the learner."""
 import threading
 
@@ -224,6 +225,51 @@ def test_graph_host_equals_eager_host_in_greedy_mode(shape, gemm_mode, monkeypat
     for t1, t2 in zip(utils.flatten(u), utils.flatten(v)):
       assert torch.equal(t1, t2)
   assert eager.info_queue.size() == graph.info_queue.size() > 0
+  agent.check_errors()
+
+
+def test_graph_host_keeps_its_workspace_through_partial_batches_of_two_sizes(monkeypatch):
+  """Eager partial batches of two other sizes between full batches evict the (1, N) workspace the graph
+  captured from the agent's cache (each thread keeps two shapes).  The host holds that workspace itself, so
+  every replay still writes into memory it owns: actions, tables and unrolls equal an eager host's."""
+  c = TOY
+  st = learner.default_settings(unroll_length=c['unroll'], burn_in=c['burn_in'])
+  monkeypatch.setattr(learner, 'apply_epsilon_greedy', lambda actions, *a, **k: actions)
+  eager = make_host(networks.DuelingLSTMDQNNet(c['A'], c['obs'], c['S'], seed=1), c['obs'], c['N'], c['num_envs'],
+                    c['num_eval'], st)
+  agent = networks.DuelingLSTMDQNNet(c['A'], c['obs'], c['S'], seed=1)
+  captured, workspace = [], agent.workspace
+
+  def recording_workspace(T1, B):
+    ws = workspace(T1, B)
+    if torch.cuda.is_current_stream_capturing():
+      captured.append(ws)
+    return ws
+  monkeypatch.setattr(agent, 'workspace', recording_workspace)
+  graph = make_host(agent, c['obs'], c['N'], c['num_envs'], c['num_eval'], st, cuda_graph=True)
+  graph.envs_epsilon.zero_()
+  rng = np.random.default_rng(5)
+  batches = [rng.permutation(c['num_envs'])[:n].astype(np.int32) for n in (c['N'], 2, c['N'], 3)]
+  evicted = False
+  for i, (ids, run_ids, env, raw) in enumerate(call_sequence(c['obs'], c['num_envs'], batches, 40, seed=6)):
+    np.testing.assert_array_equal(eager.inference(ids, run_ids, env, raw), graph.inference(ids, run_ids, env, raw),
+                                  err_msg='call %d' % i)
+    if captured:
+      cached = agent._workspaces[threading.get_ident()].values()
+      evicted |= not any(ws is captured[0] for ws in cached)
+  assert len(captured) == 1 and graph._g_workspace is captured[0]
+  assert evicted                                                   # the case this test is about happened
+  for x, y in ((eager.first_agent_states, graph.first_agent_states), (eager.agent_states, graph.agent_states),
+               (eager.actions, graph.actions)):
+    for t, u in zip(x._state, y._state):
+      assert torch.equal(t, u), x.name
+  for t, u in zip(eager.store._state + [eager.store._index], graph.store._state + [graph.store._index]):
+    assert torch.equal(t, u)
+  qa, qb = drain(eager), drain(graph)
+  assert len(qa) == len(qb) > 0
+  for u, v in zip(qa, qb):
+    for t1, t2 in zip(utils.flatten(u), utils.flatten(v)):
+      assert torch.equal(t1, t2)
   agent.check_errors()
 
 
