@@ -413,6 +413,25 @@ int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_train, const fl
                              const float* importance_weights, float gamma, int n_steps, float eta,
                              float value_rescaling_eps, float* loss, float* priorities, float* dq,
                              void* scratch, seedrl_stream_t stream);
+/* Retrace(lambda) targets (Munos et al. 2016) in place of the n-step ones; NOT in the reference.
+ *   The target policy is greedy in the online network, a*_i = argmax_a q_train (first maximum), so
+ *   the trace is c_i = lambda * 1[a_i == a*_i] for any epsilon-greedy behaviour and no behaviour
+ *   probabilities are needed.  With q*_i = h^-1(q_target[i, a*_i]), qa_i = h^-1(q_target[i, a_i]),
+ *   g_i = gamma * (1 - done_i), in the indexing of n_step_bellman_target (row i of reward / done is
+ *   the transition into x_i):
+ *     Y[T-1] = r_{T-1} + g_{T-1} q*_{T-1};   Y[i] = r_i + g_i (q*_i + c_i (Y[i+1] - qa_i)), i >= 1;
+ *     td_t = h(Y[t+1]) - q_train[t, a_t], t < T-1.
+ *   Loss, priorities and dq are those of seedrl_r2d2_loss_fwd_bwd (agents/r2d2/learner.py:258-330,
+ *   :604); lambda = 0 equals it at n_steps = 1.  One launch, deterministic.  scratch:
+ *   seedrl_r2d2_retrace_loss_scratch_bytes.  Errors: T < 2, lambda outside [0, 1] or NaN, a null
+ *   pointer (importance_weights may be NULL = all ones). */
+size_t seedrl_r2d2_retrace_loss_scratch_bytes(int T, int B);
+int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
+                                     const int64_t* replay_action, const float* reward,
+                                     const uint8_t* done, const float* importance_weights, float gamma,
+                                     float lambda_, float eta, float value_rescaling_eps, float* loss,
+                                     float* priorities, float* dq, void* scratch,
+                                     seedrl_stream_t stream);
 /* <- agents/r2d2/learner.py:155-177 (apply_epsilon_greedy) on the device.  actions int32 [N]: the
  *   greedy actions on entry, the chosen ones on exit; envs_epsilon float32 [num_envs] (the table of
  *   get_envs_epsilon, :129-152), read at env_ids[n].  Row n draws

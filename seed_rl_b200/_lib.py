@@ -145,6 +145,9 @@ SIGNATURES = {
     'seedrl_r2d2_loss_scratch_bytes': (c_size_t, [c_int, c_int, c_int]),
     'seedrl_r2d2_loss_fwd_bwd': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, c_float, c_int, c_float, c_float,
                                          P, P, P, P, P]),
+    'seedrl_r2d2_retrace_loss_scratch_bytes': (c_size_t, [c_int, c_int]),
+    'seedrl_r2d2_retrace_loss_fwd_bwd': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, c_float, c_float, c_float,
+                                                 c_float, P, P, P, P, P]),
     'seedrl_r2d2_epsilon_greedy': (c_int, [c_int, c_int, P, P, c_u64, P, P, P]),
     'seedrl_replay_sample': (c_int, [c_int, P, c_float, c_float, c_int, P, P, P, P, P]),
     'seedrl_clip_scratch_bytes': (c_size_t, []),

@@ -4,7 +4,9 @@
   Unroll / SampledUnrolls / EpisodeInfo            :96-112
   get_replay_insertion_batch_size, get_envs_epsilon, apply_epsilon_greedy   :115-177
   compute_loss_and_priorities_from_agent_outputs   :258-330 (+ value rescaling :180-192 and
-                                                   n-step Bellman targets :195-255, fused)
+                                                   n-step Bellman targets :195-255, fused; or,
+                                                   opt-in and not in the reference, Retrace(lambda)
+                                                   targets with a greedy target policy)
   compute_loss_and_priorities                      :333-386  (burn-in, two unrolls per network)
   minimize (R2D2LearnerStep)                       :581-634  (importance-weighted mean loss,
                                                    global-norm clip :604-609, Keras Adam)
@@ -13,8 +15,8 @@
                                                    -> ReplayFeeder over common.utils.PrioritizedReplay
 
 Device work per step = 2 burn-in unrolls + 2 suffix unrolls (seedrl_r2d2_net_forward) ->
-seedrl_r2d2_loss_fwd_bwd -> seedrl_r2d2_net_backward -> seedrl_clip_by_global_norm ->
-seedrl_adam_apply -> priority write-back.  There is no autograd tape.
+seedrl_r2d2_loss_fwd_bwd (or seedrl_r2d2_retrace_loss_fwd_bwd) -> seedrl_r2d2_net_backward ->
+seedrl_clip_by_global_norm -> seedrl_adam_apply -> priority write-back.  There is no autograd tape.
 """
 import collections
 
@@ -26,6 +28,7 @@ from seed_rl_b200.common import common_flags  # pylint: disable=unused-import
 from seed_rl_b200.common import utils
 
 FLAGS = flags.FLAGS
+BELLMAN_TARGETS = ('n_step', 'retrace')
 
 
 def _define(fn, name, default, help_):
@@ -58,6 +61,11 @@ _define(flags.DEFINE_float, 'clip_norm', 40, 'We clip gradient norm to this valu
 _define(flags.DEFINE_float, 'value_function_rescaling_epsilon', 1e-3, 'Epsilon used for value function rescaling.')
 _define(flags.DEFINE_integer, 'n_steps', 5, 'n-step returns: how far ahead we look for computing the Bellman targets.')
 _define(flags.DEFINE_float, 'discounting', .997, 'Discounting factor.')
+_define(flags.DEFINE_string, 'bellman_target', 'n_step',
+        'Bellman targets of the loss: "n_step", the reference\'s n-step double-DQN targets, or "retrace", '
+        'Retrace(lambda) targets (Munos et al. 2016) with a target policy greedy in the online network. '
+        'Retrace is not in the reference; under it --n_steps is unused.')
+_define(flags.DEFINE_float, 'retrace_lambda', 0.95, 'Trace coefficient lambda in [0, 1] of --bellman_target=retrace.')
 _define(flags.DEFINE_float, 'eval_epsilon', 1e-3, 'Epsilon (as in epsilon-greedy) used for evaluation.')
 _define(flags.DEFINE_bool, 'inference_cuda_graph', False,
         'Replay the device side of every full inference batch as one CUDA graph, with epsilon-greedy '
@@ -73,20 +81,24 @@ EpisodeInfo = collections.namedtuple('EpisodeInfo', 'num_frames returns raw_retu
 # flag defaults of the reference (learner.py:47-87)
 N_STEPS = 5
 VALUE_FUNCTION_RESCALING_EPSILON = 1e-3
+RETRACE_LAMBDA = 0.95
 
 R2D2Settings = collections.namedtuple(
     'R2D2Settings',
     'batch_size replay_ratio unroll_length update_target_every_n_step replay_buffer_size '
     'replay_buffer_min_size priority_exponent burn_in importance_sampling_exponent clip_norm '
-    'value_function_rescaling_epsilon n_steps discounting eval_epsilon num_training_tpus')
+    'value_function_rescaling_epsilon n_steps discounting eval_epsilon num_training_tpus bellman_target '
+    'retrace_lambda')
 
 
 def default_settings(**kw):
-  """The reference's flag defaults (learner.py:47-92)."""
+  """The reference's flag defaults (learner.py:47-92), plus the n-step targets of the reference as the
+  default `bellman_target`."""
   d = dict(batch_size=64, replay_ratio=1.5, unroll_length=100, update_target_every_n_step=2500,
            replay_buffer_size=100, replay_buffer_min_size=10, priority_exponent=0.9, burn_in=40,
            importance_sampling_exponent=0.6, clip_norm=40., value_function_rescaling_epsilon=1e-3, n_steps=5,
-           discounting=.997, eval_epsilon=1e-3, num_training_tpus=1)
+           discounting=.997, eval_epsilon=1e-3, num_training_tpus=1, bellman_target='n_step',
+           retrace_lambda=RETRACE_LAMBDA)
   d.update(kw)
   return R2D2Settings(**d)
 
@@ -140,13 +152,28 @@ def device_epsilon_greedy(actions, env_ids_i32, envs_epsilon, num_actions, seed,
       int(seed) & 0xFFFFFFFFFFFFFFFF, _lib.ptr(counter), _lib.ptr(actions), _lib.stream_ptr()))
 
 
+def check_bellman_target(bellman_target, retrace_lambda):
+  """Raises ValueError for an unknown target kind or, under 'retrace', a lambda outside [0, 1]."""
+  if bellman_target not in BELLMAN_TARGETS:
+    raise ValueError('bellman_target must be one of %s, got %r' % (BELLMAN_TARGETS, bellman_target))
+  if bellman_target == 'retrace' and not 0. <= float(retrace_lambda) <= 1.:
+    raise ValueError('retrace_lambda must be in [0, 1], got %r' % (retrace_lambda,))
+
+
 def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target_agent_output, env_outputs,
                                                    agent_outputs, gamma, eta=0.9, n_steps=N_STEPS,
                                                    importance_weights=None,
-                                                   value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON):
+                                                   value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON,
+                                                   bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA):
   """reference :258-330.  Returns (loss [B], priorities [B]); the gradient of
   mean(loss * importance_weights) w.r.t. training_agent_output.q_values (reference :604) is
-  returned as the third element (the reference gets it from the tape)."""
+  returned as the third element (the reference gets it from the tape).
+
+  bellman_target='n_step' is the reference's rule.  'retrace' (not in the reference) replaces the
+  n-step targets by Retrace(retrace_lambda) targets whose target policy is greedy in the online
+  network, so the trace is retrace_lambda * 1[replayed action == argmax_a Q_online]; n_steps is then
+  unused (seedrl_r2d2_retrace_loss_fwd_bwd in include/seedrl_b200.h states the targets)."""
+  check_bellman_target(bellman_target, retrace_lambda)
   f32 = torch.float32
   q = _lib.require_cuda(training_agent_output.q_values, f32, 'training q_values')
   qt = _lib.require_cuda(target_agent_output.q_values, f32, 'target q_values')
@@ -160,6 +187,13 @@ def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target
   L = _lib.lib()
   loss = torch.empty(B, dtype=f32, device=q.device); prio = torch.empty_like(loss)
   dq = torch.empty_like(q)
+  if bellman_target == 'retrace':
+    scratch = torch.empty(int(L.seedrl_r2d2_retrace_loss_scratch_bytes(T, B)), dtype=torch.uint8, device=q.device)
+    _lib.check(L.seedrl_r2d2_retrace_loss_fwd_bwd(
+        T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn), _lib.ptr(w), float(gamma),
+        float(retrace_lambda), float(eta), float(value_function_rescaling_epsilon), _lib.ptr(loss), _lib.ptr(prio),
+        _lib.ptr(dq), _lib.ptr(scratch), _lib.stream_ptr()))
+    return loss, prio, dq
   scratch = torch.empty(int(L.seedrl_r2d2_loss_scratch_bytes(T, B, n_steps)), dtype=torch.uint8, device=q.device)
   _lib.check(L.seedrl_r2d2_loss_fwd_bwd(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn),
                                         _lib.ptr(w), float(gamma), int(n_steps), float(eta),
@@ -210,11 +244,13 @@ def split_structure(structure, prefix_length):
 
 def compute_loss_and_priorities(training_agent, target_agent, agent_state, prev_actions, env_outputs, agent_outputs,
                                 gamma, burn_in, importance_weights=None, n_steps=N_STEPS,
-                                value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON):
+                                value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON,
+                                bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA):
   """reference :333-386.  Time-major inputs with burn_in + unroll_length + 1 rows.  Burn-in
   unrolls update the recurrent state of both networks without gradient (:365-371); the suffix is
   unrolled by the training agent (kept for `backward`) and the target agent.  Returns
   (loss [B], priorities [B], dq [T_suffix, B, A])."""
+  check_bellman_target(bellman_target, retrace_lambda)     # before any network work
   if burn_in:
     (pa_pre, env_pre), (pa_suf, env_suf) = split_structure((prev_actions, tuple(env_outputs)), burn_in)
     _, ao_suf = split_structure(tuple(agent_outputs), burn_in)
@@ -227,7 +263,8 @@ def compute_loss_and_priorities(training_agent, target_agent, agent_state, prev_
   target_out, _ = target_agent((pa_suf, env_suf), target_state, unroll=True)
   return compute_loss_and_priorities_from_agent_outputs(
       training_out, target_out, utils.EnvOutput(*env_suf), AgentOutput(*ao_suf), gamma, n_steps=n_steps,
-      importance_weights=importance_weights, value_function_rescaling_epsilon=value_function_rescaling_epsilon)
+      importance_weights=importance_weights, value_function_rescaling_epsilon=value_function_rescaling_epsilon,
+      bellman_target=bellman_target, retrace_lambda=retrace_lambda)
 
 
 class R2D2LearnerStep(object):
@@ -237,6 +274,7 @@ class R2D2LearnerStep(object):
   def __init__(self, agent, target_agent, optimizer, settings=None, process_group=None):
     self.agent, self.target_agent, self.optimizer = agent, target_agent, optimizer
     self.settings = settings or default_settings()
+    check_bellman_target(self.settings.bellman_target, self.settings.retrace_lambda)
     self.pg = process_group
     import torch.distributed as td
     self.world = td.get_world_size(process_group) if (td.is_available() and td.is_initialized()) else 1
@@ -254,7 +292,8 @@ class R2D2LearnerStep(object):
     loss, priorities, dq = compute_loss_and_priorities(
         self.agent, self.target_agent, u.agent_state, u.prev_actions, u.env_outputs, u.agent_outputs,
         gamma=s.discounting, burn_in=s.burn_in, importance_weights=w, n_steps=s.n_steps,
-        value_function_rescaling_epsilon=s.value_function_rescaling_epsilon)
+        value_function_rescaling_epsilon=s.value_function_rescaling_epsilon, bellman_target=s.bellman_target,
+        retrace_lambda=s.retrace_lambda)
     grads = self.agent.backward(dq)
     if s.clip_norm:
       norm = clip_by_global_norm(grads, s.clip_norm)                 # :606-609 (use_norm = the same norm)

@@ -43,6 +43,7 @@ class R2D2InferenceHost(inference_host.InferenceHostBase):
     than `generator`'s, so the explored actions differ; the distribution is the same).  Other batch
     sizes take the eager path."""
     self.settings = s = settings or learner.default_settings()
+    learner.check_bellman_target(s.bellman_target, s.retrace_lambda)
     self.num_envs, self.num_eval_envs = int(num_envs), int(num_eval_envs)
     self.num_training_envs = self.num_envs - self.num_eval_envs                      # :122-123
     if self.num_training_envs <= 0:
@@ -90,7 +91,7 @@ class R2D2InferenceHost(inference_host.InferenceHostBase):
 
   def _completed_unrolls(self, nc):
     """(:805-824) the completed unrolls with their first agent states and initial priorities from the
-    behaviour Q values of the suffix."""
+    behaviour Q values of the suffix, under the learner's `bellman_target`."""
     s = self.settings
     completed_ids, unrolls = self.store.complete(nc)
     _, unrolled_env, unrolled_agent = unrolls
@@ -100,7 +101,8 @@ class R2D2InferenceHost(inference_host.InferenceHostBase):
     ao = learner.AgentOutput(*ao_suf)
     _, priorities, _ = learner.compute_loss_and_priorities_from_agent_outputs(
         ao, ao, utils.EnvOutput(*env_suf), ao, s.discounting, n_steps=s.n_steps,
-        value_function_rescaling_epsilon=s.value_function_rescaling_epsilon)
+        value_function_rescaling_epsilon=s.value_function_rescaling_epsilon, bellman_target=s.bellman_target,
+        retrace_lambda=s.retrace_lambda)
     return completed_ids, learner.Unroll(first, priorities, *unrolls)
 
 
@@ -130,7 +132,8 @@ def learner_loop(create_env_fn, create_agent_fn, create_optimizer_fn):
   logging.info('Starting learner loop')
   utils.validate_learner_config(FLAGS)
   s = learner.settings_from_flags()
-  assert s.n_steps >= 1, '--n_steps < 1 does not make sense.'
+  assert s.n_steps >= 1, '--n_steps < 1 does not make sense.'       # unused under --bellman_target=retrace
+  learner.check_bellman_target(s.bellman_target, s.retrace_lambda)
   env = create_env_fn(0, FLAGS)
   num_actions = env.action_space.n
   TS = utils.TensorSpec

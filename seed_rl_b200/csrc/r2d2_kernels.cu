@@ -3,6 +3,8 @@
 //   r2d2_stack_frames_kernel   atari/networks.py:57-173   bit-packed frame stacking (uint8/int32)
 //   r2d2_loss_kernel           agents/r2d2/learner.py:180-330  h / h^-1, n-step double-DQN
 //                              targets, per-sequence loss, priorities and d loss / d q
+//   r2d2_retrace_loss_kernel   the same loss with Retrace(lambda) targets (Munos et al. 2016), greedy
+//                              target policy; not in the reference (opt-in)
 //   replay_sample_kernel       common/utils.py:327-352    p_i ~ prio_i^alpha, inverse-CDF draw,
 //                              importance weights normalised by their max
 //   global-norm clip           tf.clip_by_global_norm, learner.py:608 (clip_norm = 40)
@@ -39,6 +41,12 @@ __global__ void r2d2_loss_kernel(const R2d2LossParams p) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= p.B) return;
   r2d2_loss_thread(p, b);
+}
+
+__global__ void r2d2_retrace_loss_kernel(const R2d2RetraceParams p) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= p.B) return;
+  r2d2_retrace_loss_thread(p, b);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -166,6 +174,32 @@ extern "C" int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_trai
   for (int k = 0; k < 8; ++k) p.gamma_pow[k] = (float)pow((double)gamma, (double)k);   // fp32(gamma ** k)
   p.loss = loss; p.priorities = priorities; p.dq = dq; p.scratch = reinterpret_cast<float*>(scratch);
   r2d2_loss_kernel<<<ceil_div(B, 64), 64, 0, (cudaStream_t)stream>>>(p);
+  count_launch(PC_LOSS, (cudaStream_t)stream);
+  SEEDRL_CHECK_LAUNCH();
+  return SEEDRL_OK;
+}
+
+extern "C" size_t seedrl_r2d2_retrace_loss_scratch_bytes(int T, int B) {
+  return (size_t)B * (size_t)T * sizeof(float);
+}
+
+extern "C" int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
+                                                const int64_t* replay_action, const float* reward,
+                                                const uint8_t* done, const float* importance_weights, float gamma,
+                                                float lambda_, float eta, float value_rescaling_eps, float* loss,
+                                                float* priorities, float* dq, void* scratch,
+                                                seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(T >= 2 && B >= 1 && A >= 1, "need T>=2, B>=1, A>=1");
+  SEEDRL_CHECK_ARG(lambda_ >= 0.f && lambda_ <= 1.f, "lambda must be in [0, 1]");   // false for NaN
+  SEEDRL_CHECK_ARG(q_train && q_target && replay_action && reward && done && loss && priorities && dq && scratch,
+                   "null pointer");
+  R2d2RetraceParams p;
+  p.T = T; p.B = B; p.A = A;
+  p.q_train = q_train; p.q_target = q_target; p.replay_action = replay_action; p.reward = reward;
+  p.done = done; p.is_weights = importance_weights;
+  p.gamma = gamma; p.lambda = lambda_; p.eta = eta; p.eps = value_rescaling_eps;
+  p.loss = loss; p.priorities = priorities; p.dq = dq; p.scratch = reinterpret_cast<float*>(scratch);
+  r2d2_retrace_loss_kernel<<<ceil_div(B, 64), 64, 0, (cudaStream_t)stream>>>(p);
   count_launch(PC_LOSS, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;

@@ -1,0 +1,19 @@
+// TEST HARNESS (never part of libseedrl_b200.so): r2d2_retrace_loss_thread -- the body the GPU kernel
+// r2d2_retrace_loss_kernel executes, from seed_rl_b200/csrc/r2d2_thread.inl -- compiled as plain host
+// C++ and run thread by thread, so that the CPU test suite can check it against tests/retrace_oracle.py.
+//   g++ -O2 -shared -fPIC -o _r2d2_retrace_host.so r2d2_retrace_host.cpp
+#define SEEDRL_HD inline
+#include "../../seed_rl_b200/csrc/r2d2_thread.inl"
+
+extern "C" int emu_r2d2_retrace_loss(int T, int B, int A, const float* q_train, const float* q_target,
+                                     const int64_t* replay_action, const float* reward, const uint8_t* done,
+                                     const float* is_weights, float gamma, float lambda_, float eta, float eps,
+                                     float* loss, float* priorities, float* dq, float* scratch) {
+  seedrl::R2d2RetraceParams p;
+  p.T = T; p.B = B; p.A = A;
+  p.q_train = q_train; p.q_target = q_target; p.replay_action = replay_action; p.reward = reward; p.done = done;
+  p.is_weights = is_weights; p.gamma = gamma; p.lambda = lambda_; p.eta = eta; p.eps = eps;
+  p.loss = loss; p.priorities = priorities; p.dq = dq; p.scratch = scratch;
+  for (int b = 0; b < B; ++b) seedrl::r2d2_retrace_loss_thread(p, b);
+  return 0;
+}
