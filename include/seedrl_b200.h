@@ -573,6 +573,15 @@ int seedrl_debug_lstm_forward(int mode, int gemm_mode, int H, int T1, int B, con
 int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, const float* U, const uint8_t* done,
                                const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
                                void* ws, size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
+/* Byte offset and size, in a seedrl_r2d2_net workspace of a (T, B) call, of the fp32 buffers the last forward
+ * left there (rows = the T * B frames, time-major; backward does not overwrite them).  The backward's ReLU
+ * derivative masks are these buffers > 0:
+ *   index 0..2  post-ReLU outputs of conv0..conv2, NHWC [T*B, Ho, Wo, filters];
+ *   index 3     the core input [T*B, 512 + 1 + num_actions]: the post-ReLU Dense(512) output in its first
+ *               512 columns, then the reward and one_hot(prev_action);
+ *   index 4, 5  post-ReLU value and advantage hidden layers [T*B, 512].
+ * Computes addresses only: nothing is launched or read. */
+int seedrl_debug_r2d2_net_views(const seedrl_r2d2_net* net, int T, int B, int index, size_t* offset, size_t* bytes);
 
 /* ---- plane-tensor convolution path (conv_mode 3) test hooks: single kernels of
  * csrc/conv_planes.cu, so the GPU parity tests can localise a failure.  Not on the product path. */

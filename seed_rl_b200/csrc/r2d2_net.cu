@@ -293,3 +293,23 @@ extern "C" int seedrl_r2d2_net_check_error(const seedrl_r2d2_net* n, int T, int 
   SEEDRL_CHECK_ARG(ws_bytes >= pl.total, "workspace too small");
   return read_error_flag(W<int>(ws, pl.tcerr), (cudaStream_t)stream, "unroll");
 }
+
+// Where the post-ReLU activations of the last forward sit in a (T, B) workspace (host arithmetic only).
+extern "C" int seedrl_debug_r2d2_net_views(const seedrl_r2d2_net* n, int T, int B, int index, size_t* offset,
+                                           size_t* bytes) {
+  SEEDRL_CHECK_ARG(n && offset && bytes && T >= 1 && B >= 1, "bad arguments");
+  SEEDRL_CHECK_ARG(index >= 0 && index <= 5, "index must be 0..5");
+  const RPlan pl = r_plan(n, T, B);
+  if (index <= 2) {
+    const StridedConv& c = n->conv[index];
+    *offset = pl.act[index];
+    *bytes = pl.N * c.hout * c.wout * (size_t)c.cout * 4;
+  } else if (index == 3) {
+    *offset = pl.core.xc;
+    *bytes = pl.N * (size_t)n->core.core_in * 4;
+  } else {
+    *offset = index == 4 ? pl.vh : pl.ah;
+    *bytes = pl.N * kRH * 4;
+  }
+  return SEEDRL_OK;
+}

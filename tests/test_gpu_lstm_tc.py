@@ -147,12 +147,13 @@ def test_r2d2_step_B64_with_tc3_recurrence_matches_oracle():
 
   Two tensors do not meet that rule and are held to 1e-2 instead: the advantage stream's hidden layer
   (kernel 6.4e-3, bias 6.7e-3 measured on an H100; 1.3e-3 with the fp32 recurrence, oracle 1e-6 response
-  1.6e-4).  No defect of the recurrence shows: test_gpu_lstm_recurrence.py measures 'tc3' alone at H = 512,
-  T1 = 141, B = 64 (Keras initialisation, resets) 2.2e-6 (hs) and 1.1e-6 (dU = hp^T dz) of the max-abs away
-  from a float64 LSTM, 100x under its bar there (8x the float64 response to a 2^-16 input perturbation) and
-  10x the fp32 modes' 2e-7.  The carve-out is consistent with that ratio (6.4e-3 against 1.3e-3 with the fp32
-  recurrence); what in the step amplifies a difference of that size was not measured.  Every other tensor meets
-  max(6e-3, 4x the oracle's response)."""
+  1.6e-4).  The cause is the step's kinks, not arithmetic: the fp32 oracle makes its own ReLU decisions, and
+  units that sit within rounding of zero take the other side in the oracle than on the GPU.  Perturbing every
+  parameter by 2^-16 moves the float64 gradient of this tensor by 8.7e-3 with the decisions free, and by 5.2e-5
+  with them held.  test_gpu_r2d2_float64.py runs this same step against a float64 reference that shares the
+  GPU's ReLU masks and greedy actions: there advantage/hidden/kernel is 3.9e-5 and the bias 2.0e-5 off, against
+  bars of 4.1e-4 and 2.8e-4.  This test keeps pinning the wiring to the oracle; that one pins the precision.
+  Every other tensor meets max(6e-3, 4x the oracle's response)."""
   import test_gpu_fullsize_r2d2 as F
   from oracle import optim_oracle
   from seed_rl_b200.agents.r2d2 import learner

@@ -396,6 +396,39 @@ def test_sgemm_kernel(ta, tb, M, N, K):
   assert _relerr(Cc.cpu().numpy(), want) < 1e-5
 
 
+# rows x width of the value head at the R2D2 suffix (101 x 64) and full (141 x 64) unroll, a row count that is odd
+# and not a multiple of 128 or 8, a width that is not a multiple of 32, tiny shapes
+@pytest.mark.parametrize('path,rows,width', [('rowdot', 6464, 512), ('rowdot', 9024, 512), ('rowdot', 6463, 500),
+                                             ('rowdot', 37, 31), ('colsum', 6464, 512), ('colsum', 9024, 512),
+                                             ('colsum', 6463, 512), ('colsum', 6465, 500), ('colsum', 33, 31)])
+def test_sgemm_n1_paths(path, rows, width):
+  """The two N = 1 paths of sgemm, which an epilogue flag turns off (test_sgemm_kernel sets them all):
+  rowdot_kernel, C[rows] = X w + bias (the value head), and the weighted colsum_kernel, C[width] = X^T d (its weight
+  gradient).  Each element within 1e-5 of the sum of the absolute products it adds, against float64: a dropped row
+  or column term is ~1/rows (1/width) of that."""
+  from seed_rl_b200 import _lib
+  rng = np.random.default_rng(rows * 7 + width)
+  X = rng.normal(size=(rows, width)).astype(np.float32)
+  v = rng.normal(size=width if path == 'rowdot' else rows).astype(np.float32)
+  bias = rng.normal(size=1).astype(np.float32)
+  X64, v64 = X.astype(np.float64), v.astype(np.float64)
+  out = _cuda(np.full(rows if path == 'rowdot' else width + 1, np.nan, np.float32))
+  Xc, vc, biasc = _cuda(X), _cuda(v), _cuda(bias)
+  if path == 'rowdot':
+    want, scale = X64 @ v64 + bias[0], np.abs(X64) @ np.abs(v64) + abs(float(bias[0]))
+    args = (0, 0, rows, 1, width, _lib.ptr(Xc), width, _lib.ptr(vc), 1, _lib.ptr(out), 1, _lib.ptr(biasc))
+  else:
+    want, scale = X64.T @ v64, np.abs(X64).T @ np.abs(v64)
+    args = (1, 0, width, 1, rows, _lib.ptr(Xc), width, _lib.ptr(vc), 1, _lib.ptr(out), 1, None)
+  _lib.check(_lib.lib().seedrl_debug_sgemm(*args, None, 0, 0, 0, 0, _lib.stream_ptr()))
+  got = out.cpu().numpy()
+  if path == 'colsum':
+    assert np.isnan(got[width])                         # nothing written past the output
+    got = got[:width]
+  err = np.abs(got.astype(np.float64) - want) / scale
+  assert err.max() < 1e-5, (float(err.max()), int(err.argmax()))
+
+
 # ---------------------------------------------------------------- (a5) network
 def _make_agent(net, A, seed=0):
   from seed_rl_b200.dmlab import networks
