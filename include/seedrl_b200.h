@@ -582,6 +582,23 @@ int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, co
  *   index 4, 5  post-ReLU value and advantage hidden layers [T*B, 512].
  * Computes addresses only: nothing is launched or read. */
 int seedrl_debug_r2d2_net_views(const seedrl_r2d2_net* net, int T, int B, int index, size_t* offset, size_t* bytes);
+/* The same for a seedrl_net (ImpalaDeep / ImpalaShallow) workspace of a (T1, B) call: the buffers that hold the
+ * ReLU and max-pool decisions of the last forward (rows = the T1 * B frames, time-major; the backward does not
+ * overwrite them).  *format: 0 fp32 NHWC, 1 a plane tensor (decode with seedrl_debug_from_planes), 2 uint8 taps
+ * [N, Ho, Wo, C] of the max-pool's first maximum, kh * 3 + kw from the TF-'SAME' window start.
+ * ImpalaDeep, index 5 s + j for stack s = 0..2 (C = 16, 32, 32 channels at the pooled resolution):
+ *   j = 0  pooled activation p, before the ReLU of res block 0;
+ *   j = 1  c0 = conv00(relu(p))        conv mode 3: relu(c0);
+ *   j = 2  o0 = conv01(relu(c0)) + p   conv mode 3: relu(o0);
+ *   j = 3  c1 = conv10(relu(o0))       conv mode 3: relu(c1);   (fp32 in conv modes 0-2, planes in mode 3)
+ *   j = 4  the max-pool taps;
+ * index 15 the last stack's o1 (fp32, before the ReLU Dense reads it through); index 16 the core input
+ * [T1*B, 256 + 1 + num_actions], the post-ReLU Dense(256) output in its first 256 columns.
+ * ImpalaShallow: index 0, 1 post-ReLU conv0 / conv1 outputs (fp32 NHWC), 2 the core input.
+ * The mask of each ReLU is its buffer > 0.  Another index, or T1, B < 1, returns SEEDRL_ERR_INVALID_ARGUMENT.
+ * Computes addresses only: nothing is launched or read. */
+int seedrl_debug_net_views(const seedrl_net* net, int T1, int B, int index, size_t* offset, size_t* bytes,
+                           int* format);
 
 /* ---- plane-tensor convolution path (conv_mode 3) test hooks: single kernels of
  * csrc/conv_planes.cu, so the GPU parity tests can localise a failure.  Not on the product path. */

@@ -199,6 +199,9 @@ SIGNATURES = {
         (c_int, [c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, c_size_t, P, P]),
     'seedrl_debug_r2d2_net_views':
         (c_int, [P, c_int, c_int, c_int, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
+    'seedrl_debug_net_views':
+        (c_int, [P, c_int, c_int, c_int, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t),
+                 ctypes.POINTER(c_int)]),
 }
 
 _lib = None

@@ -559,6 +559,41 @@ extern "C" int seedrl_net_check_error(const seedrl_net* n, int T1, int B, void* 
   return read_error_flag(W<int>(ws, pl.tcerr), (cudaStream_t)stream, "step");
 }
 
+// Where the ReLU and max-pool decisions of the last forward sit in a (T1, B) workspace (host arithmetic only).
+extern "C" int seedrl_debug_net_views(const seedrl_net* n, int T1, int B, int index, size_t* offset, size_t* bytes,
+                                      int* format) {
+  SEEDRL_CHECK_ARG(n && offset && bytes && format && T1 >= 1 && B >= 1, "bad arguments");
+  const Plan pl = make_plan(n, T1, B);
+  const size_t N = pl.N;
+  const bool deep = n->cfg.net == SEEDRL_NET_DEEP;
+  const int last = deep ? 16 : 2;
+  SEEDRL_CHECK_ARG(index >= 0 && index <= last, deep ? "index must be 0..16" : "index must be 0..2");
+  if (index == last) {
+    *offset = pl.core.xc; *bytes = N * (size_t)n->core.core_in * 4; *format = 0;
+  } else if (!deep) {
+    const StridedConv& l = n->sh[index];
+    *offset = index == 0 ? pl.sh_a1 : pl.sh_a2; *bytes = N * l.hout * l.wout * (size_t)l.cout * 4; *format = 0;
+  } else if (index == 15) {
+    const Stack& k = n->stacks.back();
+    *offset = pl.st.back().o1; *bytes = N * k.hout * k.wout * (size_t)k.c * 4; *format = 0;
+  } else {
+    const Stack& k = n->stacks[index / 5];
+    const StackBufs& b = pl.st[index / 5];
+    const int j = index % 5;
+    const size_t pooled = N * k.hout * k.wout * (size_t)k.c;
+    if (j == 4) {
+      *offset = b.idx; *bytes = pooled; *format = 2;
+    } else if (n->conv_mode == 3) {
+      const size_t off[4] = {b.praw, b.c0r, b.o0relu, b.c1r};
+      *offset = off[j]; *bytes = planes_bytes(pl.N, k.hout, k.wout, k.c); *format = 1;
+    } else {
+      const size_t off[4] = {b.p, b.c0, b.o0, b.c1};
+      *offset = off[j]; *bytes = pooled * 4; *format = 0;
+    }
+  }
+  return SEEDRL_OK;
+}
+
 // ---- backward -------------------------------------------------------------------
 static int conv_bwd(Call& c, const ConvLayer& l, int N, int H, int Wd, const void* x, int x_mode, const float* dy,
                     const float* dmask, const float* dres, float* dx) {
