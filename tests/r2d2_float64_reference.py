@@ -16,6 +16,9 @@ r2d2_oracle.stack_frames, optim_oracle.keras_adam_step), with two differences:
     decisions a GPU step made (its ReLU outputs > 0, the first maximum of its q), the reference is a smooth
     function of the parameters and the inputs, so its distance to that step measures arithmetic alone.
 
+`forward` is the network part alone over T >= 1 steps (central inference: T = 1), conditioned the same way, and
+`priorities` the initial priorities central inference computes from a completed unroll's behaviour q.
+
 The forward values of a ReLU are continuous through its kink, so the burn-in unrolls and the target network need
 no conditioning: they always use their own masks.
 """
@@ -30,19 +33,23 @@ MASKS = ('conv0', 'conv1', 'conv2', 'dense', 'value', 'advantage')
 
 
 class _Relu(object):
-  """z * mask, mask = z > 0 or the given one; records the masks it used ([rows, ...] bool numpy)."""
+  """z * mask, mask = z > 0 or the given one; records the masks it used ([rows, ...] bool numpy), the
+  pre-activations (`acts`) and, where a given mask differs from z > 0, |z| there (`ties`)."""
 
   def __init__(self, given=None):
-    self.given, self.used = given, {}
+    self.given, self.used, self.acts, self.ties = given, {}, {}, {}
 
   def __call__(self, name, z):
+    own = z.detach() > 0
     if self.given is None:
-      m = z.detach() > 0
+      m = own
     else:
       m = torch.as_tensor(np.asarray(self.given[name], bool))
       if tuple(m.shape) != tuple(z.shape):
         raise ValueError('mask %s has shape %s, the layer %s' % (name, tuple(m.shape), tuple(z.shape)))
+      self.ties[name] = z.detach()[m != own].abs().numpy()
     self.used[name] = m.numpy()
+    self.acts[name] = z.detach().numpy()
     return z * m.to(z.dtype)
 
 
@@ -120,6 +127,42 @@ def n_step_bellman_target(rewards, done, q_target, gamma, n_steps, F):
   return target
 
 
+def n_step_targets(target_q, greedy, reward, done, st, F):
+  """The rescaled n-step double-DQN targets of rows 0..T-2: target_q [T,B,A] at the greedy actions [T,B]."""
+  T, B = np.shape(greedy)
+  tt, bb = np.meshgrid(np.arange(T), np.arange(B), indexing='ij')
+  qtarget_max = inverse_value_function_rescaling(np.asarray(target_q)[tt, bb, greedy], st.eps, F)
+  return value_function_rescaling(n_step_bellman_target(reward, done, qtarget_max, st.gamma, st.n_steps, F)[1:],
+                                  st.eps, F)
+
+
+def priorities(q, target_q, action, reward, done, greedy, st, F):
+  """The step's priorities [B] from given q-values alone (numpy, in F): the initial priorities of a completed
+  unroll, which central inference computes with q = target_q = the behaviour q of the suffix."""
+  q = np.asarray(q, F)
+  T, B = np.shape(greedy)
+  td = n_step_targets(target_q, greedy, reward, done, st, F) - np.take_along_axis(
+      q, np.asarray(action).astype(np.int64)[..., None], axis=2)[:-1, :, 0]
+  abs_td = np.abs(td).astype(F)
+  return (F(st.eta) * abs_td.max(axis=0) + F(1 - st.eta) * abs_td.mean(axis=0, dtype=F)).astype(F)
+
+
+def forward(params, inputs, num_actions, stack_size, dtype=torch.float64, masks=None):
+  """The network's forward over T >= 1 steps (central inference: T = 1), without gradients.  inputs:
+  prev_actions, reward, done [T,B], observation uint8 [T,B,H,W,1], h0 / c0 [B,512] (any float dtype) and, when
+  stack_size > 1, frame_state int32 [B, H*W]; masks as in `step` (rows = the T * B frames, time-major).
+  Returns a dict: q [T,B,A], h, c, frame_state (the state after the last step), acts (the ReLU inputs), masks
+  and ties (see _Relu)."""
+  p = {k: torch.as_tensor(np.asarray(v)).to(dtype) for k, v in params.items()}
+  state = (torch.as_tensor(np.asarray(inputs['h0'])).to(dtype), torch.as_tensor(np.asarray(inputs['c0'])).to(dtype),
+           inputs['frame_state'] if stack_size > 1 else ())
+  relu = _Relu(masks)
+  with torch.no_grad():
+    q, (h, c, fs) = _unroll(p, inputs, state, num_actions, stack_size, dtype, relu)
+  return dict(q=q.numpy(), h=h.numpy(), c=c.numpy(), frame_state=fs, acts=relu.acts, masks=relu.used,
+              ties=relu.ties)
+
+
 # ---- the step ----------------------------------------------------------------------------------------------------
 Settings = collections.namedtuple('Settings', 'num_actions stack_size gamma burn_in n_steps eps clip_norm lr '
                                               'adam_eps eta')
@@ -163,10 +206,7 @@ def step(params, target_params, batch, st, dtype=torch.float64, masks=None, gree
   a_star = qn.argmax(-1) if greedy is None else np.asarray(greedy)
   if a_star.shape != (T, B):
     raise ValueError('greedy must be [%d, %d]' % (T, B))
-  tt, bb = np.meshgrid(np.arange(T), np.arange(B), indexing='ij')
-  qtarget_max = inverse_value_function_rescaling(qtn[tt, bb, a_star], st.eps, F)
-  target = value_function_rescaling(n_step_bellman_target(suf['reward'], suf['done'], qtarget_max, st.gamma,
-                                                          st.n_steps, F)[1:], st.eps, F)
+  target = n_step_targets(qtn, a_star, suf['reward'], suf['done'], st, F)
   replay_q = torch.gather(q, 2, torch.as_tensor(np.asarray(suf['action'])).long()[..., None])[..., 0][:-1]
   td = torch.as_tensor(target) - replay_q
   loss = 0.5 * (td * td).sum(dim=0)

@@ -84,11 +84,12 @@ def _shape(net, name, N):
   return (N, hw, hw, c)
 
 
-def _read_views(agent, net, T1, Bn):
-  """{reference name: the GPU buffer as a CPU array} (fp32 NHWC / decoded planes / uint8 taps)."""
+def _read_views(agent, net, T1, Bn, ws=None):
+  """{reference name: the GPU buffer as a CPU array} (fp32 NHWC / decoded planes / uint8 taps) of the (T1, Bn)
+  workspace `ws` (default: the agent's own)."""
   from seed_rl_b200 import _lib
   L = _lib.lib()
-  ws = agent.workspace(T1, Bn)
+  ws = agent.workspace(T1, Bn) if ws is None else ws
   N = T1 * Bn
   out = {}
   for i, name, _ in _view_names(net, agent.conv_mode):

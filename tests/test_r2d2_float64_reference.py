@@ -6,6 +6,9 @@ another implementation's ReLU masks and greedy actions (tests/test_gpu_r2d2_floa
   * conditioning on its own decisions changes nothing, bit for bit; a flipped mask or greedy action changes only
     the rows that depend on it;
   * float64 and float32 agree to fp32 rounding where they make the same decisions;
+  * its `forward` (central inference's T-step forward) in float32 is oracle/r2d2_net_oracle.py's unroll, final
+    state included; K chained one-step calls are one K-step call; conditioning on its own masks changes nothing;
+    `priorities` restates the step's;
   * seedrl_debug_r2d2_net_views names disjoint buffers of the sizes the masks need, inside the workspace.
 """
 import ctypes
@@ -145,6 +148,66 @@ def test_float64_and_float32_agree_to_fp32_rounding():
   # the forward to a few fp32 roundings; the TD errors cancel (target - q) and carry that into the rest
   assert errs['q'] < 2e-6 and errs['target_q'] < 2e-6, errs
   assert errs[worst] < 1e-4, errs
+
+
+def _inputs(b, t0=0, t1=None, h0=None, c0=None, frame_state=None):
+  """forward's inputs: rows t0..t1-1 of the batch, from the given state (default the batch's)."""
+  keys = ('prev_actions', 'reward', 'done', 'observation')
+  return dict({k: b[k][t0:t1] for k in keys}, h0=b['h0'] if h0 is None else h0, c0=b['c0'] if c0 is None else c0,
+              frame_state=b['frame_state'] if frame_state is None else frame_state)
+
+
+def test_float32_forward_is_the_oracle_unroll():
+  params, _, b, _ = _problem()
+  state = NO.AgentState((torch.as_tensor(b['h0']), torch.as_tensor(b['c0'])), b['frame_state'])
+  out, new_state = NO.unroll({k: torch.as_tensor(v) for k, v in params.items()}, b['prev_actions'], b['reward'],
+                             b['done'], b['observation'], state, A, S)
+  r = RF.forward(params, _inputs(b), A, S, torch.float32)
+  np.testing.assert_array_equal(r['q'], out.q_values.numpy())
+  np.testing.assert_array_equal(r['h'], new_state.core_state[0].numpy())
+  np.testing.assert_array_equal(r['c'], new_state.core_state[1].numpy())
+  np.testing.assert_array_equal(r['frame_state'], new_state.frame_stacking_state)
+  np.testing.assert_array_equal(r['q'].argmax(-1), out.action.numpy())
+
+
+def test_chained_one_step_forwards_are_one_unroll():
+  """T calls of one step, each from the state (h, c and the frame-stacking state) the previous one returned,
+  across the batch's done-resets, equal one T-step call in float64; so do two calls of 4 and T-4 steps."""
+  params, _, b, _ = _problem()
+  assert b['done'].any(axis=0).sum() >= 2
+  whole = RF.forward(params, _inputs(b), A, S, torch.float64)
+  for cuts in ([(t, t + 1) for t in range(T)], [(0, 4), (4, T)]):
+    h, c, fs, q = b['h0'], b['c0'], b['frame_state'], []
+    for t0, t1 in cuts:
+      r = RF.forward(params, _inputs(b, t0, t1, h, c, fs), A, S, torch.float64)
+      h, c, fs = r['h'], r['c'], r['frame_state']
+      q.append(r['q'])
+    errs = {'q': _relmax(np.concatenate(q), whole['q']), 'h': _relmax(h, whole['h']), 'c': _relmax(c, whole['c'])}
+    assert max(errs.values()) < 1e-12, (cuts, errs)
+    np.testing.assert_array_equal(fs, whole['frame_state'])
+
+
+def test_forward_conditioned_on_its_own_masks_changes_nothing():
+  params, _, b, _ = _problem()
+  r0 = RF.forward(params, _inputs(b, 5, 6), A, S, torch.float64)
+  r1 = RF.forward(params, _inputs(b, 5, 6), A, S, torch.float64, masks=r0['masks'])
+  for k in ('q', 'h', 'c', 'frame_state'):
+    np.testing.assert_array_equal(r1[k], r0[k], err_msg=k)
+  for k in RF.MASKS:
+    np.testing.assert_array_equal(r1['acts'][k], r0['acts'][k], err_msg=k)
+    np.testing.assert_array_equal(r0['masks'][k], r0['acts'][k] > 0, err_msg=k)
+  assert set(r1['ties']) == set(RF.MASKS) and all(v.size == 0 for v in r1['ties'].values())
+  assert r0['masks']['dense'].shape == (B, 512)
+
+
+@pytest.mark.parametrize('dtype', [torch.float32, torch.float64])
+def test_priorities_restate_the_step(dtype):
+  _, _, b, st = _problem()
+  r = _run(dtype)
+  F = np.float64 if dtype == torch.float64 else np.float32
+  got = RF.priorities(r['q'], r['target_q'], b['action'][BURN_IN:], b['reward'][BURN_IN:], b['done'][BURN_IN:],
+                      r['greedy'], st, F)
+  np.testing.assert_array_equal(got, r['priorities'])
 
 
 def test_debug_views_are_disjoint_buffers_of_the_mask_sizes():

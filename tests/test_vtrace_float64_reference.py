@@ -7,6 +7,8 @@ another implementation's ReLU masks and max-pool taps (tests/test_gpu_vtrace_flo
     so overlapping windows sum in the same order); a flipped mask or tap at frame (t, b) changes only the rows of
     column b from t up to the next done-reset;
   * float64 and float32 agree to fp32 rounding where they make the same decisions;
+  * its `forward` (central inference's T1-step forward) in float32 is oracle/net_oracle.py's unroll, final state
+    included; K chained one-step calls are one K-step call; conditioning on its own decisions changes nothing;
   * seedrl_debug_net_views names disjoint buffers of the sizes and formats the decisions need, inside the
     workspace, in every conv mode.
 """
@@ -144,6 +146,57 @@ def test_a_flipped_decision_changes_only_the_rows_that_depend_on_it(net, name):
   for k in ('dlogits', 'dbaseline'):
     np.testing.assert_array_equal(np.delete(r1[k], b, axis=1), np.delete(r0[k], b, axis=1), err_msg=k)
   assert r1['total'] != r0['total']
+
+
+def _inputs(b, t0=0, t1=None, h0=None, c0=None):
+  """forward's inputs: rows t0..t1-1 of the batch, from state (h0, c0) (default the batch's)."""
+  keys = ('prev_actions', 'reward', 'done', 'observation')
+  return dict({k: b[k][t0:t1] for k in keys}, h0=b['h0'] if h0 is None else h0, c0=b['c0'] if c0 is None else c0)
+
+
+@pytest.mark.parametrize('net', ['deep', 'shallow'])
+def test_float32_forward_is_the_oracle_unroll(net):
+  params, b, _ = _problem(net)
+  logits, baseline, (h, c) = net_oracle.unroll(
+      net, net_oracle.to_torch(params), torch.as_tensor(b['prev_actions']), torch.as_tensor(b['reward']),
+      torch.as_tensor(b['done']), torch.as_tensor(b['observation']), (torch.as_tensor(b['h0']),
+                                                                     torch.as_tensor(b['c0'])), A)
+  r = RF.forward(net, params, _inputs(b), torch.float32)
+  for k, v in (('logits', logits), ('baseline', baseline), ('h', h), ('c', c)):
+    np.testing.assert_array_equal(r[k], v.detach().numpy(), err_msg=k)
+  # the step's forward is this one
+  np.testing.assert_array_equal(r['logits'], _run(net, torch.float32)['logits'])
+
+
+@pytest.mark.parametrize('net', ['deep', 'shallow'])
+def test_chained_one_step_forwards_are_one_unroll(net):
+  """T+1 calls of one step, each from the state the previous one returned, across the done-resets of every
+  column (rows 2, 3 and 4), equal one (T+1)-step call in float64; so do two calls of 2 and T-1 steps."""
+  params, b, _ = _problem(net)
+  whole = RF.forward(net, params, _inputs(b), torch.float64)
+  for cuts in ([(t, t + 1) for t in range(T + 1)], [(0, 2), (2, T + 1)]):
+    h, c, logits, baseline = b['h0'], b['c0'], [], []
+    for t0, t1 in cuts:
+      r = RF.forward(net, params, _inputs(b, t0, t1, h, c), torch.float64)
+      h, c = r['h'], r['c']
+      logits.append(r['logits']); baseline.append(r['baseline'])
+    errs = {'logits': _relmax(np.concatenate(logits), whole['logits']),
+            'baseline': _relmax(np.concatenate(baseline), whole['baseline']),
+            'h': _relmax(h, whole['h']), 'c': _relmax(c, whole['c'])}
+    assert max(errs.values()) < 1e-12, (cuts, errs)
+
+
+@pytest.mark.parametrize('net', ['deep', 'shallow'])
+def test_forward_conditioned_on_its_own_decisions_changes_nothing(net):
+  params, b, _ = _problem(net)
+  r0 = RF.forward(net, params, _inputs(b, 2, 3), torch.float64)
+  r1 = RF.forward(net, params, _inputs(b, 2, 3), torch.float64, masks=r0['masks'], taps=r0['taps'])
+  for k in ('logits', 'baseline', 'h', 'c'):
+    np.testing.assert_array_equal(r1[k], r0[k], err_msg=k)
+  for k in r0['acts']:
+    np.testing.assert_array_equal(r1['acts'][k], r0['acts'][k], err_msg=k)
+  assert all(v.size == 0 for v in r1['ties'].values()) and set(r1['ties']) == set(RF.MASKS[net] + RF.POOLS[net])
+  assert r0['masks']['dense'].shape == (B, 256)
 
 
 def test_a_tap_outside_the_image_is_an_error():

@@ -21,6 +21,7 @@ Decision names (masks over the T+1 * B frames, time-major, NHWC or [rows, units]
                  between their convolutions), 'o1' (the last stack's output, ReLU'd as Dense reads it), 'dense';
                  pools 'stack<s>/pool': uint8 taps [N, Ho, Wo, C], kh * 3 + kw from the TF-'SAME' window start.
   ImpalaShallow  'conv0', 'conv1', 'dense'; no pools.
+`forward` is the network part alone over T1 >= 1 steps (central inference: T1 = 1), returning the final state too.
 Nothing else needs sharing: the V-trace clips enter the loss as stop-gradient values that are continuous in the
 logits, log-softmax, entropy and the LSTM are smooth, and done-resets and the reward clip act on inputs.
 """
@@ -140,7 +141,7 @@ def _torso(net, p, prev_action, reward, frame, A, dtype, dec):
 
 
 def _unroll(net, p, batch, A, dtype, dec):
-  """net_oracle.unroll in `dtype`: -> logits [T1,B,A], baseline [T1,B]."""
+  """net_oracle.unroll in `dtype`: -> logits [T1,B,A], baseline [T1,B], the final (h, c) [B,256]."""
   prev_actions = torch.as_tensor(np.asarray(batch['prev_actions']))
   T1, B = prev_actions.shape
   frame = torch.as_tensor(np.asarray(batch['observation']))
@@ -159,7 +160,7 @@ def _unroll(net, p, batch, A, dtype, dec):
   core = torch.stack(outs)
   logits = core @ p['policy_logits/kernel'] + p['policy_logits/bias']
   baseline = (core @ p['baseline/kernel'] + p['baseline/bias'])[..., 0]
-  return logits, baseline
+  return logits, baseline, (h, c)
 
 
 # ---- compute_loss after the unroll: loss_oracle / vtrace_oracle restated in `dtype` -------------------------------
@@ -259,7 +260,7 @@ def step(net, params, batch, cfg, dtype=torch.float64, masks=None, taps=None):
   ecp_value = np.float32(np.log(cfg.entropy_cost) / mul)            # the fp32 parameter both sides hold
   ecp = torch.tensor(float(ecp_value), dtype=dtype, requires_grad=True)
   dec = _Decisions(masks, taps)
-  logits, baseline = _unroll(net, p, batch, A, dtype, dec)
+  logits, baseline, _ = _unroll(net, p, batch, A, dtype, dec)
   logits.retain_grad()
   baseline.retain_grad()
   total, logs = compute_loss(cfg, logits, baseline, batch, ecp, dtype)
@@ -282,6 +283,20 @@ def step(net, params, batch, cfg, dtype=torch.float64, masks=None, taps=None):
               logs=collections.OrderedDict((k, float(v.detach())) for k, v in logs.items() if k not in skip),
               dlogits=logits.grad.numpy().copy(), dbaseline=baseline.grad.numpy().copy(), acts=dec.acts, grads=g,
               params_after=after, update=update, masks=dec.masks, taps=dec.taps, ties=dec.ties)
+
+
+def forward(net, params, inputs, dtype=torch.float64, masks=None, taps=None):
+  """The network's forward over T1 >= 1 steps (central inference: T1 = 1), without gradients.  inputs:
+  prev_actions [T1,B], reward, done [T1,B], observation [T1,B,H,W,C] uint8, h0 / c0 [B,256] (any float dtype);
+  params, masks and taps as in `step` (rows = the T1 * B frames, time-major).  Returns a dict: logits [T1,B,A],
+  baseline [T1,B], h, c (the state after the last step), acts, masks, taps and ties (see _Decisions)."""
+  A = np.shape(params['policy_logits/bias'])[0]
+  p = {k: torch.as_tensor(np.asarray(v)).to(dtype) for k, v in params.items()}
+  dec = _Decisions(masks, taps)
+  with torch.no_grad():
+    logits, baseline, (h, c) = _unroll(net, p, inputs, A, dtype, dec)
+  return dict(logits=logits.numpy(), baseline=baseline.numpy(), h=h.numpy(), c=c.numpy(), acts=dec.acts,
+              masks=dec.masks, taps=dec.taps, ties=dec.ties)
 
 
 def perturbed(params, batch, delta, seed=0):
