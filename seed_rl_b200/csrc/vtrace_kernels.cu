@@ -90,12 +90,11 @@ __global__ void categorical_logprob_entropy_kernel(int N, int A, const float* __
   }
   se = warp_sum(se);
   sel = warp_sum(sel);
-  const float lse = m + logf(se);
   if (lane == 0) {
     if (logp) {
       int64_t a = actions[warp];
       a = a < 0 ? 0 : (a >= A ? A - 1 : a);
-      logp[warp] = l[a] - lse;
+      logp[warp] = (l[a] - m) - logf(se);   // not l[a] - (m + log se): m + log se rounds to ulp(m)
     }
     if (entropy) entropy[warp] = logf(se) - sel / se;   // H = lse - sum p*l
   }
@@ -150,7 +149,10 @@ __global__ void categorical_sample_kernel(int N, int A, const float* __restrict_
 //   phase C  thread-per-column reverse scan (vs, pg_adv) + loss partial sums
 //   phase D  thread-per-row gradient in place, written back with float4 stores
 // Per-CTA partial sums go to scratch[cta][8]; the last CTA to finish (ticket)
-// reduces them in index order (deterministic) and writes loss_terms.
+// reduces them in index order (deterministic) and writes loss_terms.  The loss sums are
+// float64 wherever they run long (the small kernel's per-thread sums, every block and grid
+// reduction): the means they make (mean value, policy loss, mean kl) are near zero against
+// terms of order one, so an fp32 running sum over T x B rows would decide their leading digits.
 constexpr int kLossThreads = 256;
 constexpr int kLossPartials = 8;
 
@@ -170,7 +172,7 @@ struct LossParams {
   float* d_ecp;
   float* vs_out;
   float* pg_out;
-  float* partials;        // [grid][8]
+  double* partials;       // [grid][8]
   unsigned int* ticket;   // self-resetting
 };
 
@@ -184,6 +186,25 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
   if (w == 0) {
     r = l < (blockDim.x >> 5) ? red[l] : 0.f;
     r = warp_sum(r);
+  }
+  return r;  // valid in warp 0
+}
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double block_reduce_sum_d(double v) {
+  __shared__ double red[32];
+  v = warp_sum_d(v);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  __syncthreads();
+  if (l == 0) red[w] = v;
+  __syncthreads();
+  double r = 0.0;
+  if (w == 0) {
+    r = l < (blockDim.x >> 5) ? red[l] : 0.0;
+    r = warp_sum_d(r);
   }
   return r;  // valid in warp 0
 }
@@ -210,7 +231,25 @@ __device__ __forceinline__ float block_reduce_max(float v, float* red) {
 // accumulators keep four loads / MUFU ops in flight per thread.  exp() is one FFMA/FMUL into
 // ex2.approx.ftz (<= 2 ulp plus 6e-8 |x| relative): the only terms it perturbs visibly are
 // the already-negligible ones; log() stays the accurate logf (two per row).
+//
+// A row's log-probabilities are log p_j = (l_j - a) - b for a pair (a, b) of the row maximum m
+// and lg = log sum_j exp(l_j - m) in [0, log A] (lse_pair).  Rows whose maximum is below
+// kSplitLseAbove in magnitude take a = m + lg, b = 0, and their exponents exp2(l_j log2 e -
+// m log2 e): one rounding each, the arithmetic of earlier versions bit for bit (a learner step's
+// result, and so a training run, is unchanged for ordinary logits).  Those forms round to an ulp
+// of m, 1e-5..1e-4 of every probability for logits of magnitude 1e2..1e3 (a peaked policy, a
+// large common offset), so larger maxima, and single-action rows (exactly log p = 0), take a = m,
+// b = lg and exp2((l_j - m) log2 e): l_j - m is exact for every entry that matters.
 constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kSplitLseAbove = 16.f;
+__device__ __forceinline__ bool split_lse(float m, int A) { return !(fabsf(m) < kSplitLseAbove && A > 1); }
+__device__ __forceinline__ void lse_pair(float m, float lg, int A, float* a, float* b) {
+  if (split_lse(m, A)) {
+    *a = m; *b = lg;
+  } else {
+    *a = m + lg; *b = 0.f;
+  }
+}
 __device__ __forceinline__ float ex2_ftz(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -271,14 +310,26 @@ __device__ __forceinline__ float row_max(const float* l, int A) {
 template <int AS>
 __device__ __forceinline__ float row_sumexp(const float* l, int A, float m) {
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-  const float nm2 = -m * kLog2e;
-  row_foreach<AS>(l, A,
-      [&](int, float x0, float x1, float x2, float x3) {
-        s0 += ex2_ftz(fmaf(x0, kLog2e, nm2)); s1 += ex2_ftz(fmaf(x1, kLog2e, nm2));
-        s2 += ex2_ftz(fmaf(x2, kLog2e, nm2)); s3 += ex2_ftz(fmaf(x3, kLog2e, nm2));
-      },
-      [&](int, float x0) { s0 += ex2_ftz(fmaf(x0, kLog2e, nm2)); });
+  auto sum = [&](auto ex) {
+    row_foreach<AS>(l, A,
+        [&](int, float x0, float x1, float x2, float x3) {
+          s0 += ex2_ftz(ex(x0)); s1 += ex2_ftz(ex(x1)); s2 += ex2_ftz(ex(x2)); s3 += ex2_ftz(ex(x3));
+        },
+        [&](int, float x0) { s0 += ex2_ftz(ex(x0)); });
+  };
+  if (split_lse(m, AS ? AS : A)) {
+    sum([&](float x) { return (x - m) * kLog2e; });         // m split off exactly
+  } else {
+    const float nm2 = -m * kLog2e;
+    sum([&](float x) { return fmaf(x, kLog2e, nm2); });     // m log2 e rounded: see lse_residual
+  }
   return (s0 + s1) + (s2 + s3);
+}
+// log sum_j exp(l_j - m) from the log of row_sumexp: rows that do not split off m summed
+// exp2(l_j log2 e - round(m log2 e)), which carries the factor 2^r of the rounding residual
+// r = m log2 e - round(m log2 e) (exact by one FMA); the split form removes it.
+__device__ __forceinline__ float lse_residual_free(float m, float lg, int A) {
+  return split_lse(m, A) ? lg : fmaf(-fmaf(m, kLog2e, -m * kLog2e), 0.6931471805599453f, lg);
 }
 // se = sum_j exp(d_j), sel = sum_j exp(d_j) d_j with d_j = l_j - m
 template <int AS>
@@ -295,15 +346,17 @@ __device__ __forceinline__ void row_sumexp_ent(const float* l, int A, float m, f
   *se = (s0 + s1) + (s2 + s3);
   *sel = (q0 + q1) + (q2 + q3);
 }
-// in place: l_j <- wpg (1[j=a] - p_j) + wec p_j (log p_j + H),  p_j = exp(l_j - lse)
+// in place: l_j <- wpg (1[j=a] - p_j) + wec p_j (log p_j + H),  log p_j = (l_j - la) - lb  (lse_pair)
 //   d(-mean(tlp*pg))/dl_j = -pg/N (1[j=a]-p_j); d(kc*mean(blp-tlp)) = -kc/N (1[j=a]-p_j)
 //   d(-ec*mean(H))/dl_j  = ec/N * p_j (log p_j + H)
 // evaluated as p_j (wec (log p_j + H) - wpg), then + wpg on the taken action.
 template <int AS>
-__device__ __forceinline__ void row_grad(float* l, int A_rt, int a, float lse, float ent, float wpg, float wec) {
+__device__ __forceinline__ void row_grad(float* l, int A_rt, int a, float la, float lb, float ent, float wpg,
+                                         float wec) {
   const int A = AS ? AS : A_rt;
+  auto run = [&](auto logp_of) {
   auto g1 = [&](float x) {
-    const float logp = x - lse;
+    const float logp = logp_of(x);
     const float pj = ex2_ftz(logp * kLog2e);
     return pj * fmaf(wec, logp + ent, -wpg);
   };
@@ -331,12 +384,17 @@ __device__ __forceinline__ void row_grad(float* l, int A_rt, int a, float lse, f
       for (; j < A; ++j) l[j] = g1(l[j]);
     }
   }
+  };
+  if (lb == 0.f)
+    run([&](float x) { return x - la; });              // (x - la) - 0, one rounding
+  else
+    run([&](float x) { return (x - la) - lb; });
   l[a] += wpg;
 }
 
 // Last CTA to arrive (ticket) reduces the per-CTA partials in index order and writes the
 // loss terms; deterministic for a given grid.
-__device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red, float ec, float invN) {
+__device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red, float ec) {
   const int tid = threadIdx.x;
   const float mul = p.cfg.entropy_cost_adjustment_speed;
   const float kc = p.cfg.kl_cost;
@@ -349,25 +407,27 @@ __device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red,
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  float acc6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  double acc5[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  float amax = 0.f;
   // deterministic: thread k sums slices k, k+256, ... then a fixed-order tree.
   for (unsigned int g = tid; g < gridDim.x; g += blockDim.x) {
-    const volatile float* q = p.partials + (size_t)g * kLossPartials;
+    const volatile double* q = p.partials + (size_t)g * kLossPartials;
 #pragma unroll
-    for (int k = 0; k < 5; ++k) acc6[k] += q[k];
-    acc6[5] = fmaxf(acc6[5], q[5]);
+    for (int k = 0; k < 5; ++k) acc5[k] += q[k];
+    amax = fmaxf(amax, (float)q[5]);
   }
-  float tot[6];
+  double tot[5];
 #pragma unroll
-  for (int k = 0; k < 5; ++k) tot[k] = block_reduce_sum(acc6[k], s_red);
-  tot[5] = block_reduce_max(acc6[5], s_red);
+  for (int k = 0; k < 5; ++k) tot[k] = block_reduce_sum_d(acc5[k]);
+  const float max_a = block_reduce_max(amax, s_red);
   if (tid == 0) {
-    const float policy_loss = -tot[0] * invN;
-    const float mse = tot[1] * invN;
+    const double n = (double)p.T * (double)p.B;
+    const float policy_loss = (float)(-tot[0] / n);
+    const float mse = (float)(tot[1] / n);
     const float v_loss = p.cfg.baseline_cost * 0.5f * mse;
-    const float mean_h = tot[2] * invN;
+    const float mean_h = (float)(tot[2] / n);
     const float entropy_loss = -ec * mean_h;
-    const float mean_kl = tot[3] * invN;
+    const float mean_kl = (float)(tot[3] / n);
     const float kl_loss = kc * mean_kl;
     float adj = 0.f, dparam = 0.f;
     if (p.cfg.has_target_entropy) {                        // :128-132
@@ -381,12 +441,12 @@ __device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red,
     L[SEEDRL_LT_ENTROPY] = entropy_loss;
     L[SEEDRL_LT_KL] = kl_loss;
     L[SEEDRL_LT_ENTROPY_ADJ] = adj;
-    L[SEEDRL_LT_V_MEAN] = tot[4] * invN;
+    L[SEEDRL_LT_V_MEAN] = (float)(tot[4] / n);
     L[SEEDRL_LT_V_L2_ERROR] = sqrtf(mse);
     L[SEEDRL_LT_MEAN_ENTROPY] = mean_h;
     L[SEEDRL_LT_ENTROPY_COST] = ec;
     L[SEEDRL_LT_MEAN_KL] = mean_kl;
-    L[SEEDRL_LT_MAX_ACTION_ABS] = tot[5];
+    L[SEEDRL_LT_MAX_ACTION_ABS] = max_a;
     for (int k = 12; k < SEEDRL_LOSS_TERMS; ++k) L[k] = 0.f;
     *p.d_ecp = dparam;
     *p.ticket = 0u;   // self-reset for the next launch
@@ -431,8 +491,9 @@ vtrace_loss_kernel(const LossParams p) {
   float* s_logits = smem;                      // [T][BB][A] dense, 16B-aligned rows of BB*A
   float* s_tlp = s_logits + (((size_t)rows * A + 3) & ~(size_t)3); // [rows] target logp -> later pg_adv
   float* s_blp = s_tlp + rows;                 // [rows] behaviour logp -> later v_err
-  float* s_lse = s_blp + rows;                 // [rows]
-  float* s_ent = s_lse + rows;                 // [rows]
+  float* s_la = s_blp + rows;                  // [rows] lse_pair a
+  float* s_lb = s_la + rows;                   // [rows] lse_pair b
+  float* s_ent = s_lb + rows;                  // [rows]
   float* s_rew = s_ent + rows;                 // [rows] clipped reward r_{t+1}
   float* s_dis = s_rew + rows;                 // [rows] discount
   float* s_val = s_dis + rows;                 // [(T+1)*BB]
@@ -463,6 +524,8 @@ vtrace_loss_kernel(const LossParams p) {
     s_val[i] = c < nb ? __ldg(p.lb + (size_t)t * B + b0 + c) : 0.f;
   }
 
+  double sum_tp = 0.0, sum_ve2 = 0.0, sum_h = 0.0, sum_kl = 0.0, sum_v = 0.0;
+
   // ---- phase A: behaviour logits ------------------------------------------
   tile_copy<true>(s_logits, p.bl + (size_t)b0 * A, T, B, A, BB, nb, tid);
   __syncthreads();
@@ -474,7 +537,11 @@ vtrace_loss_kernel(const LossParams p) {
       const float se = row_sumexp<0>(l, A, m);
       int a = s_act[i];
       a = a < 0 ? 0 : (a >= A ? A - 1 : a);
-      s_blp[i] = l[a] - (m + logf(se));                    // :97-98
+      const float lg = logf(se);
+      float la, lb;
+      lse_pair(m, lg, A, &la, &lb);
+      s_blp[i] = (l[a] - la) - lb;                         // :97-98, for rho
+      s_la[i] = (l[a] - m) - lse_residual_free(m, lg, A);  // split form, for the kl sum (until phase B)
     }
   }
   __syncthreads();
@@ -491,15 +558,22 @@ vtrace_loss_kernel(const LossParams p) {
       const float lg = logf(se);
       int a = s_act[i];
       a = a < 0 ? 0 : (a >= A ? A - 1 : a);
-      s_lse[i] = m + lg;
-      s_tlp[i] = l[a] - (m + lg);                          // :95-96
+      float la, lb;
+      lse_pair(m, lg, A, &la, &lb);
+      const float tl = (l[a] - la) - lb;                   // :95-96
+      const float tls = (l[a] - m) - lg;                   // split form: the loss sums
+      sum_kl += s_la[i] - tls;                             // :124
+      s_la[i] = la;
+      s_lb[i] = lb;
+      s_tlp[i] = tls;
+      s_blp[i] = tl - s_blp[i];                            // log rho
       s_ent[i] = lg - sel / se;                            // :119-120
     }
   }
   __syncthreads();
 
   // ---- phase C: reverse-time V-trace scan, one thread per column -----------
-  float sum_tp = 0.f, sum_ve2 = 0.f, sum_h = 0.f, sum_kl = 0.f, sum_v = 0.f, max_a = 0.f;
+  float max_a = 0.f;
   if (tid < nb) {
     const int c = tid;
     const bool hcr = !isnan(p.cfg.clip_rho_threshold);
@@ -508,8 +582,8 @@ vtrace_loss_kernel(const LossParams p) {
     float acc = 0.f, vs_next = bootv, v_next = bootv;
     for (int t = T - 1; t >= 0; --t) {
       const int i = t * BB + c;
-      const float tl = s_tlp[i], bp = s_blp[i];
-      const float rho = expf(tl - bp);
+      const float tl = s_tlp[i];
+      const float rho = expf(s_blp[i]);
       const float crho = hcr ? fminf(p.cfg.clip_rho_threshold, rho) : rho;
       const float cc = fminf(1.0f, rho) * p.cfg.lambda_;
       const float v = s_val[i], d = s_dis[i], r = s_rew[i];
@@ -524,7 +598,6 @@ vtrace_loss_kernel(const LossParams p) {
       sum_tp += tl * pg;                                   // :111-112
       sum_ve2 += verr * verr;                              // :116
       sum_h += s_ent[i];
-      sum_kl += bp - tl;                                   // :124
       sum_v += v;
       max_a = fmaxf(max_a, fabsf((float)s_act[i]));
       s_tlp[i] = pg;     // reuse: pg_adv
@@ -543,11 +616,10 @@ vtrace_loss_kernel(const LossParams p) {
     const int c = i % BB;
     if (c < nb) {
       float* l = s_logits + (size_t)i * A;
-      const float lse = s_lse[i], ent = s_ent[i];
       const float wpg = -(s_tlp[i] + kc) * invN, wec = ec * invN;
       int a = s_act[i];
       a = a < 0 ? 0 : (a >= A ? A - 1 : a);
-      row_grad<0>(l, A, a, lse, ent, wpg, wec);
+      row_grad<0>(l, A, a, s_la[i], s_lb[i], s_ent[i], wpg, wec);
     }
   }
   __syncthreads();
@@ -565,15 +637,15 @@ vtrace_loss_kernel(const LossParams p) {
   }
 
   // ---- per-CTA partials, then last-CTA finalisation -------------------------
-  float r;
-  float* part = p.partials + (size_t)blockIdx.x * kLossPartials;
-  r = block_reduce_sum(sum_tp, s_red);  if (tid == 0) part[0] = r;
-  r = block_reduce_sum(sum_ve2, s_red); if (tid == 0) part[1] = r;
-  r = block_reduce_sum(sum_h, s_red);   if (tid == 0) part[2] = r;
-  r = block_reduce_sum(sum_kl, s_red);  if (tid == 0) part[3] = r;
-  r = block_reduce_sum(sum_v, s_red);   if (tid == 0) part[4] = r;
+  double r;
+  double* part = p.partials + (size_t)blockIdx.x * kLossPartials;
+  r = block_reduce_sum_d(sum_tp);  if (tid == 0) part[0] = r;
+  r = block_reduce_sum_d(sum_ve2); if (tid == 0) part[1] = r;
+  r = block_reduce_sum_d(sum_h);   if (tid == 0) part[2] = r;
+  r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
+  r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  loss_finalize(p, s_red, ec, invN);
+  loss_finalize(p, s_red, ec);
 }
 
 
@@ -636,8 +708,9 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   float* s_tiles = smem;                             // [3] x [T][BB][A], 128-byte aligned each
   float* s_tlp = s_tiles + (size_t)3 * tile_stride_f;   // [rows] target logp
   float* s_acc = s_tlp + rows;                       // [rows] behaviour logp -> delta -> vs - V
-  float* s_lse = s_acc + rows;
-  float* s_ent = s_lse + rows;
+  float* s_la = s_acc + rows;                        // [rows] lse_pair a
+  float* s_lb = s_la + rows;                         // [rows] lse_pair b
+  float* s_ent = s_lb + rows;
   float* s_rew = s_ent + rows;
   float* s_dis = s_rew + rows;
   float* s_dc = s_dis + rows;                        // [rows] discount_t * c_t
@@ -668,6 +741,8 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   }
   __syncthreads();
 
+  // per-thread sums stay fp32 (a thread adds one or a few rows per tile); the block and grid
+  // reductions are float64
   float sum_tp = 0.f, sum_ve2 = 0.f, sum_h = 0.f, sum_kl = 0.f, sum_v = 0.f, max_a = 0.f;
   // one thread, one instruction per tile
   auto issue_load = [&](int k, const CUtensorMap* tm, int tile) {
@@ -744,7 +819,11 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
         const float* l = tileA + (size_t)i * A;
         const float m = row_max<AS>(l, A);
         const float se = row_sumexp<AS>(l, A, m);
-        s_acc[i] = l[s_act[i]] - (m + logf(se));           // :97-98
+        const float lg = logf(se);
+        float la, lb;
+        lse_pair(m, lg, A, &la, &lb);
+        s_acc[i] = (l[s_act[i]] - la) - lb;                // :97-98, for rho
+        s_dc[i] = (l[s_act[i]] - m) - lse_residual_free(m, lg, A);   // split form, for the kl sum
       }
     }
     __syncthreads();
@@ -766,14 +845,18 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
       row_sumexp_ent<AS>(l, A, m, &se, &sel);
       const float lg = logf(se);
       const int a = s_act[i];
-      const float tl = l[a] - (m + lg);                    // :95-96
+      float la, lb;
+      lse_pair(m, lg, A, &la, &lb);
+      const float tl = (l[a] - la) - lb;                   // :95-96
+      const float tls = (l[a] - m) - lg;                   // split form: the loss sums
       const float bp = s_acc[i];
       const float ent = lg - sel / se;                     // :119-120
-      s_lse[i] = m + lg;
-      s_tlp[i] = tl;
+      s_la[i] = la;
+      s_lb[i] = lb;
+      s_tlp[i] = tls;
       s_ent[i] = ent;
       sum_h += ent;
-      sum_kl += bp - tl;                                   // :124
+      sum_kl += s_dc[i] - tls;                             // :124
       const float rho = expf(tl - bp);                     // vtrace.py:84,110
       const float crho = hcr ? fminf(p.cfg.clip_rho_threshold, rho) : rho;
       const float cc = fminf(1.0f, rho) * p.cfg.lambda_;
@@ -834,7 +917,7 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
       if (p.vs_out) p.vs_out[g] = verr + v;
       if (p.pg_out) p.pg_out[g] = pg;
       p.dbaseline[g] = -p.cfg.baseline_cost * verr * invN;
-      row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_lse[i], s_ent[i], -(pg + kc) * invN, ec * invN);
+      row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_la[i], s_lb[i], s_ent[i], -(pg + kc) * invN, ec * invN);
     }
     // generic-proxy writes of the gradient tile -> visible to the TMA (async) proxy
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -857,20 +940,20 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 
   // ---- per-CTA partials, then last-CTA finalisation (same as vtrace_loss_kernel) ---------
-  float r;
-  float* part = p.partials + (size_t)blockIdx.x * kLossPartials;
-  r = block_reduce_sum(sum_tp, s_red);  if (tid == 0) part[0] = r;
-  r = block_reduce_sum(sum_ve2, s_red); if (tid == 0) part[1] = r;
-  r = block_reduce_sum(sum_h, s_red);   if (tid == 0) part[2] = r;
-  r = block_reduce_sum(sum_kl, s_red);  if (tid == 0) part[3] = r;
-  r = block_reduce_sum(sum_v, s_red);   if (tid == 0) part[4] = r;
+  double r;
+  double* part = p.partials + (size_t)blockIdx.x * kLossPartials;
+  r = block_reduce_sum_d(sum_tp);  if (tid == 0) part[0] = r;
+  r = block_reduce_sum_d(sum_ve2); if (tid == 0) part[1] = r;
+  r = block_reduce_sum_d(sum_h);   if (tid == 0) part[2] = r;
+  r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
+  r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  loss_finalize(p, s_red, ec, invN);
+  loss_finalize(p, s_red, ec);
 }
 
 static size_t loss_smem_bytes(int T, int A, int BB) {
   const size_t rows = (size_t)T * BB;
-  return (((rows * A + 3) & ~(size_t)3) + rows * 6 + (size_t)(T + 1) * BB + rows + 32) * 4;
+  return (((rows * A + 3) & ~(size_t)3) + rows * 7 + (size_t)(T + 1) * BB + rows + 32) * 4;
 }
 
 // Columns per CTA for vtrace_loss_kernel: the largest power of two <= 16 whose tile fits in
@@ -890,7 +973,7 @@ static int stream_tile_stride_f(int T, int A, int BB) {   // floats per ring buf
 }
 static size_t stream_smem_bytes(int T, int A, int BB) {
   const size_t rows = (size_t)T * BB;
-  return (3 * (size_t)stream_tile_stride_f(T, A, BB) + 8 * rows + (size_t)(T + 1) * BB + rows + 32) * 4 + 3 * 8 + 128;
+  return (3 * (size_t)stream_tile_stride_f(T, A, BB) + 9 * rows + (size_t)(T + 1) * BB + rows + 32) * 4 + 3 * 8 + 128;
 }
 
 static int num_sms() {
@@ -1075,7 +1158,7 @@ extern "C" int seedrl_categorical_sample_counter(int N, int A, const float* logi
 
 extern "C" size_t seedrl_vtrace_loss_scratch_bytes(int T1, int B, int A) {
   (void)T1; (void)A;   // one partial slot per CTA; at most one CTA per column
-  return 256 + (size_t)(B > kNumSMs ? B : kNumSMs) * kLossPartials * sizeof(float);
+  return 256 + (size_t)(B > kNumSMs ? B : kNumSMs) * kLossPartials * sizeof(double);
 }
 
 extern "C" int seedrl_vtrace_loss_fwd_bwd(
@@ -1098,7 +1181,7 @@ extern "C" int seedrl_vtrace_loss_fwd_bwd(
   p.loss_terms = loss_terms; p.dlogits = dlogits; p.dbaseline = dbaseline;
   p.d_ecp = d_entropy_cost_param; p.vs_out = vs_out; p.pg_out = pg_advantages_out;
   p.ticket = reinterpret_cast<unsigned int*>(scratch);
-  p.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + 256);
+  p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
   static bool attr_set = false;
   if (!attr_set) {
     SEEDRL_CUDA(cudaFuncSetAttribute(vtrace_loss_kernel,

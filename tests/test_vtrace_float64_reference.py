@@ -229,6 +229,62 @@ def test_float64_and_float32_agree_to_fp32_rounding(net):
   assert errs[worst] < 1e-4, errs
 
 
+# the shapes and settings of test_gpu_parity.py::test_vtrace_loss_fwd_bwd_vs_oracle
+_LOSS_CASES = [(21, 64, 18, {}),
+               (21, 64, 18, dict(kl_cost=0.3, entropy_cost=0.01, max_abs_reward=1.0, target_entropy=1.5, lambda_=0.9)),
+               (2, 1, 1, {}), (6, 3, 5, dict(kl_cost=0.1)), (21, 70, 18, {}), (101, 33, 9, {}), (4, 257, 2, {})]
+
+
+def _loss_inputs(T1, B, A, kw, seed=11):
+  from test_gpu_parity import _loss_case
+  c, _ = _loss_case(T1, B, A, seed)
+  cfg = loss_oracle.default_config(**kw)
+  ecp = np.float32(np.log(cfg.entropy_cost) / cfg.entropy_cost_adjustment_speed)
+  return cfg, [c[k] for k in ('ll', 'lb', 'bl', 'act', 'rew', 'done')], ecp
+
+
+@pytest.mark.parametrize('T1,B,A,kw', _LOSS_CASES)
+def test_float32_loss_and_grads_is_the_oracle(T1, B, A, kw):
+  """The loss-only reference in float32 is oracle/loss_oracle.loss_and_grads bit for bit: loss, the 11 logged
+  terms, d loss / d logits and d baseline, d loss / d entropy_cost_param, vs and the pg advantages."""
+  cfg, args, ecp = _loss_inputs(T1, B, A, kw)
+  total, logs, dl, db, dep, aux = loss_oracle.loss_and_grads(cfg, *args)
+  r = RF.loss_and_grads(cfg, *args, ecp, torch.float32)
+  assert r[0] == float(total)
+  assert list(r[1]) == list(logs) and len(logs) == 11
+  for k, v in logs.items():
+    assert r[1][k] == v, k
+  np.testing.assert_array_equal(r[2], dl)
+  np.testing.assert_array_equal(r[3], db)
+  assert r[4] == dep
+  np.testing.assert_array_equal(r[5], aux['vs'].numpy())
+  np.testing.assert_array_equal(r[6], aux['pg_advantages'].numpy())
+  assert r[2].dtype == r[3].dtype == r[5].dtype == np.float32
+  if kw.get('target_entropy'):
+    assert dep != 0.0
+
+
+@pytest.mark.parametrize('dtype', [torch.float32, torch.float64])
+def test_loss_and_grads_in_column_chunks_is_one_evaluation(dtype):
+  """Column chunks of 16 and of 48 (a ragged last chunk) give the one-chunk result: vs and the pg advantages bit for
+  bit, the gradients and the loss terms to the rounding of the means' divisors and of the float64 recombination."""
+  kw = dict(kl_cost=0.3, entropy_cost=0.01, max_abs_reward=1.0, target_entropy=1.5, lambda_=0.9)
+  cfg, args, ecp = _loss_inputs(21, 64, 18, kw)
+  whole = RF.loss_and_grads(cfg, *args, ecp, dtype)
+  tol = 1e-14 if dtype == torch.float64 else 1e-5
+  for chunk in (16, 48):
+    part = RF.loss_and_grads(cfg, *args, ecp, dtype, chunk=chunk)
+    for i in (5, 6):
+      np.testing.assert_array_equal(part[i], whole[i])
+    for i in (2, 3):
+      assert _relmax(part[i], whole[i]) < tol, (chunk, i, _relmax(part[i], whole[i]))
+    assert abs(part[0] - whole[0]) <= tol * abs(whole[0])
+    assert abs(part[4] - whole[4]) <= tol * abs(whole[4])
+    assert list(part[1]) == list(whole[1])
+    for k in whole[1]:
+      assert abs(part[1][k] - whole[1][k]) <= tol * abs(whole[1][k]) + 1e-300, (chunk, k)
+
+
 def _views(net, mode):
   """{index: (offset, bytes, format)} of seedrl_debug_net_views for a (21, 64) call, and the workspace size."""
   from seed_rl_b200 import _lib

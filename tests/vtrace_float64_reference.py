@@ -190,6 +190,11 @@ def vtrace_from_importance_weights(target_action_log_probs, behaviour_action_log
 
 def compute_loss(cfg, logits, baseline, batch, entropy_cost_param, dtype):
   """loss_oracle.compute_loss_from_outputs in `dtype`: -> (total, logs {name: tensor})."""
+  return _compute_loss(cfg, logits, baseline, batch, entropy_cost_param, dtype)[:2]
+
+
+def _compute_loss(cfg, logits, baseline, batch, entropy_cost_param, dtype):
+  """compute_loss, and the stop-gradient V-trace targets: -> (total, logs, vs, pg_advantages)."""
   FT = np.float64 if dtype == torch.float64 else np.float32
   behaviour_logits = torch.as_tensor(np.asarray(batch['behaviour_logits'])).to(dtype)
   actions = torch.as_tensor(np.asarray(batch['action'])).long()
@@ -240,7 +245,65 @@ def compute_loss(cfg, logits, baseline, batch, entropy_cost_param, dtype):
       ('policy/entropy_cost', entropy_cost),
       ('policy/kl(old|new)', kl.mean()),
   ])
-  return total, logs
+  return total, logs, vs, pg_adv
+
+
+# Logged terms that are means over the T x B rows, and may be averaged over column chunks with weights Bc / B.
+_MEAN_LOGS = ('V/value function', 'losses/policy', 'losses/V', 'losses/entropy', 'losses/kl', 'losses/total',
+              'policy/entropy', 'policy/entropy_cost', 'policy/kl(old|new)')
+
+
+def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, dtype, chunk=None):
+  """loss_oracle.loss_and_grads in `dtype`, on the network outputs alone (inputs time-major with T+1 rows:
+  ll, bl [T1,B,A], lb, act, rew, done [T1,B]; ecp the entropy cost parameter as the GPU holds it).
+  Returns (total, logs {name: float}, dlogits [T1,B,A], dbaseline [T1,B], d_entropy_cost_param, vs [T,B],
+  pg_advantages [T,B]); vs and pg_advantages are stop-gradient, as in compute_loss.
+
+  `chunk` columns at a time keep the autograd graph of a large B within host memory.  Every output but the
+  loss terms is per column; the loss terms are means over all T x B rows, so a chunk of Bc columns contributes
+  its own means with weight Bc / B (and its gradients scaled by the same weight), summed in float64.  The one
+  term that is not a mean, V/L2 error = sqrt(mean (vs - V)^2), is rebuilt from the weighted mean of its square.
+  With a single chunk (the default) this is compute_loss and autograd, unchanged."""
+  ll, lb, bl = (np.asarray(x) for x in (ll, lb, bl))
+  B = ll.shape[1]
+  chunk = B if chunk is None else min(int(chunk), B)
+  dl = np.empty(ll.shape, np.float64 if dtype == torch.float64 else np.float32)
+  db = np.empty(lb.shape, dl.dtype)
+  vs = np.empty((lb.shape[0] - 1, B), dl.dtype)
+  pg = np.empty_like(vs)
+  sums = collections.OrderedDict()
+  total = dep = 0.0
+  for b0 in range(0, B, chunk):
+    cols = slice(b0, min(b0 + chunk, B))
+    w = (cols.stop - cols.start) / B
+    logits = torch.tensor(ll[:, cols], dtype=dtype, requires_grad=True)
+    baseline = torch.tensor(lb[:, cols], dtype=dtype, requires_grad=True)
+    ep = torch.tensor(float(ecp), dtype=dtype, requires_grad=True)
+    batch = dict(behaviour_logits=bl[:, cols], action=np.asarray(act)[:, cols], reward=np.asarray(rew)[:, cols],
+                 done=np.asarray(done)[:, cols])
+    t, logs, vs_c, pg_c = _compute_loss(cfg, logits, baseline, batch, ep, dtype)
+    t.backward()
+    if w == 1.0:
+      dl[:], db[:] = logits.grad.numpy(), baseline.grad.numpy()
+    else:
+      dl[:, cols], db[:, cols] = logits.grad.numpy() * w, baseline.grad.numpy() * w
+    vs[:, cols], pg[:, cols] = vs_c.numpy(), pg_c.numpy()
+    total += w * float(t.detach())
+    dep += w * (float(ep.grad) if ep.grad is not None else 0.0)
+    for k, v in logs.items():
+      v = float(v.detach())
+      if k == 'policy/max_action_abs(before_tanh)':
+        sums[k] = max(sums.get(k, 0.0), v)
+      elif k == 'V/L2 error':
+        sums[k] = sums.get(k, 0.0) + w * v * v
+      else:
+        assert k in _MEAN_LOGS, k
+        sums[k] = sums.get(k, 0.0) + w * v
+  if chunk == B:
+    sums['V/L2 error'] = float(logs['V/L2 error'].detach())
+  else:
+    sums['V/L2 error'] = float(np.sqrt(sums['V/L2 error']))
+  return total, sums, dl, db, dep, vs, pg
 
 
 # ---- the step ------------------------------------------------------------------------------------------------------
