@@ -48,11 +48,22 @@ static ConvLayer add_conv(seedrl_net* n, const std::string& prefix, int k, int c
 }
 
 // ---- workspace plan -----------------------------------------------------------
+// Where an activation x of the deep torso sits: its raw value (a conv input or residual operand) and relu(x)
+// (a conv input, and in the backward the ReLU mask x > 0).  fp32 NHWC (conv modes 0-2): one buffer, raw == relu,
+// and a conv that reads relu(x) applies the ReLU as it loads it (IN_RELU).  Plane tensors (conv mode 3,
+// conv_planes.cu): relu(x) is a plane tensor of its own, and a copy that nothing reads is not kept (kNone).
+// Gradients use the same description with their one buffer in `raw`.
+constexpr size_t kNone = ~(size_t)0;
+struct Act {
+  size_t raw, relu;
+  bool planes;
+};
+static Act f32_act(size_t off) { return Act{off, off, false}; }
+
 struct StackBufs {
-  size_t a0, p, idx, c0, o0, c1, o1;
-  // conv_mode 3 (plane tensors, conv_planes.cu): raw / ReLU'd pooled activation, ReLU'd c0 / c1,
-  // raw / ReLU'd o0, raw o1 (the last stack's o1 stays fp32 NHWC for the Dense layer)
-  size_t praw, prelu, c0r, o0raw, o0relu, c1r, o1p;
+  Act a0;                  // the stack's first conv before the max-pool: fp32 NHWC, full resolution
+  size_t idx;              // max-pool taps
+  Act p, c0, o0, c1, o1;   // pooled resolution; the last stack's o1 is fp32 NHWC for the Dense layer
 };
 
 // packed-weight slot: (hi + lo) x 9 x 32 x 32 bf16; deferred weight-gradient partials of all
@@ -66,12 +77,23 @@ struct Plan {
   size_t sh_a1, sh_a2;         // shallow conv outputs (post-relu)
   size_t sh_col0, sh_col1;     // shallow net, tensor-core modes: im2col matrices (kept for the backward)
   CorePlan core;
-  // backward scratch
-  size_t gA, gB, gC, gFull, wt, partial, wq, tcerr, gemm_ws, wq_all, partial_all;
-  size_t gP1, gP2, gP3, gFP;   // conv_mode 3: plane-tensor gradients (pooled resolution x3, full resolution)
+  // backward scratch.  gA: d loss / d (torso output) from Dense, fp32; g: the deep torso's pooled-resolution
+  // gradients (fp32: g[0] is gA); gPool: the gradient of the max-pool input of stacks 1 and 2; gFull: fp32 at
+  // full resolution (the max-pool backward of the first layer's unfused paths)
+  size_t gA, gFull, wt, partial, wq, tcerr, gemm_ws, wq_all, partial_all;
+  Act g[3], gPool;
   size_t obs4, w0pad, dw0pad;  // 3-channel frames: zero-padded frames / first-conv weights / their gradient
   size_t total;
 };
+
+// Carves one activation: an fp32 NHWC buffer, or a plane tensor for each copy that is read.
+static Act take_act(Bump& b, bool planes, size_t f32_bytes, size_t planes_bytes, bool raw, bool relu) {
+  if (!planes) return f32_act(b.take(f32_bytes));
+  Act a{kNone, kNone, true};
+  if (raw) a.raw = b.take(planes_bytes);
+  if (relu) a.relu = b.take(planes_bytes);
+  return a;
+}
 
 static Plan make_plan(const seedrl_net* n, int T1, int B) {
   Plan p;
@@ -83,26 +105,21 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
   if (n->cfg.net == SEEDRL_NET_DEEP) {
     for (size_t si = 0; si < n->stacks.size(); ++si) {
       const Stack& s = n->stacks[si];
-      StackBufs sb = StackBufs();
+      StackBufs sb;
       const size_t full = N * s.hin * s.win * s.c, pooled = N * s.hout * s.wout * s.c;
-      sb.a0 = b.take(full * 4);
+      const size_t pb = planes_bytes((int)N, s.hout, s.wout, s.c);
+      sb.a0 = f32_act(b.take(full * 4));
       sb.idx = b.take(pooled);
-      if (!planes) {
-        sb.p = b.take(pooled * 4);
-        sb.c0 = b.take(pooled * 4);
-        sb.o0 = b.take(pooled * 4);
-        sb.c1 = b.take(pooled * 4);
-        sb.o1 = b.take(pooled * 4);
-      } else {
-        const size_t pb = planes_bytes((int)N, s.hout, s.wout, s.c);
-        sb.praw = b.take(pb); sb.prelu = b.take(pb); sb.c0r = b.take(pb);
-        sb.o0raw = b.take(pb); sb.o0relu = b.take(pb); sb.c1r = b.take(pb);
-        if (si + 1 < n->stacks.size()) sb.o1p = b.take(pb); else sb.o1 = b.take(pooled * 4);
-        if (pb > pooled_planes_max) pooled_planes_max = pb;
-        if (si > 0) {
-          const size_t fb = planes_bytes((int)N, s.hin, s.win, s.c);
-          if (fb > full_planes_max) full_planes_max = fb;
-        }
+      // p and o0 are ReLU'd conv inputs and residuals, c0 and c1 only ReLU'd conv inputs, o1 the next stack's input
+      sb.p = take_act(b, planes, pooled * 4, pb, true, true);
+      sb.c0 = take_act(b, planes, pooled * 4, pb, false, true);
+      sb.o0 = take_act(b, planes, pooled * 4, pb, true, true);
+      sb.c1 = take_act(b, planes, pooled * 4, pb, false, true);
+      sb.o1 = take_act(b, planes && si + 1 < n->stacks.size(), pooled * 4, pb, true, false);
+      if (pb > pooled_planes_max) pooled_planes_max = pb;
+      if (si > 0) {
+        const size_t fb = planes_bytes((int)N, s.hin, s.win, s.c);
+        if (fb > full_planes_max) full_planes_max = fb;
       }
       p.st.push_back(sb);
       if (pooled > pooled_max) pooled_max = pooled;
@@ -130,17 +147,12 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
     p.dw0pad = b.take(9 * 4 * 16 * 4);
   }
   p.gA = b.take(pooled_max * 4);
-  p.gB = p.gC = p.gP1 = p.gP2 = p.gP3 = p.gFP = 0;
-  if (!planes) {
-    p.gB = b.take(pooled_max * 4);
-    p.gC = b.take(pooled_max * 4);
-  } else {
-    p.gP1 = b.take(pooled_planes_max);
-    p.gP2 = b.take(pooled_planes_max);
-    p.gP3 = b.take(pooled_planes_max);
-    p.gFP = b.take(full_planes_max);
-  }
+  p.g[0] = planes ? take_act(b, true, 0, pooled_planes_max, true, false) : f32_act(p.gA);
+  p.g[1] = take_act(b, planes, pooled_max * 4, pooled_planes_max, true, false);
+  p.g[2] = take_act(b, planes, pooled_max * 4, pooled_planes_max, true, false);
+  if (planes) p.gPool = take_act(b, true, 0, full_planes_max, true, false);
   p.gFull = b.take(full_max * 4);
+  if (!planes) p.gPool = f32_act(p.gFull);
   p.wt = b.take(64 * 1024 * 4);
   p.wq = b.take(2 * 64 * 1024 * 2);
   p.gemm_ws = b.take(gemm_tc_workspace_bytes());
@@ -154,13 +166,49 @@ static Plan make_plan(const seedrl_net* n, int T1, int B) {
 
 // The torso's output, the flat features Dense(256) reads (the deep net's is ReLU'd as it is read).
 static const float* flat_features(const seedrl_net* n, const Plan& pl, void* ws) {
-  return W<float>(ws, n->cfg.net == SEEDRL_NET_DEEP ? pl.st.back().o1 : pl.sh_a2);
+  return W<float>(ws, n->cfg.net == SEEDRL_NET_DEEP ? pl.st.back().o1.raw : pl.sh_a2);
+}
+
+// The deep net's first layer (stack 0's conv + max-pool on the uint8 frames) runs one of four kernel paths.
+// The forward and the backward pick theirs independently: the fused kernels' limits differ (conv_first.cu).
+enum FirstPath {
+  kFirstFused,     // conv0pool_forward / first_wgrad_pooled (plane tensors): no full-resolution tensor
+  kFirstStaged,    // 4-channel frames: wgmma conv on staged uint8 tiles + max-pool, wgmma weight gradient
+  kFirstSimt4,     // the same on the fp32 SIMT kernels
+  kFirstGeneric,   // SIMT channel-generic conv3x3_u8_* (1 to 16 channels) + max-pool
+};
+
+// test hook: 1 = conv mode 3 keeps the dense (full-resolution) first-layer paths
+static int g_first_dense = 0;
+
+// Channels of the frames the deep net's first layer reads: 3-channel frames run on their zero-padded
+// 4-channel copy (pad_first_layer); every other count (1..16) is read as it is, zero-filled in shared memory.
+static inline int first_c(const seedrl_net* n) { return n->cfg.obs_c == 3 ? 4 : n->cfg.obs_c; }
+// frames that only the channel-generic first-layer kernels take (conv modes 0 and 3)
+static inline bool generic_first(const seedrl_net* n) {
+  return n->cfg.net == SEEDRL_NET_DEEP && first_c(n) != 4;
+}
+
+// The first layer's path for a forward or a backward call of the deep net, or the refusal of frames that no
+// path of this conv mode takes.
+static int first_layer(const seedrl_net* n, bool backward, FirstPath* path) {
+  const Stack& k = n->stacks[0];
+  const bool fused = n->conv_mode == 3 && !g_first_dense &&
+                     (backward ? first_wgrad_pooled_supported(first_c(n), k.c, k.hin, k.win)
+                               : conv0pool_supported(first_c(n), k.c, k.hin, k.win));
+  if (n->conv_mode == 3 && !fused && generic_first(n))
+    return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
+                     g_first_dense || backward
+                         ? "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames"
+                         : "conv mode 3: the fused first layer takes frames up to 107 pixels wide");
+  *path = fused ? kFirstFused : generic_first(n) ? kFirstGeneric : n->conv_mode >= 1 ? kFirstStaged : kFirstSimt4;
+  return SEEDRL_OK;
 }
 
 // State of one forward or backward call, passed down the schedule: the GEMM execution, the weights
-// pre-packed for this call, the deferred weight-gradient reductions, and for 3-channel frames the
-// zero-padded first-conv weights and their gradient (pad_first_layer), which stand in for that one
-// parameter in P() / G().
+// pre-packed for this call, the deferred weight-gradient reductions, the first layer's path, and for
+// 3-channel frames the zero-padded first-conv weights and their gradient (pad_first_layer), which stand
+// in for that one parameter in P() / G().
 struct Call {
   const seedrl_net* n;
   const Plan& pl;
@@ -170,6 +218,7 @@ struct Call {
   GemmExec ex;
   PackTable packed;
   WgradBatch wb;
+  FirstPath first = kFirstSimt4;     // deep net: first_layer() of this call's direction
   int w0_index = -1;
   const float* w0_pad = nullptr;
   float* dw0_pad = nullptr;
@@ -183,6 +232,8 @@ struct Call {
   }
   const float* P(int idx) const { return idx == w0_index && w0_pad ? w0_pad : prm + n->params.offset(idx); }
   float* G(int idx) const { return idx == w0_index && dw0_pad ? dw0_pad : grd + n->params.offset(idx); }
+  template <typename T = void>
+  T* at(size_t off) const { return off == kNone ? nullptr : W<T>(ws, off); }   // a workspace buffer, or null
 };
 
 __global__ void pad_frames3_kernel(size_t npix, const uint8_t* __restrict__ src, uchar4* __restrict__ dst) {
@@ -204,19 +255,9 @@ __global__ void unpad_dw0_kernel(int cout, const float* __restrict__ dwp, float*
   dw[i] = dwp[(tap * 4 + ci) * cout + co];
 }
 
-// test hook: 1 = keep the dense (pool backward + full-resolution weight gradient) first-layer path
-static int g_first_dense = 0;
-
-// Channels of the frames the deep net's first layer reads: 3-channel frames run on their zero-padded
-// 4-channel copy (pad_first_layer); every other count (1..16) is read as it is, zero-filled in shared memory.
-static inline int first_c(const seedrl_net* n) { return n->cfg.obs_c == 3 ? 4 : n->cfg.obs_c; }
-// frames that only the channel-generic first-layer kernels take (conv modes 0 and 3)
-static inline bool generic_first(const seedrl_net* n) {
-  return n->cfg.net == SEEDRL_NET_DEEP && first_c(n) != 4;
-}
-
 // Packs the weights of every conv of the deep torso with one launch: forward forms, or the
-// flipped/transposed forms of the data-gradient convolutions (all but the first layer).
+// flipped/transposed forms of the data-gradient convolutions (all but the first layer).  The first
+// conv is packed only for the staged kernel, in that kernel's layout.
 static int pack_all_weights(Call& c, int flip) {
   const seedrl_net* n = c.n;
   c.packed.n = 0;
@@ -227,15 +268,15 @@ static int pack_all_weights(Call& c, int flip) {
     const ConvLayer* ls[5] = {&k.conv, &k.r00, &k.r01, &k.r10, &k.r11};
     for (int i = 0; i < 5; ++i) {
       const ConvLayer& l = *ls[i];
-      if (flip && s == 0 && i == 0) continue;          // no data gradient into the frames
-      if (s == 0 && i == 0 && generic_first(n)) continue;   // conv0pool packs its own [3,3,C,16] weights
+      const bool first = s == 0 && i == 0;
+      if (first && (flip || c.first != kFirstStaged)) continue;   // no data gradient into the frames
       const int cin = flip ? l.cout : l.cin, cout = flip ? l.cin : l.cout;
       if (c.packed.n >= kMaxPackJobs) return SEEDRL_OK;
       PackJob j;
       j.w = c.P(l.w);
       j.wq = base + (size_t)c.packed.n * kPackSlotBytes;
       j.ck = cin < 16 ? 16 : cin; j.cout = cout; j.cin_src = cin; j.flip = flip;
-      j.legacy = (s == 0 && i == 0) ? 1 : 0;           // the uint8 first conv runs the staged kernel
+      j.legacy = first;
       c.packed.jobs[c.packed.n++] = j;
     }
   }
@@ -254,24 +295,88 @@ static int packed_weights(const Call& c, int cin, int cout, const float* w, int 
   return SEEDRL_OK;
 }
 
-// One 3x3 'same' convolution of the schedule.  flip != 0: data-gradient (weights flipped and
-// transposed; cin/cout are those of the *gradient* convolution).  Dispatches to the wgmma
-// kernel when the net runs in tensor-core mode and the shape is supported, else fp32 SIMT.
-static int run_conv(const Call& c, int cin, int cout, int in_mode, int N, int H, int Wd, const void* in,
-                    const float* w, const float* bias, const float* mask, const float* res, float* out, int flip) {
+// ---- the operations of the stack schedule, on either storage format ----------------------------
+// One 3x3 'same' convolution of layer l: out = conv(x) + bias + res, x = relu(in) (in_mode IN_RELU) or in
+// (IN_F32), res the raw value of `res`.  flip != 0: the data gradient (weights flipped and transposed, no
+// bias), out = 0 where `mask` <= 0 (the ReLU'd copy of the forward input).  Plane tensors run convp; fp32
+// NHWC runs the wgmma kernel when the net runs in tensor-core mode and the shape is supported, else fp32
+// SIMT.  out may be fp32 NHWC in either format.
+static int run_conv(const Call& c, const ConvLayer& l, int H, int Wd, int in_mode, const Act& in, const Act* res,
+                    const Act& out, int flip = 0, const Act* mask = nullptr) {
   cudaStream_t st = c.ex.st;
+  const int N = c.pl.N, cin = flip ? l.cout : l.cin, cout = flip ? l.cin : l.cout;
+  const float* w = c.P(l.w);
+  const float* bias = flip ? nullptr : c.P(l.b);
+  const void* x = c.at(in_mode == IN_RELU ? in.relu : in.raw);
+  const float* m = mask ? c.at<float>(mask->relu) : nullptr;
+  const float* r = res ? c.at<float>(res->raw) : nullptr;
+  const void* wq;
+  if (in.planes) {
+    SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, 2, &wq));
+    PlaneConv pc;
+    pc.N = N; pc.H = H; pc.W = Wd; pc.in = x; pc.wq = wq; pc.bias = bias; pc.mask = m; pc.res = r;
+    pc.out_raw = out.planes ? c.at(out.raw) : nullptr; pc.out_relu = out.planes ? c.at(out.relu) : nullptr;
+    pc.out_nhwc = out.planes ? nullptr : c.at<float>(out.raw); pc.err = c.ex.err;
+    return convp_forward(cin, cout, pc, st);
+  }
   if (c.n->conv_mode >= 1 && conv3x3_tc_supported(cin, cout, in_mode)) {
     const int split = c.n->conv_mode >= 2;
-    const void* wq;
     SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, split, &wq));
-    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, in, wq, bias, mask, res, out, 0, c.ex.err, st);
+    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, x, wq, bias, m, r, c.at<float>(out.raw), 0,
+                              c.ex.err, st);
   }
   if (flip) {
     float* wt = W<float>(c.ws, c.pl.wt);
     SEEDRL_TRY(conv3x3_flip_weights(cout, cin, w, wt, st));   // source layout is [tap][cout][cin]
-    return conv3x3_forward(cin, cout, in_mode, N, H, Wd, in, wt, bias, mask, res, out, st);
+    w = wt;
   }
-  return conv3x3_forward(cin, cout, in_mode, N, H, Wd, in, w, bias, mask, res, out, st);
+  return conv3x3_forward(cin, cout, in_mode, N, H, Wd, x, w, bias, m, r, c.at<float>(out.raw), st);
+}
+
+// Backward of run_conv(l, in_mode, x) -> dy: the weight and bias gradient, then the data gradient
+// dx = flipped conv of dy, masked by x > 0 where the forward read relu(x), plus dres.
+static int conv_bwd(Call& c, const ConvLayer& l, int H, int Wd, int x_mode, const Act& x, const Act& dy,
+                    const Act* dres, const Act& dx) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; cudaStream_t st = c.ex.st;
+  const void* xin = c.at(x_mode == IN_RELU ? x.relu : x.raw);
+  if (x.planes) {
+    SEEDRL_TRY(wgradp(l.cin, l.cout, pl.N, H, Wd, xin, c.at(dy.raw), c.G(l.w), c.G(l.b), c.ex.err, &c.wb, st));
+  } else if (n->conv_mode >= 1 && conv3x3_wgrad_tc_supported(l.cin, l.cout, x_mode)) {
+    SEEDRL_TRY(conv3x3_wgrad_tc(l.cin, l.cout, x_mode, n->conv_mode >= 2, pl.N, H, Wd, xin, c.at<float>(dy.raw),
+                                c.G(l.w), c.G(l.b), W<float>(c.ws, pl.partial), conv3x3_wgrad_partial_bytes(),
+                                c.ex.err, &c.wb, st));
+  } else {
+    SEEDRL_TRY(conv3x3_wgrad(l.cin, l.cout, x_mode, pl.N, H, Wd, xin, c.at<float>(dy.raw), c.G(l.w), c.G(l.b),
+                             W<float>(c.ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
+  }
+  g_conv_cat = PC_CONV_DGRAD;
+  const int rc = run_conv(c, l, H, Wd, IN_F32, dy, dres, dx, 1, x_mode == IN_RELU ? &x : nullptr);
+  g_conv_cat = PC_CONV_FWD;
+  return rc;
+}
+
+// max-pool 3x3/2 'SAME' of the stack's first conv output a0 into p, recording the taps
+static int pool_forward(const Call& c, const Stack& k, const StackBufs& b) {
+  const float* a0 = c.at<float>(b.a0.raw);
+  uint8_t* idx = c.at<uint8_t>(b.idx);
+  if (b.p.planes) return poolp_forward(c.pl.N, k.hin, k.win, k.c, a0, c.at(b.p.raw), c.at(b.p.relu), idx, c.ex.st);
+  return maxpool3s2_forward(c.pl.N, k.hin, k.win, k.c, a0, c.at<float>(b.p.raw), idx, c.ex.st);
+}
+// its backward: the pooled gradient dy -> dx at full resolution
+static int pool_backward(const Call& c, const Stack& k, size_t idx, const Act& dy, const Act& dx) {
+  const uint8_t* taps = c.at<uint8_t>(idx);
+  if (dy.planes)
+    return poolp_backward(c.pl.N, k.hin, k.win, k.c, c.at(dy.raw), taps, dx.planes ? c.at(dx.raw) : nullptr,
+                          dx.planes ? nullptr : c.at<float>(dx.raw), c.ex.st);
+  return maxpool3s2_backward(c.pl.N, k.hin, k.win, k.c, c.at<float>(dy.raw), taps, c.at<float>(dx.raw), c.ex.st);
+}
+
+// d loss / d o1 of the last stack, which Dense's backward leaves in gA (fp32 NHWC), into g[0]
+static int gradient_from_dense(const Call& c) {
+  const Act& g = c.pl.g[0];
+  if (!g.planes) return SEEDRL_OK;   // g[0] is gA
+  const Stack& k = c.n->stacks.back();
+  return to_planes(c.pl.N, k.hout, k.wout, k.c, 0, W<float>(c.ws, c.pl.gA), c.at(g.raw), c.ex.st);
 }
 
 // 3-channel frames (DMLab's 72x96x3, dmlab/env.py:44-54): the first convolution's kernels are built
@@ -294,6 +399,52 @@ static int pad_first_layer(Call& c, const uint8_t** obs) {
   *obs = W<uint8_t>(c.ws, pl.obs4);
   c.w0_index = wi; c.w0_pad = W<float>(c.ws, pl.w0pad); c.dw0_pad = W<float>(c.ws, pl.dw0pad);
   return SEEDRL_OK;
+}
+
+// The first layer forward: frames -> stack 0's pooled activation p and the max-pool taps.
+static int first_forward(const Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; cudaStream_t st = c.ex.st;
+  const Stack& k = n->stacks[0];
+  const StackBufs& b = c.pl.st[0];
+  const int N = c.pl.N, split = n->conv_mode >= 2;
+  const float *w = c.P(k.conv.w), *bias = c.P(k.conv.b);
+  float* a0 = c.at<float>(b.a0.raw);
+  const void* wq;
+  if (c.first == kFirstFused)   // conv + bias + max-pool in one kernel
+    return conv0pool_forward(N, k.hin, k.win, first_c(n), obs, w, bias, c.at(b.p.raw), c.at(b.p.relu),
+                             c.at<uint8_t>(b.idx), c.ex.err, st);
+  if (c.first == kFirstStaged) {
+    SEEDRL_TRY(packed_weights(c, k.cin, k.c, w, 0, split, &wq));
+    SEEDRL_TRY(conv3x3_tc_forward(k.cin, k.c, IN_U8, split, N, k.hin, k.win, obs, wq, bias, nullptr, nullptr, a0, 0,
+                                  c.ex.err, st));
+  } else if (c.first == kFirstSimt4) {
+    SEEDRL_TRY(conv3x3_forward(k.cin, k.c, IN_U8, N, k.hin, k.win, obs, w, bias, nullptr, nullptr, a0, st));
+  } else {
+    SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, w, bias, a0, st));
+  }
+  return pool_forward(c, k, b);
+}
+
+// The first layer backward: stack 0's pooled gradient g[0] -> the first conv's weight and bias gradient (no
+// gradient flows into the frames).
+static int first_backward(Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl; cudaStream_t st = c.ex.st;
+  const Stack& k = n->stacks[0];
+  const int N = pl.N;
+  float *dw = c.G(k.conv.w), *db = c.G(k.conv.b);
+  if (c.first == kFirstFused)   // straight from the pooled gradient and the pool's taps
+    return first_wgrad_pooled(N, k.hin, k.win, first_c(n), obs, c.at(pl.g[0].raw), c.at<uint8_t>(pl.st[0].idx), dw,
+                              db, &c.wb, st);
+  SEEDRL_TRY(pool_backward(c, k, pl.st[0].idx, pl.g[0], f32_act(pl.gFull)));
+  const float* gF = W<float>(c.ws, pl.gFull);
+  float* partial = W<float>(c.ws, pl.partial);
+  const size_t pbytes = conv3x3_wgrad_partial_bytes();
+  if (c.first == kFirstStaged)
+    return conv3x3_wgrad_tc(k.cin, k.c, IN_U8, n->conv_mode >= 2, N, k.hin, k.win, obs, gF, dw, db, partial, pbytes,
+                            c.ex.err, &c.wb, st);
+  if (c.first == kFirstSimt4)
+    return conv3x3_wgrad(k.cin, k.c, IN_U8, N, k.hin, k.win, obs, gF, dw, db, partial, pbytes, st);
+  return conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, dw, db, partial, pbytes, st);
 }
 
 }  // namespace seedrl
@@ -400,97 +551,25 @@ extern "C" size_t seedrl_net_workspace_bytes(const seedrl_net* net, int T1, int 
 }
 
 // ---- forward --------------------------------------------------------------------
-static int torso_forward_deep(const Call& c, const uint8_t* obs) {
-  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
-  const int N = pl.N;
-  const void* in = obs;
-  int in_mode = IN_U8;
+// _Stack.__call__, dmlab/networks.py:46-60, for every stack: conv, max-pool 3x3/2, two residual blocks.
+static int torso_forward(const Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl;
   for (size_t s = 0; s < n->stacks.size(); ++s) {
     const Stack& k = n->stacks[s];
     const StackBufs& b = pl.st[s];
-    float* a0 = W<float>(ws, b.a0); float* p = W<float>(ws, b.p);
-    float* c0 = W<float>(ws, b.c0); float* o0 = W<float>(ws, b.o0);
-    float* c1 = W<float>(ws, b.c1); float* o1 = W<float>(ws, b.o1);
-    // _Stack.__call__, dmlab/networks.py:46-60
-    if (s == 0 && generic_first(n))
-      SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, c.P(k.conv.w), c.P(k.conv.b), a0,
-                                    st));
-    else
-      SEEDRL_TRY(run_conv(c, k.cin, k.c, in_mode, N, k.hin, k.win, in, c.P(k.conv.w),
-                          c.P(k.conv.b), nullptr, nullptr, a0, 0));
-    SEEDRL_TRY(maxpool3s2_forward(N, k.hin, k.win, k.c, a0, p, W<uint8_t>(ws, b.idx), st));
-    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, p, c.P(k.r00.w),
-                        c.P(k.r00.b), nullptr, nullptr, c0, 0));
-    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, c0, c.P(k.r01.w),
-                        c.P(k.r01.b), nullptr, p, o0, 0));
-    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, o0, c.P(k.r10.w),
-                        c.P(k.r10.b), nullptr, nullptr, c1, 0));
-    SEEDRL_TRY(run_conv(c, k.c, k.c, IN_RELU, N, k.hout, k.wout, c1, c.P(k.r11.w),
-                        c.P(k.r11.b), nullptr, o0, o1, 0));
-    in = o1;
-    in_mode = IN_F32;
-  }
-  return SEEDRL_OK;
-}
-
-// conv_mode 3: the same _Stack schedule on plane tensors (conv_planes.cu).  The first conv reads the
-// uint8 frames with the staged wgmma kernel (bf16x3) and writes fp32 NHWC for the max-pool; from
-// there on every conv input is a TMA tile of an HBM-resident operand.
-static int planes_conv(const Call& c, int cin, int cout, int N, int H, int Wd, const void* in, const float* w,
-                       int flip, const float* bias, const void* mask, const void* res, void* out_raw, void* out_relu,
-                       float* out_nhwc) {
-  const void* wq;
-  SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, 2, &wq));
-  PlaneConv pc;
-  pc.N = N; pc.H = H; pc.W = Wd; pc.in = in; pc.wq = wq; pc.bias = bias; pc.mask = mask; pc.res = res;
-  pc.out_raw = out_raw; pc.out_relu = out_relu; pc.out_nhwc = out_nhwc; pc.err = c.ex.err;
-  return convp_forward(cin, cout, pc, c.ex.st);
-}
-
-static int torso_forward_planes(const Call& c, const uint8_t* obs) {
-  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
-  const int N = pl.N;
-  const void* prev = nullptr;
-  const size_t ns = n->stacks.size();
-  for (size_t s = 0; s < ns; ++s) {
-    const Stack& k = n->stacks[s];
-    const StackBufs& b = pl.st[s];
-    float* a0 = W<float>(ws, b.a0);
-    void* praw = W<void>(ws, b.praw); void* prelu = W<void>(ws, b.prelu);
-    void* c0r = W<void>(ws, b.c0r); void* o0raw = W<void>(ws, b.o0raw);
-    void* o0relu = W<void>(ws, b.o0relu); void* c1r = W<void>(ws, b.c1r);
-    const bool last = s + 1 == ns;
-    if (s == 0 && generic_first(n) && g_first_dense)
-      return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
-                       "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
-    if (s == 0 && conv0pool_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
-      // first conv + bias + max-pool in one kernel: the full-resolution activation never reaches HBM
-      SEEDRL_TRY(conv0pool_forward(N, k.hin, k.win, first_c(n), obs, c.P(k.conv.w), c.P(k.conv.b), praw,
-                                   prelu, W<uint8_t>(ws, b.idx), W<int>(ws, pl.tcerr), st));
-    } else if (s == 0 && generic_first(n)) {
-      return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv mode 3: the fused first layer takes frames up to 107 pixels wide");
+    const int H = k.hout, Wd = k.wout;
+    if (s == 0) {
+      SEEDRL_TRY(first_forward(c, obs));
     } else {
-      if (s == 0)
-        SEEDRL_TRY(run_conv(c, k.cin, k.c, IN_U8, N, k.hin, k.win, obs, c.P(k.conv.w),
-                            c.P(k.conv.b), nullptr, nullptr, a0, 0));
-      else
-        SEEDRL_TRY(planes_conv(c, k.cin, k.c, N, k.hin, k.win, prev, c.P(k.conv.w), 0,
-                               c.P(k.conv.b), nullptr, nullptr, nullptr, nullptr, a0));
-      SEEDRL_TRY(poolp_forward(N, k.hin, k.win, k.c, a0, praw, prelu, W<uint8_t>(ws, b.idx), st));
+      SEEDRL_TRY(run_conv(c, k.conv, k.hin, k.win, IN_F32, pl.st[s - 1].o1, nullptr, b.a0));
+      SEEDRL_TRY(pool_forward(c, k, b));
     }
-    const int H = k.hout, Wd = k.wout, C = k.c;
     // res block 0: c0 = conv00(relu(p)); o0 = conv01(relu(c0)) + p        (networks.py:52-58)
-    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, prelu, c.P(k.r00.w), 0, c.P(k.r00.b), nullptr,
-                           nullptr, nullptr, c0r, nullptr));
-    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, c0r, c.P(k.r01.w), 0, c.P(k.r01.b), nullptr,
-                           praw, o0raw, o0relu, nullptr));
+    SEEDRL_TRY(run_conv(c, k.r00, H, Wd, IN_RELU, b.p, nullptr, b.c0));
+    SEEDRL_TRY(run_conv(c, k.r01, H, Wd, IN_RELU, b.c0, &b.p, b.o0));
     // res block 1: c1 = conv10(relu(o0)); o1 = conv11(relu(c1)) + o0
-    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, o0relu, c.P(k.r10.w), 0, c.P(k.r10.b), nullptr,
-                           nullptr, nullptr, c1r, nullptr));
-    SEEDRL_TRY(planes_conv(c, C, C, N, H, Wd, c1r, c.P(k.r11.w), 0, c.P(k.r11.b), nullptr,
-                           o0raw, last ? nullptr : W<void>(ws, b.o1p), nullptr,
-                           last ? W<float>(ws, b.o1) : nullptr));
-    prev = W<void>(ws, b.o1p);
+    SEEDRL_TRY(run_conv(c, k.r10, H, Wd, IN_RELU, b.o0, nullptr, b.c1));
+    SEEDRL_TRY(run_conv(c, k.r11, H, Wd, IN_RELU, b.c1, &b.o0, b.o1));
   }
   return SEEDRL_OK;
 }
@@ -531,9 +610,10 @@ extern "C" int seedrl_net_forward(const seedrl_net* n, const float* prm, int T1,
   // this forward or the matching backward, read back by seedrl_net_check_error
   SEEDRL_CUDA(cudaMemsetAsync(W<int>(ws, pl.tcerr), 0, sizeof(int), st));
   if (n->cfg.net == SEEDRL_NET_DEEP) {
+    SEEDRL_TRY(first_layer(n, false, &c.first));
     SEEDRL_TRY(pad_first_layer(c, &observation));
     SEEDRL_TRY(pack_all_weights(c, 0));
-    SEEDRL_TRY(n->conv_mode == 3 ? torso_forward_planes(c, observation) : torso_forward_deep(c, observation));
+    SEEDRL_TRY(torso_forward(c, observation));
   } else {
     SEEDRL_TRY(torso_forward_shallow(c, observation));
   }
@@ -573,143 +653,57 @@ extern "C" int seedrl_debug_net_views(const seedrl_net* n, int T1, int B, int in
   } else if (!deep) {
     const StridedConv& l = n->sh[index];
     *offset = index == 0 ? pl.sh_a1 : pl.sh_a2; *bytes = N * l.hout * l.wout * (size_t)l.cout * 4; *format = 0;
-  } else if (index == 15) {
-    const Stack& k = n->stacks.back();
-    *offset = pl.st.back().o1; *bytes = N * k.hout * k.wout * (size_t)k.c * 4; *format = 0;
   } else {
-    const Stack& k = n->stacks[index / 5];
-    const StackBufs& b = pl.st[index / 5];
-    const int j = index % 5;
+    // stack s, j = 0..3: p, c0, o0, c1, j = 4: the taps; index 15: the last stack's o1 (j = 5)
+    const size_t s = index == 15 ? n->stacks.size() - 1 : index / 5;
+    const int j = index == 15 ? 5 : index % 5;
+    const Stack& k = n->stacks[s];
+    const StackBufs& b = pl.st[s];
     const size_t pooled = N * k.hout * k.wout * (size_t)k.c;
+    const Act* acts[6] = {&b.p, &b.c0, &b.o0, &b.c1, nullptr, &b.o1};
     if (j == 4) {
       *offset = b.idx; *bytes = pooled; *format = 2;
-    } else if (n->conv_mode == 3) {
-      const size_t off[4] = {b.praw, b.c0r, b.o0relu, b.c1r};
-      *offset = off[j]; *bytes = planes_bytes(pl.N, k.hout, k.wout, k.c); *format = 1;
     } else {
-      const size_t off[4] = {b.p, b.c0, b.o0, b.c1};
-      *offset = off[j]; *bytes = pooled * 4; *format = 0;
+      // p and o1 before their ReLU; c0, o0 and c1 as the buffer the next conv reads relu(x) from
+      const Act& a = *acts[j];
+      *offset = j == 0 || j == 5 ? a.raw : a.relu;
+      *bytes = a.planes ? planes_bytes(pl.N, k.hout, k.wout, k.c) : pooled * 4;
+      *format = a.planes ? 1 : 0;
     }
   }
   return SEEDRL_OK;
 }
 
 // ---- backward -------------------------------------------------------------------
-static int conv_bwd(Call& c, const ConvLayer& l, int N, int H, int Wd, const void* x, int x_mode, const float* dy,
-                    const float* dmask, const float* dres, float* dx) {
-  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
-  // weight + bias gradient
-  if (n->conv_mode >= 1 && conv3x3_wgrad_tc_supported(l.cin, l.cout, x_mode)) {
-    SEEDRL_TRY(conv3x3_wgrad_tc(l.cin, l.cout, x_mode, n->conv_mode >= 2, N, H, Wd, x, dy,
-                                c.G(l.w), c.G(l.b), W<float>(ws, pl.partial),
-                                conv3x3_wgrad_partial_bytes(), c.ex.err, &c.wb, st));
-  } else {
-    SEEDRL_TRY(conv3x3_wgrad(l.cin, l.cout, x_mode, N, H, Wd, x, dy, c.G(l.w), c.G(l.b),
-                             W<float>(ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
-  }
-  if (dx) {  // data gradient = conv with flipped, transposed weights
-    g_conv_cat = PC_CONV_DGRAD;
-    const int rc = run_conv(c, l.cout, l.cin, IN_F32, N, H, Wd, dy, c.P(l.w), nullptr,
-                            dmask, dres, dx, 1);
-    g_conv_cat = PC_CONV_FWD;
-    SEEDRL_TRY(rc);
-  }
-  return SEEDRL_OK;
-}
-
-static int torso_backward_deep(Call& c, const uint8_t* obs) {
-  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
-  // On entry gA holds d loss / d o1 of the last stack.
-  const int N = pl.N;
-  float* gA = W<float>(ws, pl.gA); float* gB = W<float>(ws, pl.gB);
-  float* gC = W<float>(ws, pl.gC); float* gF = W<float>(ws, pl.gFull);
-  for (int s = (int)n->stacks.size() - 1; s >= 0; --s) {
-    const Stack& k = n->stacks[s];
-    const StackBufs& b = pl.st[s];
-    const float* p = W<float>(ws, b.p);  const float* c0 = W<float>(ws, b.c0);
-    const float* o0 = W<float>(ws, b.o0); const float* c1 = W<float>(ws, b.c1);
-    const int H = k.hout, Wd = k.wout;
-    // block 1: o1 = conv11(relu(c1)) + o0 ; c1 = conv10(relu(o0))
-    SEEDRL_TRY(conv_bwd(c, k.r11, N, H, Wd, c1, IN_RELU, gA, c1, nullptr, gB));
-    SEEDRL_TRY(conv_bwd(c, k.r10, N, H, Wd, o0, IN_RELU, gB, o0, gA, gC));
-    // block 0: o0 = conv01(relu(c0)) + p ; c0 = conv00(relu(p))
-    SEEDRL_TRY(conv_bwd(c, k.r01, N, H, Wd, c0, IN_RELU, gC, c0, nullptr, gB));
-    SEEDRL_TRY(conv_bwd(c, k.r00, N, H, Wd, p, IN_RELU, gB, p, gC, gA));
-    // max-pool, then the stack's first conv
-    SEEDRL_TRY(maxpool3s2_backward(N, k.hin, k.win, k.c, gA, W<uint8_t>(ws, b.idx), gF, st));
-    const void* x = s == 0 ? (const void*)obs : (const void*)W<float>(ws, pl.st[s - 1].o1);
-    if (s == 0 && generic_first(n))
-      SEEDRL_TRY(conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, c.G(k.conv.w), c.G(k.conv.b),
-                                  W<float>(ws, pl.partial), conv3x3_wgrad_partial_bytes(), st));
-    else
-      SEEDRL_TRY(conv_bwd(c, k.conv, N, k.hin, k.win, x, s == 0 ? IN_U8 : IN_F32, gF, nullptr,
-                          nullptr, s == 0 ? nullptr : gA));
-  }
-  return SEEDRL_OK;
-}
-
-// conv_mode 3 backward: every gradient between the Dense layer and the first conv is a plane tensor.
-static int planes_conv_bwd(Call& c, const ConvLayer& l, int N, int H, int Wd, const void* x, const void* dy,
-                           const void* dmask, const void* dres, void* dx) {
-  SEEDRL_TRY(wgradp(l.cin, l.cout, N, H, Wd, x, dy, c.G(l.w), c.G(l.b), c.ex.err, &c.wb, c.ex.st));
-  if (dx) {
-    g_conv_cat = PC_CONV_DGRAD;
-    const int rc = planes_conv(c, l.cout, l.cin, N, H, Wd, dy, c.P(l.w), 1, nullptr, dmask, dres,
-                               dx, nullptr, nullptr);
-    g_conv_cat = PC_CONV_FWD;
-    SEEDRL_TRY(rc);
-  }
-  return SEEDRL_OK;
-}
-
-static int torso_backward_planes(Call& c, const uint8_t* obs) {
-  const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
-  // On entry gA (fp32 NHWC) holds d loss / d o1 of the last stack.
-  const int N = pl.N;
-  void* g1 = W<void>(ws, pl.gP1); void* g2 = W<void>(ws, pl.gP2); void* g3 = W<void>(ws, pl.gP3);
-  void* gfp = W<void>(ws, pl.gFP); float* gF = W<float>(ws, pl.gFull);
-  {
-    const Stack& k = n->stacks.back();
-    SEEDRL_TRY(to_planes(N, k.hout, k.wout, k.c, 0, W<float>(ws, pl.gA), g1, st));
-  }
+// The mirror image of torso_forward.  On entry gA holds d loss / d o1 of the last stack.
+static int torso_backward(Call& c, const uint8_t* obs) {
+  const seedrl_net* n = c.n; const Plan& pl = c.pl;
+  const Act* g = pl.g;
+  SEEDRL_TRY(gradient_from_dense(c));
   for (int s = (int)n->stacks.size() - 1; s >= 0; --s) {
     const Stack& k = n->stacks[s];
     const StackBufs& b = pl.st[s];
     const int H = k.hout, Wd = k.wout;
-    const void* prelu = W<void>(ws, b.prelu); const void* c0r = W<void>(ws, b.c0r);
-    const void* o0relu = W<void>(ws, b.o0relu); const void* c1r = W<void>(ws, b.c1r);
     // block 1: o1 = conv11(relu(c1)) + o0 ; c1 = conv10(relu(o0))
-    SEEDRL_TRY(planes_conv_bwd(c, k.r11, N, H, Wd, c1r, g1, c1r, nullptr, g2));
-    SEEDRL_TRY(planes_conv_bwd(c, k.r10, N, H, Wd, o0relu, g2, o0relu, g1, g3));
+    SEEDRL_TRY(conv_bwd(c, k.r11, H, Wd, IN_RELU, b.c1, g[0], nullptr, g[1]));
+    SEEDRL_TRY(conv_bwd(c, k.r10, H, Wd, IN_RELU, b.o0, g[1], &g[0], g[2]));
     // block 0: o0 = conv01(relu(c0)) + p ; c0 = conv00(relu(p))
-    SEEDRL_TRY(planes_conv_bwd(c, k.r01, N, H, Wd, c0r, g3, c0r, nullptr, g2));
-    SEEDRL_TRY(planes_conv_bwd(c, k.r00, N, H, Wd, prelu, g2, prelu, g3, g1));
+    SEEDRL_TRY(conv_bwd(c, k.r01, H, Wd, IN_RELU, b.c0, g[2], nullptr, g[1]));
+    SEEDRL_TRY(conv_bwd(c, k.r00, H, Wd, IN_RELU, b.p, g[1], &g[2], g[0]));
     // max-pool, then the stack's first conv
-    if (s == 0 && first_wgrad_pooled_supported(first_c(n), k.c, k.hin, k.win) && !g_first_dense) {
-      // no gradient flows into the frames: the weight gradient is taken straight from the pooled
-      // gradient and the pool's arg-max taps (conv_first.cu), the full-resolution tensor never exists
-      SEEDRL_TRY(first_wgrad_pooled(N, k.hin, k.win, first_c(n), obs, g1, W<uint8_t>(ws, b.idx), c.G(k.conv.w),
-                                    c.G(k.conv.b), &c.wb, st));
-    } else if (s == 0 && generic_first(n)) {
-      return set_error(SEEDRL_ERR_INVALID_ARGUMENT,
-                       "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames");
-    } else if (s == 0) {
-      SEEDRL_TRY(poolp_backward(N, k.hin, k.win, k.c, g1, W<uint8_t>(ws, b.idx), nullptr, gF, st));
-      SEEDRL_TRY(conv_bwd(c, k.conv, N, k.hin, k.win, obs, IN_U8, gF, nullptr, nullptr, nullptr));
-    } else {
-      SEEDRL_TRY(poolp_backward(N, k.hin, k.win, k.c, g1, W<uint8_t>(ws, b.idx), gfp, nullptr, st));
-      SEEDRL_TRY(planes_conv_bwd(c, k.conv, N, k.hin, k.win, W<void>(ws, pl.st[s - 1].o1p), gfp, nullptr,
-                                 nullptr, g1));
+    if (s > 0) {
+      SEEDRL_TRY(pool_backward(c, k, b.idx, g[0], pl.gPool));
+      SEEDRL_TRY(conv_bwd(c, k.conv, k.hin, k.win, IN_F32, pl.st[s - 1].o1, pl.gPool, nullptr, g[0]));
     }
   }
-  return SEEDRL_OK;
+  return first_backward(c, obs);
 }
 
 static int torso_backward_shallow(Call& c, const uint8_t* obs) {
   const seedrl_net* n = c.n; const Plan& pl = c.pl; void* ws = c.ws; cudaStream_t st = c.ex.st;
   // On entry gA holds d loss / d a2 (already masked by a2 > 0).
   const int N = pl.N;
-  float* gA = W<float>(ws, pl.gA); float* gB = W<float>(ws, pl.gB);
+  float* gA = W<float>(ws, pl.gA); float* gB = W<float>(ws, pl.g[1].raw);
   const float* a1 = W<float>(ws, pl.sh_a1);
   if (n->conv_mode >= 1 && n->cfg.obs_c % 4 == 0) {
     const StridedConv &l0 = n->sh[0], &l1 = n->sh[1];
@@ -760,10 +754,11 @@ static int net_backward(const seedrl_net* n, const float* prm, int T1, int B, co
   SEEDRL_TRY(core_backward(n->core, n->params, pl.core, c.ex, ws, prm, grd, done, flat_features(n, pl, ws),
                            W<float>(ws, pl.gA), head_ready));
   if (n->cfg.net == SEEDRL_NET_DEEP) {
+    SEEDRL_TRY(first_layer(n, true, &c.first));
     c.wb = WgradBatch{W<float>(ws, pl.partial_all), kPartialAllBytes / sizeof(float), 0, 0, {}};
     SEEDRL_TRY(pad_first_layer(c, &observation));
     SEEDRL_TRY(pack_all_weights(c, 1));
-    SEEDRL_TRY(n->conv_mode == 3 ? torso_backward_planes(c, observation) : torso_backward_deep(c, observation));
+    SEEDRL_TRY(torso_backward(c, observation));
     SEEDRL_TRY(wgrad_reduce_batch(&c.wb, st));
     if (c.dw0_pad) {        // padded [3,3,4,16] gradient -> the [3,3,3,16] parameter slot
       unpad_dw0_kernel<<<ceil_div(9 * 3 * 16, 128), 128, 0, st>>>(16, c.dw0_pad,

@@ -2,8 +2,8 @@
 """Single-kernel timings of the plane-tensor conv path (csrc/conv_planes.cu) at the learner's
 layer shapes: python tools/planes_bench.py  [SEEDRL_PLANES_CHUNK=16|32|64|128 in the env].
 
-Every convp_kernel configuration the default ImpalaDeep step (net.cu torso_forward_planes /
-torso_backward_planes) launches is timed with its real epilogue: shape x {bias, ReLU mask,
+Every convp_kernel configuration the default ImpalaDeep step (net.cu torso_forward /
+torso_backward in conv mode tc3p) launches is timed with its real epilogue: shape x {bias, ReLU mask,
 residual, raw / ReLU'd / fp32 NHWC output, flipped weights}.  Per configuration: ms per launch
 (CUDA events over back-to-back launches after warm-up; each launch includes the debug entry
 point's small weight-packing kernel), algorithmic HBM bytes (4 B per element of every plane
@@ -129,7 +129,7 @@ def kernel_ms(fn, k=ITERS):
   return out
 
 
-# (cin, cout, H, launches per step): net.cu torso_backward_planes
+# (cin, cout, H, launches per step): net.cu torso_backward in conv mode tc3p
 WGRAD = [(16, 16, 42, 4), (16, 32, 42, 1), (32, 32, 21, 5), (32, 32, 11, 4)]
 wg = out['wgrad'] = {}
 sums = dict(wgradp=0.0, reduce=0.0, first_wgrad_pooled=0.0, MB=0.0, tma_MB=0.0)
