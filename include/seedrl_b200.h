@@ -446,12 +446,15 @@ int seedrl_r2d2_epsilon_greedy(int N, int A, const int32_t* env_ids, const float
 /* <- common/utils.py:327-352 (PrioritizedReplay.sample, priority_exp != 0): prob_i =
  *   prio_i^alpha / sum over the first `limit` slots; index_j = inverse CDF of uniforms[j] in
  *   [0,1) (the reference draws with tf.random.categorical: same distribution, different
- *   stream); weights_j = ((1/limit)/prob_{index_j})^beta / max_j.  probs_out may be NULL. */
+ *   stream); weights_j = ((1/limit)/prob_{index_j})^beta / max_j, with prob_{index_j} taken from
+ *   that item's own prio^alpha.  probs_out may be NULL.  limit > 8192 is refused. */
 int seedrl_replay_sample(int limit, const float* priorities, float priority_exp,
                          float importance_sampling_exp, int num_samples, const float* uniforms,
                          int64_t* indices, float* weights, float* probs_out, seedrl_stream_t stream);
 /* <- tf.clip_by_global_norm (agents/r2d2/learner.py:608, clip_norm = 40) over the flat gradient
- *   arena: g *= clip_norm / max(||g||_2, clip_norm); *norm_out = ||g||_2 (may be NULL). */
+ *   arena: g *= clip_norm * min(1/||g||_2, 1/clip_norm) + (||g||_2 - ||g||_2), so a non-finite
+ *   norm makes every element NaN, as in TF; *norm_out = ||g||_2 (may be NULL), 0 when n == 0
+ *   (grads may then be NULL). */
 size_t seedrl_clip_scratch_bytes(void);
 int seedrl_clip_by_global_norm(size_t n, float* grads, float clip_norm, float* norm_out,
                                void* scratch, seedrl_stream_t stream);

@@ -50,8 +50,9 @@ __global__ void r2d2_retrace_loss_kernel(const R2d2RetraceParams p) {
 }
 
 // ---------------------------------------------------------------------------------------
-// Single CTA (the replay holds ~100 unrolls): prob = prio^alpha / sum; inclusive CDF in shared
-// memory; sample j = first i with cdf[i] > u_j * total; weights = ((1/limit)/prob_i)^beta / max.
+// Single CTA (the replay holds ~100 unrolls): inclusive CDF of prio^alpha in shared memory; sample
+// j = first i with cdf[i] > u_j * total; prob_i = prio_i^alpha / total from the item's own mass
+// (for the weights and probs_out alike); weights = ((1/limit)/prob_i)^beta / max.
 constexpr int kReplayMax = 8192;
 __global__ void __launch_bounds__(1024)
 replay_sample_kernel(int limit, const float* __restrict__ priorities, float priority_exp, float is_exp,
@@ -67,11 +68,11 @@ replay_sample_kernel(int limit, const float* __restrict__ priorities, float prio
   __syncthreads();
   const float total = s_red[0];
   if (probs_out)
-    for (int i = tid; i < limit; i += blockDim.x)
-      probs_out[i] = (s_cdf[i] - (i ? s_cdf[i - 1] : 0.f)) / total;
+    for (int i = tid; i < limit; i += blockDim.x) probs_out[i] = replay_mass(i, priorities, priority_exp) / total;
   float wmax = 0.f;
   for (int j = tid; j < num_samples; j += blockDim.x)
-    wmax = fmaxf(wmax, replay_sample_thread(j, limit, s_cdf, total, is_exp, uniforms, indices, weights));
+    wmax = fmaxf(wmax, replay_sample_thread(j, limit, s_cdf, total, priorities, priority_exp, is_exp, uniforms,
+                                            indices, weights));
   // max over the CTA, then normalise
   for (int o = 16; o; o >>= 1) wmax = fmaxf(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
   __syncthreads();
@@ -83,7 +84,10 @@ replay_sample_kernel(int limit, const float* __restrict__ priorities, float prio
 }
 
 // ---------------------------------------------------------------------------------------
-// tf.clip_by_global_norm: g *= clip / max(||g||_2, clip).  Deterministic two-stage reduction.
+// tf.clip_by_global_norm: g *= clip * min(1/norm, 1/clip) + (norm - norm), norm = ||g||_2.  The
+// (norm - norm) term is TF's: an infinite or NaN norm turns every element into NaN, so a broken
+// gradient is visible instead of being zeroed (inf) or passed unclipped (NaN).  Deterministic
+// two-stage reduction.
 __global__ void sumsq_partial_kernel(size_t n, const float* __restrict__ g, float* __restrict__ partial) {
   __shared__ float red[32];
   float s = 0.f;
@@ -105,7 +109,8 @@ __global__ void clip_scale_kernel(size_t n, float* __restrict__ g, const float* 
     float t = 0.f;
     for (int k = 0; k < nparts; ++k) t += partial[k];        // fixed order
     const float norm = sqrtf(t);
-    s_scale = clip_norm / fmaxf(norm, clip_norm);
+    // fminf drops a NaN operand: the NaN of a non-finite norm comes in through (norm - norm) only
+    s_scale = clip_norm * fminf(1.f / norm, 1.f / clip_norm) + (norm - norm);
     if (norm_out && blockIdx.x == 0) *norm_out = norm;
   }
   __syncthreads();
@@ -241,11 +246,14 @@ extern "C" size_t seedrl_clip_scratch_bytes(void) { return 1024 * sizeof(float);
 
 extern "C" int seedrl_clip_by_global_norm(size_t n, float* grads, float clip_norm, float* norm_out,
                                           void* scratch, seedrl_stream_t stream) {
-  SEEDRL_CHECK_ARG(grads && scratch && clip_norm > 0.f, "bad arguments");
-  if (n == 0) return SEEDRL_OK;
+  SEEDRL_CHECK_ARG((grads || n == 0) && scratch && clip_norm > 0.f, "bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) {                                              // the norm of an empty arena is 0
+    if (norm_out) SEEDRL_CUDA(cudaMemsetAsync(norm_out, 0, sizeof(float), st));
+    return SEEDRL_OK;
+  }
   const int parts = 4 * kNumSMs;
   float* partial = reinterpret_cast<float*>(scratch);
-  cudaStream_t st = (cudaStream_t)stream;
   sumsq_partial_kernel<<<parts, 256, 0, st>>>(n, grads, partial);
   count_launch(PC_ADAM, st);
   SEEDRL_CHECK_LAUNCH();

@@ -34,19 +34,36 @@ extern "C" int emu_r2d2_loss(int T, int B, int A, const float* q_train, const fl
   return 0;
 }
 
-// replay_sample_kernel's phases in the order the kernel runs them (one CTA)
-extern "C" int emu_replay_sample(int limit, const float* priorities, float priority_exp, float is_exp,
-                                 int num_samples, const float* uniforms, int64_t* indices, float* weights,
-                                 float* probs_out) {
+// replay_sample_kernel's phases in the order the kernel runs them (one CTA); prefix_only draws with
+// the overload that takes the probability from cdf[i] - cdf[i-1] instead of the item's mass
+static void replay_sample(bool prefix_only, int limit, const float* priorities, float priority_exp, float is_exp,
+                          int num_samples, const float* uniforms, int64_t* indices, float* weights,
+                          float* probs_out) {
   float* cdf = new float[limit];
   for (int i = 0; i < limit; ++i) seedrl::replay_pow_thread(i, priorities, priority_exp, cdf);
   const float total = seedrl::replay_prefix_serial(limit, cdf);
   if (probs_out)
-    for (int i = 0; i < limit; ++i) probs_out[i] = (cdf[i] - (i ? cdf[i - 1] : 0.f)) / total;
+    for (int i = 0; i < limit; ++i) probs_out[i] = seedrl::replay_mass(i, priorities, priority_exp) / total;
   float wmax = 0.f;
   for (int j = 0; j < num_samples; ++j)
-    wmax = fmaxf(wmax, seedrl::replay_sample_thread(j, limit, cdf, total, is_exp, uniforms, indices, weights));
+    wmax = fmaxf(wmax, prefix_only
+                           ? seedrl::replay_sample_thread(j, limit, cdf, total, is_exp, uniforms, indices, weights)
+                           : seedrl::replay_sample_thread(j, limit, cdf, total, priorities, priority_exp, is_exp,
+                                                          uniforms, indices, weights));
   for (int j = 0; j < num_samples; ++j) weights[j] /= wmax;
   delete[] cdf;
+}
+
+extern "C" int emu_replay_sample(int limit, const float* priorities, float priority_exp, float is_exp,
+                                 int num_samples, const float* uniforms, int64_t* indices, float* weights,
+                                 float* probs_out) {
+  replay_sample(false, limit, priorities, priority_exp, is_exp, num_samples, uniforms, indices, weights, probs_out);
+  return 0;
+}
+
+extern "C" int emu_replay_sample_prefix_only(int limit, const float* priorities, float priority_exp, float is_exp,
+                                             int num_samples, const float* uniforms, int64_t* indices,
+                                             float* weights) {
+  replay_sample(true, limit, priorities, priority_exp, is_exp, num_samples, uniforms, indices, weights, nullptr);
   return 0;
 }

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from oracle import r2d2_oracle as R
+import test_gpu_replay_clip_float64 as RC
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -88,20 +89,58 @@ def test_loss_thread_body_vs_oracle(emu, T, B, A, n):
     np.testing.assert_allclose(scratch[b, :T], R.n_step_bellman_target(r, d, qmax, gamma, n)[:, b], rtol=2e-6, atol=1e-6)
 
 
+def _emu_replay_sample(emu, prio, limit, alpha, beta, u):
+  n = len(u)
+  idx = np.zeros(n, np.int64); w = np.zeros(n, np.float32); probs = np.zeros(limit, np.float32)
+  f = ctypes.c_float
+  assert emu.emu_replay_sample(limit, ptr(prio), f(alpha), f(beta), n, ptr(u), ptr(idx), ptr(w), ptr(probs)) == 0
+  return idx, w, probs
+
+
 def test_replay_sample_phase_bodies(emu):                       # common/utils.py:327-352
   rng = np.random.default_rng(0)
   prio = (rng.random(100) + 0.01).astype(np.float32); limit = 70
   u = rng.random(4096).astype(np.float32)
-  idx = np.zeros(4096, np.int64); w = np.zeros(4096, np.float32); probs = np.zeros(limit, np.float32)
-  f = ctypes.c_float
-  assert emu.emu_replay_sample(limit, ptr(prio), f(0.9), f(0.6), 4096, ptr(u), ptr(idx), ptr(w), ptr(probs)) == 0
+  idx, w, probs = _emu_replay_sample(emu, prio, limit, 0.9, 0.6, u)
   p = R.replay_probabilities(prio, limit, 0.9)
   np.testing.assert_allclose(probs, p, rtol=2e-5)
   assert idx.min() >= 0 and idx.max() < limit and w.max() == 1.0
-  np.testing.assert_allclose(w, R.replay_importance_weights(p, idx, 0.6), rtol=2e-4)
+  RC.check_sample(prio, limit, 0.9, 0.6, u, idx, w, probs)     # weights and probs_out vs float64
   freq = np.bincount(idx, minlength=limit) / len(idx)
   assert np.abs(freq - p).max() < 0.02                         # statistical, like tests/utils_test.py:353-365
   # the draw is the inverse CDF of the given uniforms
   cdf = np.cumsum(np.power(prio[:limit], np.float32(0.9)).astype(np.float32), dtype=np.float32)
   want = np.minimum(np.searchsorted(cdf, u * cdf[-1], side='right'), limit - 1)
   assert (idx == want).mean() > 0.999                          # (equal up to fp32 prefix rounding at bin edges)
+
+
+@pytest.mark.parametrize('kind', ['uniform', 'lognormal2', 'lognormal3', 'equal', 'spike', 'zeros'])
+@pytest.mark.parametrize('limit', [100, 1000, 8192])
+def test_replay_sample_phase_bodies_vs_float64(emu, limit, kind):
+  """The replay sampler's bodies against float64 (the checks of test_gpu_replay_clip_float64.py): the
+  weights of rare items with wide priority spreads, probs_out, and weights of exactly 1 for equal priorities."""
+  prio = RC.priorities(kind, limit)
+  u = np.concatenate([RC.PINNED, np.random.default_rng(limit).random(4093).astype(np.float32)])
+  for alpha, beta in RC.EXPONENTS:
+    idx, w, probs = _emu_replay_sample(emu, prio, limit, alpha, beta, u)
+    RC.check_sample(prio, limit, alpha, beta, u, idx, w, probs)
+  ug = RC.grid_uniforms()
+  idx, _, _ = _emu_replay_sample(emu, prio, limit, 0.9, 0.6, ug)
+  RC.check_grid(prio, limit, 0.9, idx)
+
+
+@pytest.mark.parametrize('limit,kind', [(1000, 'lognormal2'), (1000, 'lognormal3'), (8192, 'lognormal2'),
+                                        (8192, 'lognormal3')])
+def test_replay_weight_bar_rejects_the_prefix_difference(emu, limit, kind):
+  """The float64 weight bar is tight enough to see the error of p_i = (cdf[i] - cdf[i-1]) / total, the
+  probability replay_sample_kernel does not use: at wide priority spreads it exceeds the bar."""
+  prio = RC.priorities(kind, limit)
+  u = np.random.default_rng(limit).random(4096).astype(np.float32)
+  idx = np.zeros(len(u), np.int64); w = np.zeros(len(u), np.float32)
+  f = ctypes.c_float
+  assert emu.emu_replay_sample_prefix_only(limit, ptr(prio), f(0.9), f(0.6), len(u), ptr(u), ptr(idx), ptr(w)) == 0
+  with pytest.raises(AssertionError, match='weights: error'):
+    RC.check_sample(prio, limit, 0.9, 0.6, u, idx, w)
+  mass_idx, mass_w, _ = _emu_replay_sample(emu, prio, limit, 0.9, 0.6, u)
+  np.testing.assert_array_equal(mass_idx, idx)                 # the two forms draw the same items
+  RC.check_sample(prio, limit, 0.9, 0.6, u, mass_idx, mass_w)
