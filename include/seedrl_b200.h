@@ -406,6 +406,8 @@ int seedrl_r2d2_stack_frames(int T, int B, int P, int stack_size, const uint8_t*
  *   value_function_rescaling / inverse (:180-192) and n_step_bellman_target (:195-255), plus the
  *   gradient of mean_b(importance_weight_b * loss_b) (:604) w.r.t. q_train.  The greedy action
  *   of the online network is re-derived as argmax_a q_train (first maximum, like tf.argmax).
+ *   h and h^-1 are the reference's functions to float32 accuracy, evaluated in a form without the
+ *   cancellation of its formulas near 0 (seed_rl_b200/csrc/r2d2_thread.inl).
  *   loss, priorities: [B]; dq: [T,B,A]; scratch: seedrl_r2d2_loss_scratch_bytes. */
 size_t seedrl_r2d2_loss_scratch_bytes(int T, int B, int n_steps);
 int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,

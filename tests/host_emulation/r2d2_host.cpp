@@ -34,6 +34,12 @@ extern "C" int emu_r2d2_loss(int T, int B, int A, const float* q_train, const fl
   return 0;
 }
 
+// the value rescaling h (inverse = 0) or h^-1 (inverse = 1) of the loss bodies, elementwise
+extern "C" int emu_vf_rescale(int n, const float* x, float eps, int inverse, float* out) {
+  for (int i = 0; i < n; ++i) out[i] = inverse ? seedrl::vf_rescale_inv(x[i], eps) : seedrl::vf_rescale(x[i], eps);
+  return 0;
+}
+
 // replay_sample_kernel's phases in the order the kernel runs them (one CTA); prefix_only draws with
 // the overload that takes the probability from cdf[i] - cdf[i-1] instead of the item's mass
 static void replay_sample(bool prefix_only, int limit, const float* priorities, float priority_exp, float is_exp,

@@ -8,7 +8,8 @@ r2d2_oracle.stack_frames, optim_oracle.keras_adam_step), with two differences:
 
   * the network, the value rescaling h and h^-1, the n-step target, the loss, the priorities and the clip scale
     are evaluated in `dtype` (float32 or float64); tests/test_r2d2_float64_reference.py pins the float32 form to
-    the oracle;
+    the oracle.  h and h^-1 take the oracle's literal formulas in float32 and a form without cancellation in
+    float64 (see value_function_rescaling below);
   * the step is piecewise smooth, and its pieces can be chosen from outside.  Every ReLU of the gradient-carrying
     suffix unroll of the online network is evaluated as z * mask, with mask = z > 0 by default or the given
     `masks[name]` (MASKS: the three convolutions, the body Dense, the value and advantage hidden layers), and the
@@ -100,16 +101,55 @@ def _unroll(p, part, state, A, stack_size, dtype, relu):
 
 
 # ---- the post-network arithmetic of r2d2_oracle, in a given numpy dtype ------------------------------------------
-def value_function_rescaling(x, eps, F):
+# h and h^-1 in two algebraically equal forms.  The literal one is the reference's text (r2d2_oracle's): in float32
+# both of its subtractions cancel, sqrt(|x| + 1) - 1 for small |x| and, with eps = 1e-3, first sqrt(...) - 1 ~ 2e-3
+# and then inner^2 - 1, so h^-1 keeps ~11 good bits near 0.  The stable one has no subtraction of nearly equal
+# numbers; it is what seed_rl_b200/csrc/r2d2_thread.inl computes, in the same order of operations.  In float32 the
+# module's step is the oracle's, so it uses the literal form; in float64 it is the function itself, the stable form.
+def literal_value_function_rescaling(x, eps, F):
+  """h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x."""
   x = np.asarray(x, F)
   return (np.sign(x) * (np.sqrt(np.abs(x) + F(1.)) - F(1.)) + F(eps) * x).astype(F)
 
 
-def inverse_value_function_rescaling(x, eps, F):
+def literal_inverse_value_function_rescaling(x, eps, F):
+  """h^-1(x) = sign(x) (((sqrt(1 + 4 eps (|x| + 1 + eps)) - 1) / (2 eps))^2 - 1)."""
   x = np.asarray(x, F)
   e = F(eps)
   inner = (np.sqrt(F(1.) + F(4.) * e * (np.abs(x) + F(1.) + e)) - F(1.)) / (F(2.) * e)
   return (np.sign(x) * (np.square(inner) - F(1.))).astype(F)
+
+
+def stable_value_function_rescaling(x, eps, F):
+  """h(x) = sign(x) |x| / (sqrt(|x| + 1) + 1) + eps x; +-inf map to themselves."""
+  x = np.asarray(x, F)
+  a = np.abs(x)
+  with np.errstate(invalid='ignore'):
+    m = np.where(a < F(np.inf), a / (np.sqrt(a + F(1.)) + F(1.)), a).astype(F)
+  return (np.sign(x) * m + F(eps) * x).astype(F)
+
+
+def stable_inverse_value_function_rescaling(x, eps, F):
+  """h^-1(x) = sign(x) d (2 + d), d = 2 |x| / (s + 1 + 2 eps), s = sqrt(1 + 4 eps (|x| + 1 + eps)): since
+  s^2 = (1 + 2 eps)^2 + 4 eps |x|, s - 1 - 2 eps = 4 eps |x| / (s + 1 + 2 eps), so the literal inner - 1 is d and
+  inner^2 - 1 = d (2 + d).  +-inf map to themselves."""
+  x = np.asarray(x, F)
+  e = F(eps)
+  a = np.abs(x)
+  s = np.sqrt(F(1.) + F(4.) * e * (a + F(1.) + e))
+  with np.errstate(invalid='ignore', over='ignore'):
+    d = np.where(a < F(np.inf), F(2.) * a / (s + F(1.) + F(2.) * e), a).astype(F)
+    return (np.sign(x) * (d * (F(2.) + d))).astype(F)
+
+
+def value_function_rescaling(x, eps, F):
+  f = literal_value_function_rescaling if F == np.float32 else stable_value_function_rescaling
+  return f(x, eps, F)
+
+
+def inverse_value_function_rescaling(x, eps, F):
+  f = literal_inverse_value_function_rescaling if F == np.float32 else stable_inverse_value_function_rescaling
+  return f(x, eps, F)
 
 
 def n_step_bellman_target(rewards, done, q_target, gamma, n_steps, F):

@@ -1,5 +1,6 @@
 """CPU ORACLE (test infrastructure, NOT product code) of the opt-in Retrace(lambda) targets of the R2D2
-learner: the targets, h and the loss in float64.
+learner: the targets, h, h^-1 and the loss in float64 (h and h^-1 in the form without cancellation of
+tests/r2d2_float64_reference.py).
 
 Retrace (Munos et al. 2016) is not in the reference.  The target policy is greedy in the online network
 (a* = argmax_a Q_online, first maximum, as the double-DQN argmax of learner.py:298-305), so the trace is
@@ -15,14 +16,18 @@ import collections
 import numpy as np
 import torch
 
-from oracle import r2d2_learner_oracle as RL, r2d2_oracle as R
+import r2d2_float64_reference as RF
+from oracle import r2d2_learner_oracle as RL
 
 F64 = np.float64
 
 
 def value_function_rescaling(x, eps=1e-3):
-  x = np.asarray(x, F64)
-  return np.sign(x) * (np.sqrt(np.abs(x) + 1.) - 1.) + eps * x
+  return RF.value_function_rescaling(x, eps, F64)
+
+
+def inverse_value_function_rescaling(x, eps=1e-3):
+  return RF.inverse_value_function_rescaling(x, eps, F64)
 
 
 def retrace_targets(reward, done, q_star, q_act, greedy, gamma, lam):
@@ -49,11 +54,11 @@ def rescaled_targets(train_q, target_q, replay_action, reward, done, gamma, lam,
   tt, bb = np.meshgrid(np.arange(T), np.arange(B), indexing='ij')
   a_star = train_q.argmax(-1)
   a = np.clip(np.asarray(replay_action), 0, A - 1)
-  # h^-1 of the target network's values as the reference evaluates it, in fp32 (the pinned restatement):
-  # (sqrt(1 + 4 eps (|x| + 1 + eps)) - 1) / (2 eps) cancels, so its fp32 rounding is part of the definition
+  # h^-1 of the target network's values in float64: the reference's fp32 evaluation of its literal formula
+  # cancels (sqrt(...) - 1, then inner^2 - 1) and is not part of the definition
   gq = np.asarray(target_q, np.float32)
-  y = retrace_targets(reward, done, R.inverse_value_function_rescaling(gq[tt, bb, a_star], eps),
-                      R.inverse_value_function_rescaling(gq[tt, bb, a], eps), a == a_star, gamma, lam)
+  y = retrace_targets(reward, done, inverse_value_function_rescaling(gq[tt, bb, a_star], eps),
+                      inverse_value_function_rescaling(gq[tt, bb, a], eps), a == a_star, gamma, lam)
   return value_function_rescaling(y[1:], eps)
 
 

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 import torch
 
+import test_gpu_r2d2_loss_float64 as LF
 from oracle import r2d2_oracle as R
 
 pytestmark = pytest.mark.gpu
@@ -31,29 +32,25 @@ def test_stack_frames_bit_exact(T, B, H, W, S):
   assert o[0].flatten().tolist() == [3, 2, 0, 0] and o[5].flatten().tolist() == [8, 7, 0, 0]
 
 
+@pytest.mark.parametrize('q', [1.0, 1e-3])
 @pytest.mark.parametrize('T,B,A,n', [(16, 6, 18, 5), (101, 64, 18, 5), (4, 2, 3, 5), (12, 3, 4, 1)])
-def test_loss_and_priorities_vs_oracle(T, B, A, n):
+def test_loss_and_priorities_vs_float64(T, B, A, n, q):
+  """Loss, priorities and dq against the float64 loss of test_gpu_r2d2_loss_float64.py, with its bars (not against
+  oracle/r2d2_oracle.py's float32 loss, whose h^-1 cancels), at Q values of scale 1 and 1e-3; dq is the gradient
+  of mean_b(w_b loss_b): -(w_b / B) * td on the replayed action, zero elsewhere and on the last row."""
   from seed_rl_b200.agents.r2d2 import learner
   from seed_rl_b200.common import utils
   rng = np.random.default_rng(T + A)
-  tq = rng.normal(size=(T, B, A)).astype(np.float32); gq = rng.normal(size=(T, B, A)).astype(np.float32)
+  tq = (rng.normal(size=(T, B, A)) * q).astype(np.float32); gq = (rng.normal(size=(T, B, A)) * q).astype(np.float32)
   ra = rng.integers(0, A, (T, B)); r = rng.normal(size=(T, B)).astype(np.float32); d = rng.random((T, B)) < 0.1
   w = rng.random(B).astype(np.float32) + 0.1
-  loss, prio, abs_td = R.loss_and_priorities(tq, tq.argmax(-1), gq, ra, r, d, 0.997, n_steps=n)
   c = lambda a: torch.as_tensor(a).cuda()
   env = utils.EnvOutput(c(r), c(d), None, None, None)
   got_loss, got_prio, dq = learner.compute_loss_and_priorities_from_agent_outputs(
       learner.AgentOutput(None, c(tq)), learner.AgentOutput(None, c(gq)), env, learner.AgentOutput(c(ra), None),
       0.997, n_steps=n, importance_weights=c(w))
-  np.testing.assert_allclose(got_loss.cpu().numpy(), loss, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(got_prio.cpu().numpy(), prio, rtol=2e-5, atol=1e-6)
-  # gradient of mean_b(w_b loss_b): -(w_b / B) * td on the replayed action, zero elsewhere / last row
-  tt, bb = np.meshgrid(np.arange(T - 1), np.arange(B), indexing='ij')
-  target = R.value_function_rescaling(R.n_step_bellman_target(
-      r, d, R.inverse_value_function_rescaling(gq[np.arange(T)[:, None], np.arange(B)[None], tq.argmax(-1)]), 0.997, n)[1:])
-  want = np.zeros((T, B, A), np.float32)
-  want[tt, bb, ra[:-1]] = -(w[None] / B) * (target - tq[tt, bb, ra[:-1]])
-  np.testing.assert_allclose(dq.cpu().numpy(), want, rtol=2e-4, atol=1e-6)   # td ~ 0 cancels to ~1e-7 abs
+  LF.check_outputs(dict(loss=got_loss.cpu().numpy(), priorities=got_prio.cpu().numpy(), dq=dq.cpu().numpy()),
+                   (tq, gq, ra, r, d, w), 'n_step', n, 0.997, 0.9, 1e-3)
 
 
 def test_replay_sample_and_clip():
@@ -300,13 +297,13 @@ def test_r2d2_inference_host_feeds_replay_and_learner():
     lo = st.burn_in if k < 5 else 0
     assert torch.equal(u.agent_outputs.action[lo:-1], u.prev_actions[lo + 1:])  # :829-830
     assert float(u.priority) > 0
-    # initial priority (:807-821) against the numpy oracle on the suffix
+    # initial priority (:807-821) against the float64 loss on the suffix, q = target q = the behaviour q
     q = u.agent_outputs.q_values[st.burn_in:].cpu().numpy()[:, None]
-    _, prio, _ = R.loss_and_priorities(q, q.argmax(-1), q, u.agent_outputs.action[st.burn_in:].cpu().numpy()[:, None],
-                                       u.env_outputs.reward[st.burn_in:].cpu().numpy()[:, None],
-                                       u.env_outputs.done[st.burn_in:].cpu().numpy()[:, None], st.discounting,
-                                       n_steps=st.n_steps)
-    np.testing.assert_allclose(float(u.priority), float(prio[0]), rtol=1e-4, atol=1e-6)
+    suf = lambda x: x[st.burn_in:].cpu().numpy()[:, None]
+    LF.check_outputs(dict(priorities=np.array([float(u.priority)])),
+                     (q, q, suf(u.agent_outputs.action).astype(np.int64), suf(u.env_outputs.reward),
+                      suf(u.env_outputs.done), None),
+                     'n_step', st.n_steps, st.discounting, 0.9, st.value_function_rescaling_epsilon)
   for k, u in enumerate(items[:5]):
     # first unroll of environment k: zero padding, then the behaviour Q values == a training-mode
     # unroll of the real steps from the initial state (the state the environment was reset to)

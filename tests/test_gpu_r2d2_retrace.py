@@ -2,12 +2,14 @@
 float64 oracle of tests/retrace_oracle.py, which tests/test_r2d2_retrace.py pins to the reference's own
 n-step targets in their two reductions.
 
-  * the kernel at (T, B, A) = (16, 6, 18), (101, 64, 18), (4, 2, 3) for lambda in {0, 0.95, 1}, with the
-    tolerances of test_gpu_r2d2.py::test_loss_and_priorities_vs_oracle; lambda = 0 bit-equal to the n-step
-    kernel at n_steps = 1; repeat launches bit-identical; bad arguments refused with nothing launched;
+  * the kernel at (T, B, A) = (16, 6, 18), (101, 64, 18), (4, 2, 3) for lambda in {0, 0.95, 1} and Q values of
+    scale 1 and 1e-3, to rtol 2e-5 (loss, priorities) and 2e-4 (dq) and within the per-sequence float64 bars of
+    test_gpu_r2d2_loss_float64.py; lambda = 0 bit-equal to the n-step kernel at n_steps = 1; repeat launches bit-identical; bad arguments
+    refused with nothing launched;
   * one learner step with bellman_target='retrace' at the `bench.py --agent r2d2` shape against
     CpuR2D2Learner, with the tolerance rule of test_gpu_fullsize_r2d2.py;
-  * R2D2InferenceHost under 'retrace' hands the replay the initial priorities the oracle computes.
+  * R2D2InferenceHost under 'retrace' hands the replay the initial priorities the oracle computes, within the
+    float64 bar of test_gpu_r2d2_loss_float64.py.
 """
 import math
 
@@ -16,6 +18,7 @@ import pytest
 import torch
 
 import retrace_oracle as RO
+import test_gpu_r2d2_loss_float64 as LF
 from oracle import optim_oracle
 
 pytestmark = pytest.mark.gpu
@@ -23,10 +26,11 @@ pytestmark = pytest.mark.gpu
 c = lambda a: torch.as_tensor(np.asarray(a)).cuda()
 
 
-def _inputs(T, B, A, seed, p_greedy=0.7):
+def _inputs(T, B, A, seed, p_greedy=0.7, q=1.0):
+  """q: the scale of the Q values."""
   rng = np.random.default_rng(seed)
-  tq = rng.normal(size=(T, B, A)).astype(np.float32)
-  gq = (rng.normal(size=(T, B, A)) * 3).astype(np.float32)
+  tq = (rng.normal(size=(T, B, A)) * q).astype(np.float32)
+  gq = (rng.normal(size=(T, B, A)) * 3 * q).astype(np.float32)
   ra = np.where(rng.random((T, B)) < p_greedy, tq.argmax(-1), rng.integers(0, A, (T, B))).astype(np.int64)
   r = rng.normal(size=(T, B)).astype(np.float32)
   d = rng.random((T, B)) < 0.1
@@ -44,15 +48,17 @@ def _loss(tq, gq, ra, r, d, w, **kw):
   return [x.cpu().numpy() for x in out]
 
 
+@pytest.mark.parametrize('q', [1.0, 1e-3])
 @pytest.mark.parametrize('lam', [0.0, 0.95, 1.0])
 @pytest.mark.parametrize('T,B,A', [(16, 6, 18), (101, 64, 18), (4, 2, 3)])
-def test_retrace_loss_vs_oracle(T, B, A, lam):
-  tq, gq, ra, r, d, w = _inputs(T, B, A, seed=T + A)
+def test_retrace_loss_vs_float64(T, B, A, lam, q):
+  tq, gq, ra, r, d, w = _inputs(T, B, A, seed=T + A, q=q)
   loss, prio, dq = _loss(tq, gq, ra, r, d, w, bellman_target='retrace', retrace_lambda=lam)
   want_loss, want_prio, _, want_dq = RO.loss_and_priorities(tq, gq, ra, r, d, 0.997, lam, importance_weights=w)
-  np.testing.assert_allclose(loss, want_loss, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(prio, want_prio, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(dq, want_dq, rtol=2e-4, atol=1e-6)
+  np.testing.assert_allclose(loss, want_loss, rtol=2e-5, atol=1e-6 * q)
+  np.testing.assert_allclose(prio, want_prio, rtol=2e-5, atol=1e-6 * q)
+  np.testing.assert_allclose(dq, want_dq, rtol=2e-4, atol=1e-6 * q)
+  LF.check_outputs(dict(loss=loss, priorities=prio, dq=dq), (tq, gq, ra, r, d, w), 'retrace', lam, 0.997, 0.9, 1e-3)
   if lam == 0.0:
     for got, want in zip((loss, prio, dq), _loss(tq, gq, ra, r, d, w, n_steps=1)):
       np.testing.assert_array_equal(got, want)
@@ -207,10 +213,12 @@ def test_retrace_inference_host_initial_priorities():
   for _ in range(n):
     u = host.unroll_queue.dequeue()
     q = u.agent_outputs.q_values[st.burn_in:].cpu().numpy()[:, None]
-    a = u.agent_outputs.action[st.burn_in:].cpu().numpy()[:, None]
+    a = u.agent_outputs.action[st.burn_in:].cpu().numpy()[:, None].astype(np.int64)
     greedy_rows += int((a == q.argmax(-1)).sum())
-    _, prio, _, _ = RO.loss_and_priorities(q, q, a, u.env_outputs.reward[st.burn_in:].cpu().numpy()[:, None],
-                                           u.env_outputs.done[st.burn_in:].cpu().numpy()[:, None], st.discounting,
-                                           st.retrace_lambda)
+    r, d = (x[st.burn_in:].cpu().numpy()[:, None] for x in (u.env_outputs.reward, u.env_outputs.done))
+    _, prio, _, _ = RO.loss_and_priorities(q, q, a, r, d, st.discounting, st.retrace_lambda)
     np.testing.assert_allclose(float(u.priority), float(prio[0]), rtol=1e-4, atol=1e-6)
+    # and within the float64 bar of test_gpu_r2d2_loss_float64.py
+    LF.check_outputs(dict(priorities=np.array([float(u.priority)])), (q, q, a, r, d, None), 'retrace',
+                     st.retrace_lambda, st.discounting, 0.9, st.value_function_rescaling_epsilon)
   assert greedy_rows > 0

@@ -1,7 +1,8 @@
 """CPU: the per-thread bodies of the R2D2 CUDA kernels (seed_rl_b200/csrc/r2d2_thread.inl -- the
 same source text the GPU executes) compiled as host C++ and run thread by thread against
-oracle/r2d2_oracle.py.  This validates the algorithm and indexing of those kernels where no GPU is
-present (their GPU parity tests are tests/test_gpu_r2d2.py); it is a test harness, not a product path."""
+oracle/r2d2_oracle.py (frame stacking) and float64 (the loss and the replay sampler).  This
+validates the algorithm and indexing of those kernels where no GPU is present (their GPU parity
+tests are tests/test_gpu_r2d2.py); it is a test harness, not a product path."""
 import ctypes
 import os
 import subprocess
@@ -10,6 +11,7 @@ import numpy as np
 import pytest
 
 from oracle import r2d2_oracle as R
+import test_gpu_r2d2_loss_float64 as LF
 import test_gpu_replay_clip_float64 as RC
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -60,10 +62,14 @@ def test_stack_frames_thread_body_reference_sequence(emu):      # atari/networks
   assert o[0].tolist() == [3, 2, 0, 0] and o[5].tolist() == [8, 7, 0, 0]
 
 
+@pytest.mark.parametrize('q', [1.0, 1e-3])
 @pytest.mark.parametrize('T,B,A,n', [(16, 6, 18, 5), (101, 8, 18, 5), (4, 2, 3, 5), (12, 3, 4, 1), (2, 1, 2, 3)])
-def test_loss_thread_body_vs_oracle(emu, T, B, A, n):
+def test_loss_thread_body_vs_float64(emu, T, B, A, n, q):
+  """r2d2_loss_thread against the float64 loss of test_gpu_r2d2_loss_float64.py, with its bars, at Q values of
+  scale 1 and 1e-3: the raw n-step targets (the scratch array, scratch[b, :T] = targets before h), loss,
+  priorities and dq.  Not against oracle/r2d2_oracle.py's float32 loss: its h^-1 cancels, the body's does not."""
   rng = np.random.default_rng(T + A)
-  tq = rng.normal(size=(T, B, A)).astype(np.float32); gq = rng.normal(size=(T, B, A)).astype(np.float32)
+  tq = (rng.normal(size=(T, B, A)) * q).astype(np.float32); gq = (rng.normal(size=(T, B, A)) * q).astype(np.float32)
   ra = rng.integers(0, A, (T, B)).astype(np.int64); r = rng.normal(size=(T, B)).astype(np.float32)
   d = rng.random((T, B)) < 0.1
   w = (rng.random(B) + 0.1).astype(np.float32)
@@ -73,20 +79,8 @@ def test_loss_thread_body_vs_oracle(emu, T, B, A, n):
   f = ctypes.c_float
   assert emu.emu_r2d2_loss(T, B, A, ptr(tq), ptr(gq), ptr(ra), ptr(r), ptr(d.astype(np.uint8)), ptr(w), f(gamma), n,
                            f(eta), f(eps), ptr(loss), ptr(prio), ptr(dq), ptr(scratch)) == 0
-  want_loss, want_prio, _ = R.loss_and_priorities(tq, tq.argmax(-1), gq, ra, r, d, gamma, n_steps=n, eta=eta, eps=eps)
-  np.testing.assert_allclose(loss, want_loss, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(prio, want_prio, rtol=2e-5, atol=1e-6)
-  tt, bb = np.meshgrid(np.arange(T), np.arange(B), indexing='ij')
-  qmax = R.inverse_value_function_rescaling(gq[tt, bb, tq.argmax(-1)], eps)
-  target = R.value_function_rescaling(R.n_step_bellman_target(r, d, qmax, gamma, n)[1:], eps)
-  want = np.zeros((T, B, A), np.float32)
-  want[tt[:-1], bb[:-1], ra[:-1]] = -(w[None] / B) * (target - tq[tt[:-1], bb[:-1], ra[:-1]])
-  np.testing.assert_allclose(dq, want, rtol=2e-4, atol=1e-7)
-  # the reference's known-answer n-step cases through the same body (learner_test.py:142-198):
-  # with h = identity-like eps the rescaling cannot be switched off, so check the raw targets
-  # through the scratch array instead (scratch[b, 1:T] = targets[1:] before rescaling)
-  for b in range(B):
-    np.testing.assert_allclose(scratch[b, :T], R.n_step_bellman_target(r, d, qmax, gamma, n)[:, b], rtol=2e-6, atol=1e-6)
+  LF.check_outputs(dict(targets=scratch[:, :T].T, loss=loss, priorities=prio, dq=dq), (tq, gq, ra, r, d, w), 'n_step',
+                   n, gamma, eta, eps)
 
 
 def _emu_replay_sample(emu, prio, limit, alpha, beta, u):

@@ -6,7 +6,7 @@
     the sequences, T = 2 to 101.
   * A hand-computed T = 4 case in which an off-policy action cuts the trace.
   * r2d2_retrace_loss_thread (seed_rl_b200/csrc/r2d2_thread.inl, the body the GPU kernel runs) compiled
-    as host C++ against the oracle: loss, priorities, dq, with ties in the argmax.
+    as host C++ against the oracle and the float64 bars: loss, priorities, dq, with ties in the argmax.
   * Validation of the flags, the Python arguments and the C entry point (no launch is reached).
 """
 import ctypes
@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 
 import retrace_oracle as RO
+import test_gpu_r2d2_loss_float64 as LF
 from oracle import r2d2_oracle as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -95,12 +96,14 @@ def test_hand_computed_T4_trace_cut():
   np.testing.assert_array_equal(y2[:3], y[:3])
 
 
-def _inputs(T, B, A, seed, ties=False, p_greedy=0.7):
+def _inputs(T, B, A, seed, ties=False, p_greedy=0.7, q=1.0):
+  """q: the scale of the Q values."""
   rng = np.random.default_rng(seed)
-  tq = rng.normal(size=(T, B, A)).astype(np.float32)
+  tq = rng.normal(size=(T, B, A))
   if ties:                                          # few distinct values: many tied maxima
-    tq = (np.round(tq * 2) / 2).astype(np.float32)
-  gq = (rng.normal(size=(T, B, A)) * 3).astype(np.float32)
+    tq = np.round(tq * 2) / 2
+  tq = (tq * q).astype(np.float32)
+  gq = (rng.normal(size=(T, B, A)) * 3 * q).astype(np.float32)
   greedy = tq.argmax(-1)
   ra = np.where(rng.random((T, B)) < p_greedy, greedy, rng.integers(0, A, (T, B))).astype(np.int64)
   if ties:                                          # a tied maximum that is not the first one is off-policy
@@ -121,19 +124,23 @@ def _run_emu(emu, tq, gq, ra, r, d, w, gamma, lam, eta, eps):
   return loss, prio, dq
 
 
+@pytest.mark.parametrize('q', [1.0, 1e-3])
 @pytest.mark.parametrize('lam', [0.0, 0.95, 1.0])
 @pytest.mark.parametrize('T,B,A,ties', [(16, 6, 18, False), (101, 8, 18, False), (4, 2, 3, False), (2, 3, 4, False),
                                         (20, 6, 4, True)])
-def test_retrace_thread_body_vs_oracle(emu, T, B, A, ties, lam):
-  tq, gq, ra, r, d, w = _inputs(T, B, A, seed=T + A, ties=ties)
+def test_retrace_thread_body_vs_float64(emu, T, B, A, ties, lam, q):
+  """r2d2_retrace_loss_thread against the float64 oracle (the explicit sum, h and h^-1 without cancellation) and
+  within the per-sequence float64 bars of test_gpu_r2d2_loss_float64.py, at Q values of scale 1 and 1e-3."""
+  tq, gq, ra, r, d, w = _inputs(T, B, A, seed=T + A, ties=ties, q=q)
   if ties:
     assert ((tq == tq.max(-1, keepdims=True)).sum(-1) > 1).any()
   gamma, eta, eps = 0.997, 0.9, 1e-3
   loss, prio, dq = _run_emu(emu, tq, gq, ra, r, d, w, gamma, lam, eta, eps)
   want_loss, want_prio, _, want_dq = RO.loss_and_priorities(tq, gq, ra, r, d, gamma, lam, eta, eps, w)
-  np.testing.assert_allclose(loss, want_loss, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(prio, want_prio, rtol=2e-5, atol=1e-6)
-  np.testing.assert_allclose(dq, want_dq, rtol=2e-4, atol=1e-7)
+  np.testing.assert_allclose(loss, want_loss, rtol=2e-5, atol=1e-6 * q)
+  np.testing.assert_allclose(prio, want_prio, rtol=2e-5, atol=1e-6 * q)
+  np.testing.assert_allclose(dq, want_dq, rtol=2e-4, atol=1e-7 * q)
+  LF.check_outputs(dict(loss=loss, priorities=prio, dq=dq), (tq, gq, ra, r, d, w), 'retrace', lam, gamma, eta, eps)
 
 
 def test_retrace_thread_body_lambda0_is_nstep_body_n1(emu, emu_nstep):
@@ -207,9 +214,13 @@ def test_c_entry_point_refuses_bad_arguments():
   assert L.seedrl_r2d2_retrace_loss_scratch_bytes(101, 64) == 101 * 64 * 4
 
 
-def test_cpu_learner_oracle_lambda0_is_n_step_1():
-  """The oracle learner's retrace rule at lambda = 0 is its n-step rule at n_steps = 1, gradients included."""
+def test_cpu_learner_oracle_lambda0_is_n_step_1(monkeypatch):
+  """The oracle learner's retrace rule at lambda = 0 is its n-step rule at n_steps = 1, gradients included.  The
+  retrace rule takes h^-1 in float64; the n-step rule (oracle/r2d2_learner_oracle.py) takes the reference's float32
+  formula, whose cancellation alone moves these priorities by 2e-5, so here it is given the float64 h^-1 too."""
   from oracle import r2d2_learner_oracle as RL
+  monkeypatch.setattr(R, 'inverse_value_function_rescaling',
+                      lambda x, eps=1e-3: RO.inverse_value_function_rescaling(x, eps).astype(np.float32))
   A, obs, S = 4, (36, 36, 1), 4
   b = RL.synthetic_replay_batch(9, 3, A, obs, seed=2, done_p=0.2)
   got = RO.CpuR2D2Learner(A, obs, S, burn_in=3, n_steps=1, bellman_target='retrace', retrace_lambda=0.0).grads(b)
