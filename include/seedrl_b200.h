@@ -189,9 +189,10 @@ int seedrl_net_set_conv_mode(seedrl_net* net, int mode);
  * tile, 16 hidden units) and one barrier counter per batch tile (csrc/lstm_tiled.cu); 3 = the same
  * scheme with the recurrent products h[t-1] U and dZ[t+1] U^T on wgmma tensor cores with bf16x3 split
  * operands (hi*hi + lo*hi + hi*lo, fp32 accumulation: fp32-faithful to ~2^-16 relative), CTA = (64-row
- * batch tile, 16 hidden units) (csrc/lstm_tc.cu); 1 = the first persistent form, CTA = 2 hidden units
- * x all rows, one grid barrier per step (csrc/lstm_persistent.cu); 0 = a GEMM + a pointwise kernel per
- * time step.  Every mode is legal with every conv mode and uses the same workspace. */
+ * batch tile, 16 hidden units) (csrc/lstm_tc.cu).  Any other mode returns SEEDRL_ERR_INVALID_ARGUMENT.
+ * Both modes are legal with every conv mode and use the same workspace.  Largest batch B per call
+ * (forward / BPTT), larger ones return SEEDRL_ERR_INVALID_ARGUMENT: mode 2 takes 2048 / 1536 rows at
+ * H = 256 (this net) and 1024 / 1024 at H = 512 (seedrl_r2d2_net); mode 3 takes 4096 at either H. */
 int seedrl_net_set_lstm_mode(seedrl_net* net, int mode);
 /* name is written into buf (NUL-terminated); shape into dims[0..3], rank returned. */
 int seedrl_net_param_info(const seedrl_net* net, int index, char* name_buf,
@@ -375,7 +376,7 @@ int seedrl_r2d2_net_num_param_tensors(const seedrl_r2d2_net* net);      /* 18 */
 size_t seedrl_r2d2_net_num_params(const seedrl_r2d2_net* net);
 size_t seedrl_r2d2_net_arena_floats(const seedrl_r2d2_net* net);
 int seedrl_r2d2_net_set_mode(seedrl_r2d2_net* net, int mode);
-int seedrl_r2d2_net_set_lstm_mode(seedrl_r2d2_net* net, int mode);   /* as seedrl_net_set_lstm_mode: 1, 2 or 3 */
+int seedrl_r2d2_net_set_lstm_mode(seedrl_r2d2_net* net, int mode);   /* as seedrl_net_set_lstm_mode: 2 or 3 */
 int seedrl_r2d2_net_param_info(const seedrl_r2d2_net* net, int index, char* name_buf, size_t name_buf_len,
                                int64_t* dims4, int* rank, size_t* offset_floats);
 size_t seedrl_r2d2_net_workspace_bytes(const seedrl_r2d2_net* net, int T, int B);
@@ -563,19 +564,19 @@ int seedrl_debug_strided_conv(int op, int mode, int gather, int in_u8, int N, in
                               int* gathered, seedrl_stream_t stream);
 /* The LSTM recurrence alone, making exactly the calls the networks make (csrc/lstm.cu
  * lstm_recurrence_forward / _backward): Keras LSTMCell(H), H = 256 or 512, with done-resets, over T1 steps.
- * mode is the network's lstm_mode: 0 per-step GEMM + pointwise kernels, H = 256 only (gemm_mode 0: fp32 SIMT
- * GEMM, 2: bf16x3 wgmma GEMM; modes 1-3 ignore it), 1 persistent, 2 tiled, 3 tiled on wgmma bf16x3.
+ * mode is the network's lstm_mode: 2 tiled, 3 tiled on wgmma bf16x3 (batch limits as seedrl_net_set_lstm_mode).
  *   forward:  z [T1,B,4H] holds x W + b on entry and the activated gates (i,f,g,o) on exit; hs, cs, hp [T1,B,H]
  *             (hp[t] = h[t-1] with step t's resets applied); h0, c0 [B,H]; U [H,4H]; done [T1,B].
  *   backward: dz [T1,B,4H] = d loss / d(x W + b) from the forward's gates and cs and dhs = d loss / d hs.
- * ws: seedrl_debug_lstm_workspace_bytes(mode, H, T1, B) bytes.  *error_flag is set (never cleared) when a
- * bounded barrier wait expires.  An H other than 256 / 512 (256 in mode 0) or a batch the mode cannot take
- * returns SEEDRL_ERR_INVALID_ARGUMENT with nothing launched. */
+ * ws: seedrl_debug_lstm_workspace_bytes(mode, H, T1, B) bytes (the 256-byte block of barrier counters).
+ * *error_flag is set (never cleared) when a bounded barrier wait expires.  A mode other than 2 / 3, an H
+ * other than 256 / 512 or a batch the mode cannot take returns SEEDRL_ERR_INVALID_ARGUMENT with nothing
+ * launched. */
 size_t seedrl_debug_lstm_workspace_bytes(int mode, int H, int T1, int B);
-int seedrl_debug_lstm_forward(int mode, int gemm_mode, int H, int T1, int B, const float* U, const uint8_t* done,
-                              float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
-                              void* ws, size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
-int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, const float* U, const uint8_t* done,
+int seedrl_debug_lstm_forward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, float* z,
+                              const float* h0, const float* c0, float* hs, float* cs, float* hp, void* ws,
+                              size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
+int seedrl_debug_lstm_backward(int mode, int H, int T1, int B, const float* U, const uint8_t* done,
                                const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
                                void* ws, size_t ws_bytes, int* error_flag, seedrl_stream_t stream);
 /* Byte offset and size, in a seedrl_r2d2_net workspace of a (T, B) call, of the fp32 buffers the last forward

@@ -194,9 +194,9 @@ SIGNATURES = {
                  c_int, P, P, c_size_t, P, c_size_t, P, ctypes.POINTER(c_int), P]),
     'seedrl_debug_lstm_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'seedrl_debug_lstm_forward':
-        (c_int, [c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P, P]),
+        (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P, P]),
     'seedrl_debug_lstm_backward':
-        (c_int, [c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, c_size_t, P, P]),
+        (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, c_size_t, P, P]),
     'seedrl_debug_r2d2_net_views':
         (c_int, [P, c_int, c_int, c_int, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
     'seedrl_debug_net_views':

@@ -79,8 +79,7 @@ class DuelingLSTMDQNNet(CudaNet):
     """gemm_mode: 'tc3' = wgmma bf16x3 (fp32-faithful) for every contraction (convolutions as
     im2col GEMMs, Dense, LSTM projection, heads); 'simt' = fp32 CUDA cores.  lstm_mode: how the
     recurrent products of the LSTM core are computed: 'tiled' = one persistent kernel each way on
-    fp32 CUDA cores, 'tc3' = the same recurrence on wgmma with bf16x3 operands, 'persistent' = the
-    first persistent form."""
+    fp32 CUDA cores, 'tc3' = the same recurrence on wgmma with bf16x3 operands."""
     L = _lib.lib()
     self._num_actions = int(num_actions)
     self._observation_shape = tuple(int(x) for x in observation_shape)
@@ -100,9 +99,9 @@ class DuelingLSTMDQNNet(CudaNet):
       raise ValueError("gemm_mode must be 'simt' or 'tc3'")
     self.gemm_mode = gemm_mode
     _lib.check(L.seedrl_r2d2_net_set_mode(h, modes[gemm_mode]))
-    lstm_modes = {'persistent': 1, 'tiled': 2, 'tc3': 3}
+    lstm_modes = {'tiled': 2, 'tc3': 3}
     if lstm_mode not in lstm_modes:
-      raise ValueError("lstm_mode must be 'tiled', 'tc3' (the tiled recurrence on wgmma bf16x3) or 'persistent'")
+      raise ValueError("lstm_mode must be 'tiled' or 'tc3' (the tiled recurrence on wgmma bf16x3)")
     self.lstm_mode = lstm_mode
     _lib.check(L.seedrl_r2d2_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
     self._setup(seed, device)

@@ -6,7 +6,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 OUT=../libseedrl_b200.so
 ARCH=sm_90a
 BUILD=build/$ARCH            # objects of another target architecture are never linked
-SRCS="capi.cu vtrace_kernels.cu r2d2_kernels.cu optim_kernels.cu conv_kernels.cu conv_tc_kernels.cu conv_planes.cu conv_first.cu convgen_kernels.cu gemm_kernels.cu gemm_tc_kernels.cu lstm_persistent.cu lstm_tiled.cu lstm_tc.cu lstm.cu net.cu r2d2_net.cu strided_conv.cu store_kernels.cu batcher.cc"
+SRCS="capi.cu vtrace_kernels.cu r2d2_kernels.cu optim_kernels.cu conv_kernels.cu conv_tc_kernels.cu conv_planes.cu conv_first.cu convgen_kernels.cu gemm_kernels.cu gemm_tc_kernels.cu lstm_tiled.cu lstm_tc.cu lstm.cu net.cu r2d2_net.cu strided_conv.cu store_kernels.cu batcher.cc"
 mkdir -p $BUILD
 OBJS=""
 pids=""

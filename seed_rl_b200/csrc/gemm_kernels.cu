@@ -237,106 +237,6 @@ int colsum(int M, int N, const float* X, int ld, float* out, cudaStream_t st, fl
   return SEEDRL_OK;
 }
 
-// ---------------------------------------------------------------------------
-// LSTM.  Keras LSTMCell: z = x W + h U + b (gate order i,f,c,o), c' = s(f) c + s(i) tanh(g),
-// h' = s(o) tanh(c').  dmlab/networks.py:160-167: state is reset to zero where done[t]
-// BEFORE consuming step t.
-//
-// hprev_masked[b, :] = done[b] ? 0 : h_src[b, :]
-__global__ void lstm_mask_state_kernel(int B, int Hd, const uint8_t* __restrict__ done,
-                                       const float* __restrict__ h_src, float* __restrict__ h_dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * Hd) return;
-  const int b = i / Hd;
-  h_dst[i] = done[b] ? 0.f : h_src[i];
-}
-
-// Pointwise part of step t.  z [B,4H] holds x W + b + h U on entry and the ACTIVATED gates
-// (i,f,g,o) on exit (kept for backward).  c_prev_src is the unmasked previous cell state.
-// Also emits hprev_next = done_next ? 0 : h (the masked recurrent input of step t+1).
-__global__ void lstm_pointwise_fwd_kernel(int B, int Hd, float* __restrict__ z,
-                                          const float* __restrict__ c_prev_src,
-                                          const uint8_t* __restrict__ done_t,
-                                          const uint8_t* __restrict__ done_next,
-                                          float* __restrict__ c_out, float* __restrict__ h_out,
-                                          float* __restrict__ hprev_next) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * Hd) return;
-  const int b = i / Hd, u = i - b * Hd;
-  float* zb = z + (size_t)b * 4 * Hd;
-  const float gi = sigmoidf_(zb[u]);
-  const float gf = sigmoidf_(zb[Hd + u]);
-  const float gg = tanhf(zb[2 * Hd + u]);
-  const float go = sigmoidf_(zb[3 * Hd + u]);
-  const float cp = done_t[b] ? 0.f : c_prev_src[i];
-  const float c = gf * cp + gi * gg;
-  const float h = go * tanhf(c);
-  zb[u] = gi; zb[Hd + u] = gf; zb[2 * Hd + u] = gg; zb[3 * Hd + u] = go;
-  c_out[i] = c;
-  h_out[i] = h;
-  if (hprev_next) hprev_next[i] = (done_next && done_next[b]) ? 0.f : h;
-}
-
-// Backward pointwise of step t.
-//   dh = dh_out[t] + (done_next ? 0 : dh_rec)        dh_rec = dZ[t+1] U^T (may be null at t=T)
-//   dc = (done_next ? 0 : dc_next) + dh * o * (1 - tanh(c)^2)
-//   dZ[t] = (di, df, dg, do) pre-activation; dc_prev_out = dc * f (unmasked; the consumer masks)
-__global__ void lstm_pointwise_bwd_kernel(int B, int Hd, const float* __restrict__ gates,
-                                          const float* __restrict__ c_t,
-                                          const float* __restrict__ c_prev_src,
-                                          const uint8_t* __restrict__ done_t,
-                                          const uint8_t* __restrict__ done_next,
-                                          const float* __restrict__ dh_out,
-                                          const float* __restrict__ dh_rec,
-                                          const float* __restrict__ dc_next,
-                                          float* __restrict__ dz, float* __restrict__ dc_prev_out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * Hd) return;
-  const int b = i / Hd, u = i - b * Hd;
-  const float* gb = gates + (size_t)b * 4 * Hd;
-  const float gi = gb[u], gf = gb[Hd + u], gg = gb[2 * Hd + u], go = gb[3 * Hd + u];
-  const bool cut = done_next && done_next[b];
-  float dh = dh_out[i];
-  if (dh_rec && !cut) dh += dh_rec[i];
-  const float tc = tanhf(c_t[i]);
-  float dc = dh * go * (1.f - tc * tc);
-  if (dc_next && !cut) dc += dc_next[i];
-  const float cp = done_t[b] ? 0.f : c_prev_src[i];
-  float* dzb = dz + (size_t)b * 4 * Hd;
-  dzb[u] = dc * gg * gi * (1.f - gi);
-  dzb[Hd + u] = dc * cp * gf * (1.f - gf);
-  dzb[2 * Hd + u] = dc * gi * (1.f - gg * gg);
-  dzb[3 * Hd + u] = dh * tc * go * (1.f - go);
-  dc_prev_out[i] = dc * gf;
-}
-
-int lstm_mask_state(int B, int Hd, const uint8_t* done, const float* h_src, float* h_dst,
-                    cudaStream_t st) {
-  lstm_mask_state_kernel<<<ceil_div(B * Hd, 256), 256, 0, st>>>(B, Hd, done, h_src, h_dst);
-  count_launch(PC_LSTM_PW, st);
-  SEEDRL_CHECK_LAUNCH();
-  return SEEDRL_OK;
-}
-int lstm_pointwise_fwd(int B, int Hd, float* z, const float* c_prev_src, const uint8_t* done_t,
-                       const uint8_t* done_next, float* c_out, float* h_out, float* hprev_next,
-                       cudaStream_t st) {
-  lstm_pointwise_fwd_kernel<<<ceil_div(B * Hd, 256), 256, 0, st>>>(B, Hd, z, c_prev_src, done_t,
-                                                                   done_next, c_out, h_out, hprev_next);
-  count_launch(PC_LSTM_PW, st);
-  SEEDRL_CHECK_LAUNCH();
-  return SEEDRL_OK;
-}
-int lstm_pointwise_bwd(int B, int Hd, const float* gates, const float* c_t, const float* c_prev_src,
-                       const uint8_t* done_t, const uint8_t* done_next, const float* dh_out,
-                       const float* dh_rec, const float* dc_next, float* dz, float* dc_prev_out,
-                       cudaStream_t st) {
-  lstm_pointwise_bwd_kernel<<<ceil_div(B * Hd, 256), 256, 0, st>>>(
-      B, Hd, gates, c_t, c_prev_src, done_t, done_next, dh_out, dh_rec, dc_next, dz, dc_prev_out);
-  count_launch(PC_LSTM_PW, st);
-  SEEDRL_CHECK_LAUNCH();
-  return SEEDRL_OK;
-}
-
 // generic helpers ------------------------------------------------------------
 __global__ void fill_kernel(size_t n, float* p, float v) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -199,24 +199,7 @@ bool gemm_tc_gather_enabled();
 int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, int lda, const float* B,
             int ldb, float* C, int ldc, const GemmEpi& e, float* ws, size_t ws_bytes, int* err,
             cudaStream_t st, const ConvGather* cg = nullptr);
-int lstm_mask_state(int B, int Hd, const uint8_t* done, const float* h_src, float* h_dst,
-                    cudaStream_t st);
-int lstm_pointwise_fwd(int B, int Hd, float* z, const float* c_prev_src, const uint8_t* done_t,
-                       const uint8_t* done_next, float* c_out, float* h_out, float* hprev_next,
-                       cudaStream_t st);
-int lstm_pointwise_bwd(int B, int Hd, const float* gates, const float* c_t, const float* c_prev_src,
-                       const uint8_t* done_t, const uint8_t* done_next, const float* dh_out,
-                       const float* dh_rec, const float* dc_next, float* dz, float* dc_prev_out,
-                       cudaStream_t st);
 int fill(size_t n, float* p, float v, cudaStream_t st);
-
-// lstm_persistent.cu (H = 256: ImpalaDeep core; H = 512: DuelingLSTMDQNNet core)
-int lstm_forward_persistent(int H, int T1, int B, const float* U, const uint8_t* done, float* z,
-                            const float* h0, const float* c0, float* hs, float* cs, float* hp,
-                            unsigned int* counter, int* err, cudaStream_t st);
-int lstm_backward_persistent(int H, int T1, int B, const float* U, const uint8_t* done, const float* gates,
-                             const float* cs, const float* c0, const float* dhs, float* dz,
-                             unsigned int* counter, int* err, cudaStream_t st);
 
 // lstm_tiled.cu: CTA = (batch tile, 16 hidden units), one barrier counter per batch tile
 int lstm_forward_tiled(int H, int T1, int B, const float* U, const uint8_t* done, float* z, const float* h0,

@@ -4,59 +4,29 @@
 
 namespace seedrl {
 
-int lstm_recurrence_forward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
-                            float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
-                            unsigned int* counter) {
-  cudaStream_t st = ex.st;
+int lstm_recurrence_forward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, float* z,
+                            const float* h0, const float* c0, float* hs, float* cs, float* hp, unsigned int* counter,
+                            int* err, cudaStream_t st) {
   // one kernel for the whole recurrence, CTA = (batch tile, 16 units) (lstm_tiled.cu)
-  if (mode == 2) return lstm_forward_tiled(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
+  if (mode == 2) return lstm_forward_tiled(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, err, st);
   // the same recurrence with the recurrent products on the tensor cores (lstm_tc.cu)
-  if (mode == 3) return lstm_forward_tc(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
-  // one cooperative kernel for the whole recurrence (lstm_persistent.cu)
-  if (mode == 1) return lstm_forward_persistent(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, ex.err, st);
-  // mode 0: per step, z[t] += hp[t] U on the caller's GEMM, then the pointwise cell update
-  SEEDRL_TRY(lstm_mask_state(B, H, done, h0, hp, st));
-  GemmEpi eacc = epi_none();
-  eacc.accumulate = 1;
-  for (int t = 0; t < T1; ++t) {
-    float* zt = z + (size_t)t * B * 4 * H;
-    SEEDRL_TRY(ex.gemm(false, false, B, 4 * H, H, hp + (size_t)t * B * H, H, U, 4 * H, zt, 4 * H, eacc));
-    const bool last = (t + 1 == T1);
-    SEEDRL_TRY(lstm_pointwise_fwd(B, H, zt, t == 0 ? c0 : cs + (size_t)(t - 1) * B * H, done + (size_t)t * B,
-                                  last ? nullptr : done + (size_t)(t + 1) * B, cs + (size_t)t * B * H,
-                                  hs + (size_t)t * B * H, last ? nullptr : hp + (size_t)(t + 1) * B * H, st));
-  }
-  return SEEDRL_OK;
+  if (mode == 3) return lstm_forward_tc(H, T1, B, U, done, z, h0, c0, hs, cs, hp, counter, err, st);
+  return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "lstm mode must be 2 (tiled) or 3 (tc3)");
 }
 
-int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
-                             const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
-                             float* dhrec, float* const dc[2], unsigned int* counter) {
-  cudaStream_t st = ex.st;
-  if (mode == 2) return lstm_backward_tiled(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
-  if (mode == 3) return lstm_backward_tc(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
-  if (mode == 1) return lstm_backward_persistent(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, ex.err, st);
-  SEEDRL_CHECK_ARG(dhrec && dc && dc[0] && dc[1], "lstm mode 0: the BPTT needs dh_rec and two dc buffers");
-  for (int t = T1 - 1; t >= 0; --t) {
-    const bool last = (t + 1 == T1);
-    const size_t o = (size_t)t * B * H;
-    SEEDRL_TRY(lstm_pointwise_bwd(B, H, gates + (size_t)t * B * 4 * H, cs + o, t == 0 ? c0 : cs + o - (size_t)B * H,
-                                  done + (size_t)t * B, last ? nullptr : done + (size_t)(t + 1) * B, dhs + o,
-                                  last ? nullptr : dhrec, last ? nullptr : dc[(t + 1) & 1],
-                                  dz + (size_t)t * B * 4 * H, dc[t & 1], st));
-    if (t > 0)
-      SEEDRL_TRY(ex.gemm(false, true, B, H, 4 * H, dz + (size_t)t * B * 4 * H, 4 * H, U, 4 * H, dhrec, H,
-                         epi_none()));
-  }
-  return SEEDRL_OK;
+int lstm_recurrence_backward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, const float* gates,
+                             const float* cs, const float* c0, const float* dhs, float* dz, unsigned int* counter,
+                             int* err, cudaStream_t st) {
+  if (mode == 2) return lstm_backward_tiled(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, err, st);
+  if (mode == 3) return lstm_backward_tc(H, T1, B, U, done, gates, cs, c0, dhs, dz, counter, err, st);
+  return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "lstm mode must be 2 (tiled) or 3 (tc3)");
 }
 
 // ---- the recurrent core of both nets ---------------------------------------------------------
-Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu,
-                 bool stepwise) {
+Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu) {
   Core k;
   k.H = H; k.flat = flat; k.A = A; k.core_in = H + 1 + A;
-  k.clip_reward = clip_reward; k.flat_relu = flat_relu; k.stepwise = stepwise;
+  k.clip_reward = clip_reward; k.flat_relu = flat_relu;
   k.dense_w = t.add(dense + "/kernel", {flat, H});
   k.dense_b = t.add(dense + "/bias", {H});
   k.w = t.add("core/kernel", {k.core_in, 4 * H});
@@ -68,21 +38,15 @@ Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A
 CorePlan core_plan(const Core& k, Bump& b, int T1, int B) {
   CorePlan p;
   p.T1 = T1; p.B = B; p.N = T1 * B;
-  const size_t N = (size_t)p.N, H = (size_t)k.H, BH = (size_t)B * H * 4;
+  const size_t N = (size_t)p.N, H = (size_t)k.H;
   p.xc = b.take(N * k.core_in * 4);
   p.z = b.take(N * 4 * H * 4);
   p.hp = b.take(N * H * 4);
   p.cs = b.take(N * H * 4);
   p.hs = b.take(N * H * 4);
-  p.c0buf = b.take(BH);
+  p.c0buf = b.take((size_t)B * H * 4);
   p.dhs = b.take(N * H * 4);
   p.dz = b.take(N * 4 * H * 4);
-  p.dhrec = p.dc[0] = p.dc[1] = 0;
-  if (k.stepwise) {
-    p.dhrec = b.take(BH);
-    p.dc[0] = b.take(BH);
-    p.dc[1] = b.take(BH);
-  }
   p.dd = b.take(N * H * 4);
   p.counter = b.take(256);
   return p;
@@ -123,9 +87,9 @@ int core_forward(const Core& k, const ParamTable& t, const CorePlan& p, const Ge
   e.bias = prm + t.offset(k.b);
   SEEDRL_TRY(ex.gemm(false, false, N, 4 * H, CI, xc, CI, prm + t.offset(k.w), 4 * H, z, 4 * H, e));
   SEEDRL_CUDA(cudaMemcpyAsync(c0buf, c0, (size_t)p.B * H * 4, cudaMemcpyDeviceToDevice, st));
-  return lstm_recurrence_forward(k.lstm_mode, ex, H, p.T1, p.B, prm + t.offset(k.u), done, z, h0, c0buf,
+  return lstm_recurrence_forward(k.lstm_mode, H, p.T1, p.B, prm + t.offset(k.u), done, z, h0, c0buf,
                                  W<float>(ws, p.hs), W<float>(ws, p.cs), W<float>(ws, p.hp),
-                                 W<unsigned int>(ws, p.counter));
+                                 W<unsigned int>(ws, p.counter), ex.err, st);
 }
 
 int core_final_state(const Core& k, const CorePlan& p, cudaStream_t st, void* ws, float* h_out, float* c_out) {
@@ -144,13 +108,11 @@ int core_backward(const Core& k, const ParamTable& t, const CorePlan& p, const G
   const float* xc = W<float>(ws, p.xc);
   float* dz = W<float>(ws, p.dz);
   float* dd = W<float>(ws, p.dd);
-  float* const dc[2] = {W<float>(ws, p.dc[0]), W<float>(ws, p.dc[1])};
   const GemmEpi e = epi_none();
-  // BPTT (mode 0 needs the stepwise scratch; a net without it gets an error, not a crash)
-  SEEDRL_TRY(lstm_recurrence_backward(k.lstm_mode, ex, H, p.T1, p.B, prm + t.offset(k.u), done, W<float>(ws, p.z),
+  // BPTT
+  SEEDRL_TRY(lstm_recurrence_backward(k.lstm_mode, H, p.T1, p.B, prm + t.offset(k.u), done, W<float>(ws, p.z),
                                       W<float>(ws, p.cs), W<float>(ws, p.c0buf), W<float>(ws, p.dhs), dz,
-                                      k.stepwise ? W<float>(ws, p.dhrec) : nullptr, k.stepwise ? dc : nullptr,
-                                      W<unsigned int>(ws, p.counter)));
+                                      W<unsigned int>(ws, p.counter), ex.err, ex.st));
   SEEDRL_TRY(ex.gemm(true, false, H, 4 * H, N, W<float>(ws, p.hp), H, dz, 4 * H, grd + t.offset(k.u), 4 * H, e));
   SEEDRL_TRY(ex.gemm(true, false, CI, 4 * H, N, xc, CI, dz, 4 * H, grd + t.offset(k.w), 4 * H, e));
   SEEDRL_TRY(ex.colsum(N, 4 * H, dz, 4 * H, grd + t.offset(k.b)));
@@ -168,68 +130,40 @@ int core_backward(const Core& k, const ParamTable& t, const CorePlan& p, const G
   return ex.gemm(false, true, N, k.flat, H, dd, H, prm + t.offset(k.dense_w), H, dflat, k.flat, em);
 }
 
-// Workspace of the test hook: the barrier counters, then (mode 0) dh_rec, the two dc buffers and the
-// GEMM's split-K partials.
-struct DebugLstmPlan {
-  size_t counter, dhrec, dc[2], gemm_ws, total;
-};
-static DebugLstmPlan debug_lstm_plan(int mode, int H, int B) {
-  DebugLstmPlan p;
-  Bump b;
-  p.counter = b.take(256);
-  p.dhrec = p.dc[0] = p.dc[1] = p.gemm_ws = 0;
-  if (mode == 0) {
-    p.dhrec = b.take((size_t)B * H * 4);
-    p.dc[0] = b.take((size_t)B * H * 4);
-    p.dc[1] = b.take((size_t)B * H * 4);
-    p.gemm_ws = b.take(gemm_tc_workspace_bytes());
-  }
-  p.total = b.off;
-  return p;
-}
-
 }  // namespace seedrl
 
 using namespace seedrl;
 
+// The test hook's workspace: the 64 barrier counters.
 extern "C" size_t seedrl_debug_lstm_workspace_bytes(int mode, int H, int T1, int B) {
-  if (mode < 0 || mode > 3 || H < 1 || T1 < 1 || B < 1) return 0;
-  return debug_lstm_plan(mode, H, B).total;
+  if (mode < 2 || mode > 3 || H < 1 || T1 < 1 || B < 1) return 0;
+  return 256;
 }
 
 // A batch a mode cannot take is refused by its launcher, before anything is launched.
-static int debug_lstm_check(int mode, int gemm_mode, int H, int T1, int B, size_t ws_bytes) {
-  SEEDRL_CHECK_ARG(mode >= 0 && mode <= 3, "lstm mode must be 0..3");
-  SEEDRL_CHECK_ARG(gemm_mode == 0 || gemm_mode == 2, "gemm_mode must be 0 (fp32 SIMT) or 2 (wgmma bf16x3)");
+static int debug_lstm_check(int mode, int H, int T1, int B, size_t ws_bytes) {
+  SEEDRL_CHECK_ARG(mode == 2 || mode == 3, "lstm mode must be 2 (tiled) or 3 (tc3)");
   SEEDRL_CHECK_ARG(H == 256 || H == 512, "lstm: hidden size must be 256 or 512");
-  SEEDRL_CHECK_ARG(mode != 0 || H == 256, "lstm mode 0 runs at H = 256 only (the IMPALA core)");
   SEEDRL_CHECK_ARG(T1 >= 1 && B >= 1 && (size_t)T1 * B * 4 * H < ((size_t)1 << 31), "bad T1 / B");
-  SEEDRL_CHECK_ARG(ws_bytes >= debug_lstm_plan(mode, H, B).total, "workspace too small");
+  SEEDRL_CHECK_ARG(ws_bytes >= 256, "workspace too small");
   return SEEDRL_OK;
 }
 
-extern "C" int seedrl_debug_lstm_forward(int mode, int gemm_mode, int H, int T1, int B, const float* U,
-                                         const uint8_t* done, float* z, const float* h0, const float* c0, float* hs,
-                                         float* cs, float* hp, void* ws, size_t ws_bytes, int* error_flag,
-                                         seedrl_stream_t stream) {
+extern "C" int seedrl_debug_lstm_forward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, float* z,
+                                         const float* h0, const float* c0, float* hs, float* cs, float* hp, void* ws,
+                                         size_t ws_bytes, int* error_flag, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(U && done && z && h0 && c0 && hs && cs && hp && ws && error_flag, "null pointer");
-  SEEDRL_TRY(debug_lstm_check(mode, gemm_mode, H, T1, B, ws_bytes));
-  const DebugLstmPlan pl = debug_lstm_plan(mode, H, B);
-  const GemmExec ex{gemm_mode, false, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes(), error_flag,
-                    (cudaStream_t)stream};
-  return lstm_recurrence_forward(mode, ex, H, T1, B, U, done, z, h0, c0, hs, cs, hp, W<unsigned int>(ws, pl.counter));
+  SEEDRL_TRY(debug_lstm_check(mode, H, T1, B, ws_bytes));
+  return lstm_recurrence_forward(mode, H, T1, B, U, done, z, h0, c0, hs, cs, hp, (unsigned int*)ws, error_flag,
+                                 (cudaStream_t)stream);
 }
 
-extern "C" int seedrl_debug_lstm_backward(int mode, int gemm_mode, int H, int T1, int B, const float* U,
-                                          const uint8_t* done, const float* gates, const float* cs, const float* c0,
-                                          const float* dhs, float* dz, void* ws, size_t ws_bytes, int* error_flag,
+extern "C" int seedrl_debug_lstm_backward(int mode, int H, int T1, int B, const float* U, const uint8_t* done,
+                                          const float* gates, const float* cs, const float* c0, const float* dhs,
+                                          float* dz, void* ws, size_t ws_bytes, int* error_flag,
                                           seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(U && done && gates && cs && c0 && dhs && dz && ws && error_flag, "null pointer");
-  SEEDRL_TRY(debug_lstm_check(mode, gemm_mode, H, T1, B, ws_bytes));
-  const DebugLstmPlan pl = debug_lstm_plan(mode, H, B);
-  const GemmExec ex{gemm_mode, false, W<float>(ws, pl.gemm_ws), gemm_tc_workspace_bytes(), error_flag,
-                    (cudaStream_t)stream};
-  float* const dc[2] = {W<float>(ws, pl.dc[0]), W<float>(ws, pl.dc[1])};
-  return lstm_recurrence_backward(mode, ex, H, T1, B, U, done, gates, cs, c0, dhs, dz, W<float>(ws, pl.dhrec), dc,
-                                  W<unsigned int>(ws, pl.counter));
+  SEEDRL_TRY(debug_lstm_check(mode, H, T1, B, ws_bytes));
+  return lstm_recurrence_backward(mode, H, T1, B, U, done, gates, cs, c0, dhs, dz, (unsigned int*)ws, error_flag,
+                                  (cudaStream_t)stream);
 }

@@ -2,8 +2,8 @@
 // done-resets (dmlab/networks.py:157-169, atari/networks.py:176-218) -- forward and BPTT -- as ONE
 // launch each, CTA = (batch tile, unit group).
 //
-// The first form (lstm_persistent.cu: CTA = 2..4 hidden units, ALL batch rows) makes every one of its
-// 128 CTAs re-read the whole h[t] (64 KB) / dZ[t+1] (256 KB) through L2 each step and synchronises
+// A CTA of 2..4 hidden units x ALL batch rows would make every one of its 128 CTAs re-read the
+// whole h[t] (64 KB) / dZ[t+1] (256 KB) through L2 each step and synchronise
 // all 128 CTAs with one grid barrier per step.  Here a CTA owns NU = 16 hidden units x RB batch rows:
 //   * it needs only ITS batch rows of h[t] / dZ[t+1] (8x less L2 traffic at B = 64),
 //   * it depends only on the CTAs of the SAME batch tile, so the per-step barrier is one counter per

@@ -30,7 +30,7 @@ struct seedrl_net {
   seedrl::ParamTable params;               // network tensors, then entropy_cost_param
   size_t logical_params;
   int p_base_w, p_base_b, p_pol_w, p_pol_b;
-  seedrl::Core core;                       // Dense(256) + LSTM(256); lstm_mode 0..3 (schedule.h)
+  seedrl::Core core;                       // Dense(256) + LSTM(256); lstm_mode 2 or 3 (schedule.h)
   std::vector<seedrl::Stack> stacks;       // deep
   seedrl::StridedConv sh[2];               // shallow: conv 8x8/4 -> 16, conv 4x4/2 -> 32
   int sh_w[2], sh_b[2];                    // their param indices
@@ -479,7 +479,7 @@ extern "C" int seedrl_net_create(const seedrl_net_config* cfg, seedrl_net** out)
   }
   // the reward is clipped (networks.py:111); the deep torso's output is ReLU'd as Dense reads it (:105), the
   // shallow one's already is
-  n->core = core_create(n->params, "conv_to_linear", kHidden, flat, A, true, cfg->net == SEEDRL_NET_DEEP, true);
+  n->core = core_create(n->params, "conv_to_linear", kHidden, flat, A, true, cfg->net == SEEDRL_NET_DEEP);
   n->p_pol_w = n->params.add("policy_logits/kernel", {kHidden, A});
   n->p_pol_b = n->params.add("policy_logits/bias", {A});
   if (cfg->net == SEEDRL_NET_DEEP) {
@@ -522,7 +522,7 @@ extern "C" int seedrl_net_num_param_tensors(const seedrl_net* net) {
 extern "C" size_t seedrl_net_num_params(const seedrl_net* net) { return net ? net->logical_params : 0; }
 extern "C" size_t seedrl_net_arena_floats(const seedrl_net* net) { return net ? net->params.arena_floats : 0; }
 extern "C" int seedrl_net_set_lstm_mode(seedrl_net* net, int mode) {
-  SEEDRL_CHECK_ARG(net && mode >= 0 && mode <= 3, "mode must be 0 (per-step launches), 1 (persistent, CTA = 2 units), 2 (persistent, CTA = batch tile x 16 units) or 3 (as 2 on wgmma bf16x3)");
+  SEEDRL_CHECK_ARG(net && (mode == 2 || mode == 3), "mode must be 2 (tiled) or 3 (tc3: tiled on wgmma bf16x3)");
   net->core.lstm_mode = mode;
   return SEEDRL_OK;
 }

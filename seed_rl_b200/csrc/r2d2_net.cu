@@ -26,7 +26,7 @@ struct seedrl_r2d2_net {
   size_t logical_params;
   seedrl::StridedConv conv[3];
   int conv_w[3], conv_b[3];               // param indices
-  seedrl::Core core;                      // Dense(512) + LSTM(512); lstm_mode 1..3 (schedule.h)
+  seedrl::Core core;                      // Dense(512) + LSTM(512); lstm_mode 2 or 3 (schedule.h)
   int p_ah_w, p_ah_b, p_a_w, p_vh_w, p_vh_b, p_v_w, p_v_b;
 };
 
@@ -138,7 +138,7 @@ extern "C" int seedrl_r2d2_net_create(int num_actions, int obs_h, int obs_w, int
     n->conv_b[i] = t.add(pre + "/bias", {k.cout});
   }
   // _torso tail (networks.py:262-273): the reward is NOT clipped, unlike ImpalaDeep
-  n->core = core_create(t, "body/dense", kRH, h * w * c, num_actions, false, false, false);
+  n->core = core_create(t, "body/dense", kRH, h * w * c, num_actions, false, false);
   n->p_vh_w = t.add("value/hidden/kernel", {kRH, 512});
   n->p_vh_b = t.add("value/hidden/bias", {512});
   n->p_v_w = t.add("value/head/kernel", {512, 1});
@@ -163,8 +163,7 @@ extern "C" int seedrl_r2d2_net_set_mode(seedrl_r2d2_net* net, int mode) {
   return SEEDRL_OK;
 }
 extern "C" int seedrl_r2d2_net_set_lstm_mode(seedrl_r2d2_net* net, int mode) {
-  SEEDRL_CHECK_ARG(net && mode >= 1 && mode <= 3,
-                   "mode must be 1 (persistent), 2 (tiled persistent) or 3 (tiled persistent on wgmma bf16x3)");
+  SEEDRL_CHECK_ARG(net && (mode == 2 || mode == 3), "mode must be 2 (tiled) or 3 (tc3: tiled on wgmma bf16x3)");
   net->core.lstm_mode = mode;
   return SEEDRL_OK;
 }

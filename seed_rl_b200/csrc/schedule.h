@@ -96,19 +96,17 @@ struct GemmExec {
 };
 
 // The LSTM recurrence of one call (lstm.cu), Keras LSTMCell(H) with done-resets over T1 steps, in lstm_mode
-// `mode`: 0 per-step launches (z[t] += hp[t] U and dh_rec = dZ[t] U^T on ex's GEMM, pointwise kernels),
-// 1 persistent (lstm_persistent.cu), 2 tiled (lstm_tiled.cu), 3 tiled on wgmma bf16x3 (lstm_tc.cu).
+// `mode`: 2 tiled (lstm_tiled.cu), 3 tiled on wgmma bf16x3 (lstm_tc.cu); any other mode is refused.
 //   forward   z [T1,B,4H]: x W + b in, activated gates out; hs, cs, hp [T1,B,H] (hp[t] = h[t-1] with step t's
 //             resets applied)
-//   backward  dz [T1,B,4H] from the forward's gates and cs and dhs [T1,B,H]; mode 0 also takes dh_rec [B,H] and
-//             two dc buffers [B,H] as scratch
-// counter: 64 barrier counters (256 B), reset by each launch; ex.err: the bounded-wait error flag.
-int lstm_recurrence_forward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
-                            float* z, const float* h0, const float* c0, float* hs, float* cs, float* hp,
-                            unsigned int* counter);
-int lstm_recurrence_backward(int mode, const GemmExec& ex, int H, int T1, int B, const float* U, const uint8_t* done,
-                             const float* gates, const float* cs, const float* c0, const float* dhs, float* dz,
-                             float* dhrec, float* const dc[2], unsigned int* counter);
+//   backward  dz [T1,B,4H] from the forward's gates and cs and dhs [T1,B,H]
+// counter: 64 barrier counters (256 B), reset by each launch; err: the bounded-wait error flag.
+int lstm_recurrence_forward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, float* z,
+                            const float* h0, const float* c0, float* hs, float* cs, float* hp, unsigned int* counter,
+                            int* err, cudaStream_t st);
+int lstm_recurrence_backward(int mode, int H, int T1, int B, const float* U, const uint8_t* done, const float* gates,
+                             const float* cs, const float* c0, const float* dhs, float* dz, unsigned int* counter,
+                             int* err, cudaStream_t st);
 
 // The recurrent core both nets share (lstm.cu): Dense(flat -> H) + ReLU, concat(that, reward,
 // one_hot(prev_action, A)) = the core input [N, core_in], then Keras LSTMCell(H) with done-resets.
@@ -117,18 +115,16 @@ struct Core {
   int dense_w, dense_b, w, u, b;        // parameter indices: Dense kernel / bias, core kernel / recurrent / bias
   bool clip_reward;                     // reward clipped to [-1, 1] (ImpalaDeep, dmlab/networks.py:111)
   bool flat_relu;                       // ReLU applied to the flat features as Dense reads them (ImpalaDeep)
-  bool stepwise;                        // the net offers lstm_mode 0: the plan carves its BPTT scratch
   int lstm_mode = 2;
 };
 // Registers Dense (`dense` + "/kernel", "/bias"), then core/{kernel,recurrent_kernel,bias}.
-Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu,
-                 bool stepwise);
+Core core_create(ParamTable& t, const std::string& dense, int H, int flat, int A, bool clip_reward, bool flat_relu);
 
 // The core's buffers in a workspace of T1 x B frames (N = T1 * B rows): core input, gates, h[t-1], c, h, the
-// copy of c0, d h, d gates, (stepwise) dh_rec and two dc buffers, d dense_out, the LSTM barrier counters.
+// copy of c0, d h, d gates, d dense_out, the LSTM barrier counters.
 struct CorePlan {
   int T1, B, N;
-  size_t xc, z, hp, cs, hs, c0buf, dhs, dz, dhrec, dc[2], dd, counter;
+  size_t xc, z, hp, cs, hs, c0buf, dhs, dz, dd, counter;
 };
 CorePlan core_plan(const Core& k, Bump& b, int T1, int B);
 

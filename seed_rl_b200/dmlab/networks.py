@@ -39,7 +39,7 @@ class _CudaAgent(CudaNet):
     tensor cores with bf16 operands and fp32 accumulation, 'tc3' = wgmma with bf16x3 split
     operands (fp32-faithful).  lstm_mode selects how the recurrent products of the LSTM core are
     computed: 'tiled' = one persistent kernel each way on fp32 CUDA cores, 'tc3' = the same
-    recurrence on wgmma with bf16x3 operands, 'persistent' / 'stepwise' = earlier forms."""
+    recurrence on wgmma with bf16x3 operands."""
     self._num_actions = int(num_actions)
     self._obs_shape = tuple(int(x) for x in obs_shape)
     if self._NET == _lib.NET_DEEP and (len(self._obs_shape) != 3 or not 1 <= self._obs_shape[2] <= 16):
@@ -58,10 +58,9 @@ class _CudaAgent(CudaNet):
       raise ValueError("conv_mode 'tc3p' is built for the deep net")
     self.conv_mode = conv_mode
     _lib.check(L.seedrl_net_set_conv_mode(h, modes[conv_mode]))
-    lstm_modes = {'stepwise': 0, 'persistent': 1, 'tiled': 2, 'tc3': 3}
+    lstm_modes = {'tiled': 2, 'tc3': 3}
     if lstm_mode not in lstm_modes:
-      raise ValueError("lstm_mode must be 'tiled', 'tc3' (the tiled recurrence on wgmma bf16x3), "
-                       "'persistent' or 'stepwise'")
+      raise ValueError("lstm_mode must be 'tiled' or 'tc3' (the tiled recurrence on wgmma bf16x3)")
     self.lstm_mode = lstm_mode
     _lib.check(L.seedrl_net_set_lstm_mode(h, lstm_modes[lstm_mode]))
     self._setup(seed, device)

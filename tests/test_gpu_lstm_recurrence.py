@@ -1,9 +1,7 @@
 """The LSTM recurrence on its own (seedrl_debug_lstm_forward / _backward: the calls the networks make, csrc/lstm.cu)
 in every lstm_mode against a float64 Keras LSTMCell with done-resets, forward and BPTT.
 
-Modes: 0 per-step GEMM + pointwise kernels (H = 256 only: R2D2 refuses it; the per-step GEMM on the fp32 SIMT
-path, gemm_mode 0, and on wgmma bf16x3, gemm_mode 2), 1 persistent, 2 tiled, 3 tiled on wgmma bf16x3 ('tc3'), at
-H = 256 (IMPALA) and H = 512 (R2D2).
+Modes: 2 tiled, 3 tiled on wgmma bf16x3 ('tc3'), at H = 256 (IMPALA) and H = 512 (R2D2).
 
 Reference: `ref_forward` / `ref_backward` below, the schedule of tests/test_backward_formulas.py in float64 on the
 same fp32 inputs the GPU gets; `test_reference_matches_torch_float64_autograd` checks it against torch autograd
@@ -11,8 +9,8 @@ through oracle/net_oracle.lstm_cell.
 
 Bars (DESIGN.md's sensitivity rule).  For each output (gates, hs, cs, hp, final (h, c), dz, and dU = hp^T dz taken
 in float64 from the GPU's hp and dz) the error is max|gpu - ref| / max|ref|.  The response is the same measure
-between the reference and the reference run on U, x W + b, h0 and c0 each multiplied by (1 +- 2^-24) (modes 0-2,
-fp32 rounding) or (1 +- 2^-16) (mode 3 and mode 0 on the bf16x3 GEMM), random signs.  The bar is
+between the reference and the reference run on U, x W + b, h0 and c0 each multiplied by (1 +- 2^-24) (mode 2,
+fp32 rounding) or (1 +- 2^-16) (mode 3), random signs.  The bar is
 max(FLOOR, K x response) with K = SENS_MULT and FLOOR below, one pair for every case.  The kernels round at every
 step while the probe perturbs the inputs once, so K leaves room for accumulation over 141 steps.
 
@@ -25,7 +23,7 @@ dz / dU, only where T1 > 1), but a defect worth a fraction of one lo product wou
 Also checked: nothing is written outside the outputs (every output has a NaN-filled extra time step and extra rows
 that must stay NaN, and every element inside must be written); two calls are bit-identical, also when a call in
 another mode used the workspace in between; the error flag stays 0; H = 128 and one row past each mode's batch
-limit are refused with nothing launched.
+limit are refused with nothing launched, and so is every mode but 2 and 3.
 """
 import zlib
 
@@ -37,9 +35,9 @@ SENS_MULT = 8
 FLOOR = 2e-6
 
 
-def _eps(mode, gemm_mode=0):
+def _eps(mode):
   """Relative input perturbation of the response: fp32 rounding, or the bf16x3 model."""
-  return 2.0 ** -16 if mode == 3 or gemm_mode == 2 else 2.0 ** -24
+  return 2.0 ** -16 if mode == 3 else 2.0 ** -24
 
 OUTPUTS = ('gates', 'hs', 'cs', 'hp', 'h_T', 'c_T', 'dz', 'dU')
 INVALID_ARGUMENT = 3
@@ -190,12 +188,8 @@ def test_reference_matches_torch_float64_autograd():
 
 # ---- batch limits of the launchers --------------------------------------------------------------------------
 def batch_limit(mode, H, bwd):
-  """The largest batch each launcher takes (lstm_persistent.cu, lstm_tiled.cu, lstm_tc.cu)."""
+  """The largest batch each launcher takes (lstm_tiled.cu, lstm_tc.cu)."""
   def fits(B):
-    if mode == 1:          # B x NU floats of cell state (gradient) in at most 200 KiB of shared memory
-      NU = 2 if H == 256 else 4
-      f = (NU * 4 * H + 2 * 64 * 132 + 64 * NU + B * NU) if bwd else (H * 4 * NU + 64 * (H + 4) + 64 * 4 * NU + B * NU)
-      return 4 * f <= 200 * 1024
     if mode == 2:          # at most 64 tiles of at most 32 rows, fewer rows where shared memory runs out
       KC = min(4 * H, 1024)
       smem = lambda r: 4 * ((4 * H * 16 + KC * r + 16 * r * 16 + r * 16) if bwd else (H * 64 + H * r + 8 * r * 64 + r * 16))
@@ -215,7 +209,6 @@ def batch_limit(mode, H, bwd):
 
 def test_batch_limits():
   """The limits the launchers are pinned to (CPU restatement; the GPU tests below run at and one past them)."""
-  assert [batch_limit(1, H, b) for H in (256, 512) for b in (False, True)] == [16000, 16064, 2240, 6464]
   assert [batch_limit(2, H, b) for H in (256, 512) for b in (False, True)] == [2048, 1536, 1024, 1024]
   assert [batch_limit(3, H, b) for H in (256, 512) for b in (False, True)] == [4096] * 4
 
@@ -243,32 +236,32 @@ class Runner:
     buf = torch.full((n + (self.B + 8) * width,), float('nan'), device='cuda')
     return buf, buf[:n].view(self.T1, self.B, width)
 
-  def forward(self, mode, gemm_mode=0):
+  def forward(self, mode):
     L = _lib()
     H = self.H
     bufs = {k: self.guarded(w) for k, w in (('z', 4 * H), ('hs', H), ('cs', H), ('hp', H))}
     bufs['z'][1].copy_(self.xwb)
     rc = L.lib().seedrl_debug_lstm_forward(
-        mode, gemm_mode, H, self.T1, self.B, L.ptr(self.U), L.ptr(self.done), L.ptr(bufs['z'][1]),
+        mode, H, self.T1, self.B, L.ptr(self.U), L.ptr(self.done), L.ptr(bufs['z'][1]),
         L.ptr(self.h0), L.ptr(self.c0), L.ptr(bufs['hs'][1]), L.ptr(bufs['cs'][1]), L.ptr(bufs['hp'][1]),
         L.ptr(self.ws), self.ws.numel(), L.ptr(self.flag), L.stream_ptr())
     return rc, bufs
 
-  def backward(self, mode, gates, cs, gemm_mode=0):
+  def backward(self, mode, gates, cs):
     L = _lib()
     buf = self.guarded(4 * self.H)
     rc = L.lib().seedrl_debug_lstm_backward(
-        mode, gemm_mode, self.H, self.T1, self.B, L.ptr(self.U), L.ptr(self.done), L.ptr(gates),
+        mode, self.H, self.T1, self.B, L.ptr(self.U), L.ptr(self.done), L.ptr(gates),
         L.ptr(cs), L.ptr(self.c0), L.ptr(self.dhs), L.ptr(buf[1]), L.ptr(self.ws), self.ws.numel(),
         L.ptr(self.flag), L.stream_ptr())
     return rc, buf
 
-  def step(self, mode, gemm_mode=0, bptt=True):
+  def step(self, mode, bptt=True):
     """forward, then BPTT from its gates and cs: {name: (guarded buffer, view)}."""
-    rc, bufs = self.forward(mode, gemm_mode)
+    rc, bufs = self.forward(mode)
     _lib().check(rc)
     if bptt:
-      rc, bufs['dz'] = self.backward(mode, bufs['z'][1], bufs['cs'][1], gemm_mode)
+      rc, bufs['dz'] = self.backward(mode, bufs['z'][1], bufs['cs'][1])
       _lib().check(rc)
     torch.cuda.synchronize()
     assert int(self.flag.item()) == 0, 'a barrier wait expired'
@@ -280,7 +273,7 @@ class Runner:
 
 
 def _ws_bytes(H, T1, B):
-  return max(_lib().lib().seedrl_debug_lstm_workspace_bytes(m, H, T1, B) for m in range(4))
+  return max(_lib().lib().seedrl_debug_lstm_workspace_bytes(m, H, T1, B) for m in (2, 3))
 
 
 def _gpu_outputs(bufs):
@@ -323,8 +316,8 @@ CASES = [
     ('noncoop_3x1024', 3, 1024, 'mixed', 'keras', (512,)),
     ('noncoop_3x640', 3, 640, 'tail', 'keras', (256,)),       # tc3: 10 tiles x 16 unit groups
 ]
-ARMS = {256: ((0, 0), (0, 2), (1, 0), (2, 0), (3, 0)), 512: ((1, 0), (2, 0), (3, 0))}    # (mode, gemm_mode)
-GRID = [(name, H, mode, g) for name, _, _, _, _, Hs in CASES for H in Hs for mode, g in ARMS[H]]
+ARMS = {256: (2, 3), 512: (2, 3)}    # lstm modes
+GRID = [(name, H, mode) for name, _, _, _, _, Hs in CASES for H in Hs for mode in ARMS[H]]
 _CACHE = {}
 
 
@@ -335,29 +328,27 @@ def _case(name, H):
     _CACHE.clear()
     _, T1, B, pattern, regime, _ = next(c for c in CASES if c[0] == name)
     inp = make_inputs(H, T1, B, pattern, regime, seed=zlib.crc32(('%s/%d' % key).encode()))
-    _CACHE[key] = (inp,) + reference_and_responses(inp, [_eps(*arm) for arm in ARMS[H]])
+    _CACHE[key] = (inp,) + reference_and_responses(inp, [_eps(mode) for mode in ARMS[H]])
   return _CACHE[key]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('name,H,mode,gemm_mode', GRID,
-                         ids=['%s-H%d-mode%d%s' % (n, H, m, '-gemm2' if g else '') for n, H, m, g in GRID])
-def test_recurrence_matches_float64(name, H, mode, gemm_mode):
+@pytest.mark.parametrize('name,H,mode', GRID, ids=['%s-H%d-mode%d' % arm for arm in GRID])
+def test_recurrence_matches_float64(name, H, mode):
   inp, ref, resp = _case(name, H)
   T1, B = inp['xwb'].shape[:2]
   r = Runner(inp, _ws_bytes(H, T1, B))
-  first = r.step(mode, gemm_mode)
-  _check('mode %d%s H %d %dx%d %s' % (mode, ' gemm 2' if gemm_mode else '', H, T1, B, name), _eps(mode, gemm_mode),
-         _gpu_outputs(first), ref, resp)
+  first = r.step(mode)
+  _check('mode %d H %d %dx%d %s' % (mode, H, T1, B, name), _eps(mode), _gpu_outputs(first), ref, resp)
   # bit-identical on a repeat after a call in another mode on the same workspace and error flag
   r.step(3 if mode != 3 else 2)
-  again = r.step(mode, gemm_mode)
+  again = r.step(mode)
   for k in first:
     assert torch.equal(first[k][0].nan_to_num(7.0), again[k][0].nan_to_num(7.0)), k
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('H,mode', [(256, 1), (256, 2), (256, 3), (512, 1), (512, 2), (512, 3)])
+@pytest.mark.parametrize('H,mode', [(256, 2), (256, 3), (512, 2), (512, 3)])
 def test_largest_batch(H, mode):
   """The forward at its mode's largest batch, the BPTT at its own (from the reference's forward, rounded to fp32,
   where that batch is past the forward's limit)."""
@@ -386,7 +377,7 @@ def test_largest_batch(H, mode):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('H,mode', [(256, 1), (256, 2), (256, 3), (512, 1), (512, 2), (512, 3)])
+@pytest.mark.parametrize('H,mode', [(256, 2), (256, 3), (512, 2), (512, 3)])
 def test_one_row_past_the_limit_is_refused(H, mode):
   L = _lib()
   for bwd in (False, True):
@@ -409,7 +400,7 @@ def test_one_row_past_the_limit_is_refused(H, mode):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('mode', [0, 1, 2, 3])
+@pytest.mark.parametrize('mode', [2, 3])
 def test_bad_hidden_size_and_arguments_are_refused(mode):
   L = _lib()
   T1, B = 2, 8
@@ -418,22 +409,22 @@ def test_bad_hidden_size_and_arguments_are_refused(mode):
   need = L.lib().seedrl_debug_lstm_workspace_bytes(mode, 256, T1, B)
   assert need > 0
 
-  def fwd(H, gemm_mode=0, ws_bytes=r.ws.numel()):
-    return L.lib().seedrl_debug_lstm_forward(mode, gemm_mode, H, T1, B, L.ptr(r.U), L.ptr(r.done), L.ptr(z),
+  def fwd(H, ws_bytes=r.ws.numel(), m=mode):
+    return L.lib().seedrl_debug_lstm_forward(m, H, T1, B, L.ptr(r.U), L.ptr(r.done), L.ptr(z),
                                              L.ptr(r.h0), L.ptr(r.c0), L.ptr(o), L.ptr(o), L.ptr(o), L.ptr(r.ws),
                                              ws_bytes, L.ptr(r.flag), L.stream_ptr())
 
-  def bwd(H, ws_bytes=r.ws.numel()):
-    return L.lib().seedrl_debug_lstm_backward(mode, 0, H, T1, B, L.ptr(r.U), L.ptr(r.done), L.ptr(z), L.ptr(o),
+  def bwd(H, ws_bytes=r.ws.numel(), m=mode):
+    return L.lib().seedrl_debug_lstm_backward(m, H, T1, B, L.ptr(r.U), L.ptr(r.done), L.ptr(z), L.ptr(o),
                                               L.ptr(r.c0), L.ptr(r.dhs), L.ptr(z), L.ptr(r.ws), ws_bytes,
                                               L.ptr(r.flag), L.stream_ptr())
   torch.cuda.synchronize()
   n0 = L.launch_count()
   assert fwd(128) == INVALID_ARGUMENT and bwd(128) == INVALID_ARGUMENT          # H = 128 (buffers hold H = 256)
   assert fwd(256, ws_bytes=need - 1) == INVALID_ARGUMENT and bwd(256, ws_bytes=need - 1) == INVALID_ARGUMENT
-  assert fwd(256, gemm_mode=1) == INVALID_ARGUMENT                             # only the fp32 / bf16x3 GEMMs
-  if mode == 0:                                                                 # the networks run mode 0 at H = 256
-    assert fwd(512) == INVALID_ARGUMENT and bwd(512) == INVALID_ARGUMENT
+  for m in (0, 1, 4, -1):                                                       # only the tiled and tc3 recurrences
+    assert L.lib().seedrl_debug_lstm_workspace_bytes(m, 256, T1, B) == 0
+    assert fwd(256, m=m) == INVALID_ARGUMENT and bwd(256, m=m) == INVALID_ARGUMENT
   torch.cuda.synchronize()
   assert L.launch_count() == n0
   assert torch.equal(z, r.xwb) and torch.isnan(o).all() and int(r.flag.item()) == 0

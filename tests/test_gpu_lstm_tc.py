@@ -305,8 +305,17 @@ def test_unknown_lstm_modes_are_rejected():
     networks.ImpalaShallow(A, OBS, lstm_mode='tc')
   with pytest.raises(ValueError, match='tc3'):
     atari_networks.DuelingLSTMDQNNet(R_A, R_OBS, R_S, lstm_mode='stepwise')
+  with pytest.raises(ValueError, match='tc3'):
+    networks.ImpalaShallow(A, OBS, lstm_mode='stepwise')
+  with pytest.raises(ValueError, match='tc3'):
+    networks.ImpalaShallow(A, OBS, lstm_mode='persistent')
+  with pytest.raises(ValueError, match='tc3'):
+    atari_networks.DuelingLSTMDQNNet(R_A, R_OBS, R_S, lstm_mode='persistent')
   agent = networks.ImpalaShallow(A, OBS, lstm_mode='tc3')
   assert _lib.lib().seedrl_net_set_lstm_mode(agent._h, 4) != 0
   r2d2 = atari_networks.DuelingLSTMDQNNet(R_A, R_OBS, R_S, lstm_mode='tc3')
   assert _lib.lib().seedrl_r2d2_net_set_lstm_mode(r2d2._h, 0) != 0
+  for mode in (0, 1):                  # only 2 (tiled) and 3 (tc3) exist
+    assert _lib.lib().seedrl_net_set_lstm_mode(agent._h, mode) == 3        # SEEDRL_ERR_INVALID_ARGUMENT
+    assert _lib.lib().seedrl_r2d2_net_set_lstm_mode(r2d2._h, mode) == 3
   assert r2d2.lstm_mode == 'tc3' and agent.lstm_mode == 'tc3'

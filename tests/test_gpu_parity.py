@@ -450,7 +450,11 @@ def _batch_to_cuda(b):
   return learner.Unroll((_cuda(b['h0']), _cuda(b['c0'])), _cuda(b['prev_actions']), env, ao)
 
 
-@pytest.mark.parametrize('net,T,B', [('deep', 3, 2), ('shallow', 3, 2), ('deep', 1, 5)])
+# The shallow net's (T, B) cover the recurrence's batch-tile classes; at B = 300 the tiled LSTM kernel takes its
+# non-cooperative launch (10 forward / 13 BPTT batch tiles x 16 unit groups > 132 SMs).
+@pytest.mark.parametrize('net,T,B', [('deep', 3, 2), ('shallow', 3, 2), ('deep', 1, 5), ('shallow', 6, 5),
+                                     ('shallow', 3, 70), ('shallow', 1, 3), ('shallow', 20, 64),
+                                     ('shallow', 5, 256), ('shallow', 4, 300)])
 def test_network_forward_matches_oracle(net, T, B):
   A = 18
   agent, params = _make_agent(net, A)
@@ -480,7 +484,7 @@ def test_network_forward_matches_oracle(net, T, B):
   np.testing.assert_allclose(o1.policy_logits.cpu().numpy(), logits[0].numpy(), rtol=2e-4, atol=2e-5)
 
 
-@pytest.mark.parametrize('net,T,B', [('deep', 4, 3), ('shallow', 4, 3)])
+@pytest.mark.parametrize('net,T,B', [('deep', 4, 3), ('shallow', 4, 3), ('shallow', 4, 300)])
 def test_learner_step_gradients_and_update_match_oracle(net, T, B):
   """compute_loss -> backward -> Adam against the CPU learner (oracle) for 3 steps."""
   from seed_rl_b200.agents.vtrace import learner

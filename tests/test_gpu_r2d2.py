@@ -97,7 +97,11 @@ def _to_cuda_inputs(b, S):
 
 
 @pytest.mark.parametrize('mode,tol', [('simt', 2e-4), ('tc3', 5e-4)])
-@pytest.mark.parametrize('T,B,A,obs,S', [(5, 3, 6, (36, 36, 1), 4), (3, 2, 18, (84, 84, 1), 4), (4, 2, 4, (44, 40, 4), 1)])
+# B = 9, 40, 64, 100: the tiled LSTM(512) kernel's 8- and 16-row batch tiles, full and ragged, and at B = 100 its
+# non-cooperative launch (7 batch tiles x 32 unit groups > 132 SMs)
+@pytest.mark.parametrize('T,B,A,obs,S', [(5, 3, 6, (36, 36, 1), 4), (3, 2, 18, (84, 84, 1), 4), (4, 2, 4, (44, 40, 4), 1),
+                                         (5, 40, 6, (36, 36, 1), 4), (3, 64, 6, (36, 36, 1), 4),
+                                         (4, 9, 6, (36, 36, 1), 4), (2, 100, 6, (36, 36, 1), 4)])
 def test_dueling_net_forward_backward_vs_oracle(mode, tol, T, B, A, obs, S):
   from oracle import r2d2_net_oracle as NO
   from seed_rl_b200.atari import networks
