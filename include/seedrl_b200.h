@@ -486,7 +486,6 @@ int seedrl_debug_set_wgrad_chunk(int kc);
 /* Output positions per tile of the tensor-core forward / data-gradient kernel: the largest
  * of 512 / 256 / 128 not above `mt` that keeps two CTAs per SM is used (default 512). */
 int seedrl_debug_set_conv_tile(int mt);
-int seedrl_debug_set_gemm_bk(int bk);     /* gemm_tc_kernel K elements per staged block: 64 or 32 */
 /* 0 = the im2col convolutions (IMPALA shallow net, R2D2 body) materialise their matrices instead of
  * gathering them while the GEMM stages its operand (default 1; bit-identical results). */
 int seedrl_debug_set_gemm_gather(int on);
@@ -515,9 +514,9 @@ int seedrl_debug_conv3x3_wgrad(int cin, int cout, int in_mode, int N, int H, int
                                seedrl_stream_t stream);
 /* wgmma (tensor-core, bf16 x bf16 -> fp32) 3x3 convolution: packs fp32 HWIO weights
  * (flip != 0: flipped + transposed, i.e. the data-gradient; split != 0: bf16x3 hi/lo
- * operands, fp32-faithful) into wq_scratch (>= 2*9*max(cin,16)*cout*2 bytes) and runs the implicit-GEMM kernel.  variant bit0/bit1 swap the
- * LBO/SBO fields of the A/B shared-memory descriptors (bring-up aid).  The kernel has no
- * bounded waits: *error_flag is left unchanged. */
+ * operands, fp32-faithful) into wq_scratch (>= 2*9*max(cin,16)*cout*2 bytes) and runs the implicit-GEMM kernel.
+ * `variant` must be 0 (any other value is refused with SEEDRL_ERR_INVALID_ARGUMENT before anything
+ * is packed or launched).  The kernel has no bounded waits: *error_flag is left unchanged. */
 int seedrl_debug_conv3x3_tc(int cin, int cout, int in_mode, int split, int N, int H, int W,
                             const void* in, const float* w, const float* bias,
                             const float* mask, const float* res, float* out, int flip,

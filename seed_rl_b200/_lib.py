@@ -171,7 +171,6 @@ SIGNATURES = {
     'seedrl_debug_set_loss_stream': (c_int, [c_int]),
     'seedrl_debug_set_wgrad_chunk': (c_int, [c_int]),
     'seedrl_debug_set_conv_tile': (c_int, [c_int]),
-    'seedrl_debug_set_gemm_bk': (c_int, [c_int]),
     'seedrl_debug_set_first_layer_dense': (c_int, [c_int]),
     'seedrl_debug_conv0pool': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P]),
     'seedrl_debug_conv0pool_c': (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P]),

@@ -1,5 +1,6 @@
 // Shared helpers for libseedrl_b200 (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -41,13 +42,14 @@ inline int set_error(int code, const std::string& msg) {
                                    cudaGetErrorString(e__));                \
   } while (0)
 
-#define SEEDRL_CUDA(call)                                                   \
+// variadic so that the call may name a template with several arguments
+#define SEEDRL_CUDA(...)                                                    \
   do {                                                                      \
-    cudaError_t e__ = (call);                                               \
+    cudaError_t e__ = (__VA_ARGS__);                                        \
     if (e__ != cudaSuccess)                                                 \
       return ::seedrl::set_error(                                           \
           SEEDRL_ERR_INTERNAL,                                              \
-          std::string(__func__) + ": " #call ": " + cudaGetErrorString(e__)); \
+          std::string(__func__) + ": " #__VA_ARGS__ ": " + cudaGetErrorString(e__)); \
   } while (0)
 
 // Optional per-category kernel timing (CUDA events on the launching stream), used by
@@ -65,6 +67,32 @@ inline void count_launch(int cat = PC_MISC, cudaStream_t st = 0) {
 }
 
 constexpr int kNumSMs = 132;  // H100 SXM
+
+// Opts kernel K into `bytes` of dynamic shared memory (more than the 48 KB default).  The attribute is
+// set on the kernel's first launch only; the function-local static is initialised exactly once even when
+// the inference and learner threads reach that launch together.
+template <auto K>
+cudaError_t allow_smem(int bytes) {
+  static const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  return e;
+}
+
+// cuTensorMapEncodeTiled of the driver the runtime loaded (the library does not link libcuda), looked up
+// once; null when that driver does not have it.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline EncodeTiledFn encode_tiled_fn() {
+  static const EncodeTiledFn fn = [] {
+    void* q = nullptr;
+    cudaDriverEntryPointQueryResult qr;
+    const bool found = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) == cudaSuccess &&
+                       qr == cudaDriverEntryPointSuccess;
+    (void)cudaGetLastError();
+    return found ? reinterpret_cast<EncodeTiledFn>(q) : nullptr;
+  }();
+  return fn;
+}
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline size_t ceil_div_sz(size_t a, size_t b) { return (a + b - 1) / b; }

@@ -17,7 +17,6 @@
 // go through the deterministic deferred reduce.
 #include <cuda.h>
 
-#include <cstdlib>
 #include <cstring>
 
 #include "kernels.h"
@@ -179,12 +178,6 @@ __global__ void __launch_bounds__(kFwThreads, kU32 ? 3 : 2) first_wgrad_pooled_k
   }
 }
 
-static void same_pad3s2_(int in, int* out, int* before) {
-  *out = (in + 1) / 2;
-  const int total = (*out - 1) * 2 + 3 - in;
-  *before = total > 0 ? total / 2 : 0;
-}
-
 bool first_wgrad_pooled_supported(int cin, int cout, int H, int W) {
   if (cin < 1 || cin > 16 || cout != 16 || H < 3 || W < 3) return false;
   const int cp = first_layer_cp(cin);
@@ -193,12 +186,7 @@ bool first_wgrad_pooled_supported(int cin, int cout, int H, int W) {
 
 template <int CP, bool kU32>
 static int launch_first_wgrad(const FirstWgradArgs& a, int grid, size_t smem, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(first_wgrad_pooled_kernel<CP, kU32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     72 * 1024));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<first_wgrad_pooled_kernel<CP, kU32>>(72 * 1024));
   first_wgrad_pooled_kernel<CP, kU32><<<grid, kFwThreads, smem, st>>>(a);
   return SEEDRL_OK;
 }
@@ -210,8 +198,8 @@ int first_wgrad_pooled(int N, int H, int W, int C, const uint8_t* frames, const 
   if (!first_wgrad_pooled_supported(C, 16, H, W))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "first_wgrad_pooled: unsupported frame shape");
   int Ho, Wo, pt, pl;
-  same_pad3s2_(H, &Ho, &pt);
-  same_pad3s2_(W, &Wo, &pl);
+  same_pad3s2(H, &Ho, &pt);
+  same_pad3s2(W, &Wo, &pl);
   const int cp = first_layer_cp(C);
   FirstWgradArgs a;
   a.N = N; a.H = H; a.W = W; a.C = C; a.Ho = Ho; a.Wo = Wo; a.pt = pt; a.pl = pl;
@@ -269,9 +257,9 @@ int first_wgrad_pooled(int N, int H, int W, int C, const uint8_t* frames, const 
 //   CP = 16 (C = 9..16): two such arrays (channels 0-7, 8-15; LBO = the array stride), one MMA per tap.
 // Such frames are read with plain loads straight from HBM (their W*C-byte row pitch rarely meets the
 // TMA's 16-byte rule, and a W*C-byte box row exceeds its 256-element limit).
-// kCpRows pooled rows per unit (template parameter: 3 -> up to 6 blocks of 128 positions, 2 CTAs / SM;
-// 2 -> up to 4 blocks, 3 CTAs / SM).
 constexpr int kCpThreadsF = 256;
+constexpr int kCpRows = 3;          // pooled rows per unit: 7 conv rows ...
+constexpr int kCpMaxBlocks = 6;     // ... in at most 6 blocks of 128 positions
 constexpr int kCpOutStride = 20;    // floats per position in the fp32 tile (16 + 4: pool reads 2-way conflict)
 
 struct Conv0PoolArgs {
@@ -302,11 +290,10 @@ __device__ __forceinline__ uint2 u8x4_to_bf16x4(uint32_t w32) {
 // nothing) into one of two raw stages; the copy of the NEXT unit's tile is in flight while this
 // unit converts, multiplies and pools.
 // CP = 4 with kTma: 4-channel frames (the tile copy above); otherwise plain loads, C <= CP channels.
-template <int kCpRows, int CP, bool kTma>
-__global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_kernel(const __grid_constant__ CUtensorMap tm_frames,
+template <int CP, bool kTma>
+__global__ void __launch_bounds__(kCpThreadsF, 2) conv0pool_kernel(const __grid_constant__ CUtensorMap tm_frames,
                                                                     const Conv0PoolArgs a) {
   static_assert(CP == 4 || !kTma, "the tile copy reads 4-channel pixels");
-  constexpr int kCpMaxBlocks = kCpRows == 2 ? 4 : 6;
   constexpr int kPlanes = CP == 16 ? 2 : 1;                   // 16-byte arrays of the A operand
   constexpr int KH = CP == 16 ? 48 : 4 * CP;                  // B rows (K) per kernel row
   constexpr int KT = 3 * KH;
@@ -547,12 +534,6 @@ __global__ void __launch_bounds__(kCpThreadsF, kCpRows == 2 ? 3 : 2) conv0pool_k
   if (timed_out && a.err) atomicExch(a.err, 1);
 }
 
-static int g_c0_rows = getenv("SEEDRL_C0_ROWS") ? (atoi(getenv("SEEDRL_C0_ROWS")) == 2 ? 2 : 3) : 3;
-void conv0pool_set_rows(int rows) { g_c0_rows = rows == 2 ? 2 : 3; }
-static int c0_rows(int W) {                      // pooled rows per unit that fit the block budget
-  if (g_c0_rows == 2 && 5 * (W + 2) <= 4 * 128) return 2;
-  return 3;
-}
 bool conv0pool_supported(int cin, int cout, int H, int W) {
   // 7 conv rows of the widest band in 6 blocks of 128 positions: W <= 107
   if (cout != 16 || H < 3 || W < 3 || 7 * (W + 2) > 6 * 128) return false;
@@ -561,73 +542,57 @@ bool conv0pool_supported(int cin, int cout, int H, int W) {
   return cin >= 1 && cin <= 16;
 }
 
-template <int ROWS, int CP, bool TMA>
+template <int CP, bool TMA>
 static int launch_conv0pool(Conv0PoolArgs a, const uint8_t* frames, cudaStream_t st) {
-  constexpr int MAXB = ROWS == 2 ? 4 : 6;
   constexpr int KT = 3 * (CP == 16 ? 48 : 4 * CP);
   const int N = a.N, H = a.H, W = a.W;
-  const size_t raw_stride = TMA ? (((size_t)(2 * ROWS + 3) * W * 4) + 127) / 128 * 128 : 0;
-  const size_t smem = (size_t)(CP == 16 ? 2 : 1) * (MAXB * 128 + 2 * (W + 2) + 8) * 16 +
-                      (size_t)MAXB * 128 * kCpOutStride * 4 + 128 + KT * 32 * 2 + 16 * 4 + 64 + 128 + 2 * raw_stride;
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(conv0pool_kernel<ROWS, CP, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     112 * 1024));
-    attr = true;
-  }
+  const size_t raw_stride = TMA ? (((size_t)(2 * kCpRows + 3) * W * 4) + 127) / 128 * 128 : 0;
+  const size_t smem = (size_t)(CP == 16 ? 2 : 1) * (kCpMaxBlocks * 128 + 2 * (W + 2) + 8) * 16 +
+                      (size_t)kCpMaxBlocks * 128 * kCpOutStride * 4 + 128 + KT * 32 * 2 + 16 * 4 + 64 + 128 +
+                      2 * raw_stride;
+  SEEDRL_CUDA(allow_smem<conv0pool_kernel<CP, TMA>>(112 * 1024));
   if (smem > 112 * 1024) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv0pool: image too wide");
   CUtensorMap tm;
   memset(&tm, 0, sizeof(tm));                    // plain-load variants never read it
   if (TMA) {
     // [N][H][W] view of the frames with one uint32 (= 4 uint8 channels) per pixel
-    typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeTiledFn enc = nullptr;
-    if (!enc) {
-      void* q = nullptr;
-      cudaDriverEntryPointQueryResult qr;
-      if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) != cudaSuccess ||
-          qr != cudaDriverEntryPointSuccess)
-        return set_error(SEEDRL_ERR_INTERNAL, "cuTensorMapEncodeTiled is not available");
-      enc = reinterpret_cast<EncodeTiledFn>(q);
-    }
+    const EncodeTiledFn enc = encode_tiled_fn();
+    if (!enc) return set_error(SEEDRL_ERR_INTERNAL, "cuTensorMapEncodeTiled is not available");
     const cuuint64_t gdim[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     const cuuint64_t gstr[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-    const cuuint32_t box[3] = {(cuuint32_t)W, (cuuint32_t)(2 * ROWS + 3), 1};
+    const cuuint32_t box[3] = {(cuuint32_t)W, (cuuint32_t)(2 * kCpRows + 3), 1};
     const cuuint32_t estr[3] = {1, 1, 1};
     if (enc(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, const_cast<uint8_t*>(frames), gdim, gstr, box, estr,
             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return set_error(SEEDRL_ERR_INTERNAL, "conv0pool: cuTensorMapEncodeTiled failed");
   }
-  const int units = N * ((a.Ho + ROWS - 1) / ROWS);
-  const int per_sm = ROWS == 2 ? 3 : 2;
-  const int grid = units < per_sm * kNumSMs ? units : per_sm * kNumSMs;
-  conv0pool_kernel<ROWS, CP, TMA><<<grid, kCpThreadsF, smem, st>>>(tm, a);
+  const int units = N * ((a.Ho + kCpRows - 1) / kCpRows);
+  const int grid = units < 2 * kNumSMs ? units : 2 * kNumSMs;       // 2 CTAs / SM
+  conv0pool_kernel<CP, TMA><<<grid, kCpThreadsF, smem, st>>>(tm, a);
   count_launch(PC_CONV_FWD, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
 }
 
 // frames: [N,H,W,C] uint8, w: [3,3,C,16].  4-channel frames take the TMA-fed kernel; other channel
-// counts the plain-load kernels with 3 pooled rows per unit.
+// counts the plain-load kernels.
 int conv0pool_forward(int N, int H, int W, int C, const uint8_t* frames, const float* w, const float* bias,
                       void* praw, void* prelu, uint8_t* idx, int* err, cudaStream_t st) {
   if (!conv0pool_supported(C, 16, H, W))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv0pool: unsupported frame shape");
   Conv0PoolArgs a;
   a.N = N; a.H = H; a.W = W; a.C = C;
-  same_pad3s2_(H, &a.Ho, &a.pt);
-  same_pad3s2_(W, &a.Wo, &a.pl);
+  same_pad3s2(H, &a.Ho, &a.pt);
+  same_pad3s2(W, &a.Wo, &a.pl);
   a.Lpp = (int)planes_positions(N, a.Ho, a.Wo); a.PWp = a.Wo + 2; a.RHp = a.Ho + 1;
   fast_div_setup((unsigned int)(W + 2), &a.sw_mul, &a.sw_sh);
   a.frames = frames; a.w = w; a.bias = bias;
   a.praw = reinterpret_cast<uint4*>(praw); a.prelu = reinterpret_cast<uint4*>(prelu); a.idx = idx; a.err = err;
-  if (C == 4) return c0_rows(W) == 2 ? launch_conv0pool<2, 4, true>(a, frames, st) : launch_conv0pool<3, 4, true>(a, frames, st);
+  if (C == 4) return launch_conv0pool<4, true>(a, frames, st);
   const int cp = first_layer_cp(C);
-  return cp == 4 ? launch_conv0pool<3, 4, false>(a, frames, st)
-                 : (cp == 8 ? launch_conv0pool<3, 8, false>(a, frames, st) : launch_conv0pool<3, 16, false>(a, frames, st));
+  return cp == 4 ? launch_conv0pool<4, false>(a, frames, st)
+                 : (cp == 8 ? launch_conv0pool<8, false>(a, frames, st) : launch_conv0pool<16, false>(a, frames, st));
 }
 
 }  // namespace seedrl

@@ -170,12 +170,7 @@ static int launch_conv3x3(int N, int H, int W, const void* in, const float* w, c
   const ConvGeom g = make_geom(N, H, W);
   const int L = Cfg::QC + 2 * g.PW + 2;
   const size_t smem = ((size_t)CIN * (L | 1) + 9 * CIN * COUT) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(conv3x3_kernel<CIN, COUT, IN_MODE>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<conv3x3_kernel<CIN, COUT, IN_MODE>>(200 * 1024));
   if (smem > 200 * 1024) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3: image too wide");
   if (g.Q + Cfg::QC + 4 * g.PW >= (1LL << 31))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3: batch too large for 32-bit positions");
@@ -393,12 +388,7 @@ static int launch_wgrad(int N, int H, int W, const void* x, const float* dy, flo
   size_t smem = ((((size_t)L * (CIN + 1) + 3) & ~(size_t)3) + (size_t)Cfg::QC * COUT) * sizeof(float);
   const size_t red = (size_t)Cfg::G * NW * sizeof(float);
   if (red > smem) smem = red;
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_kernel<CIN, COUT, IN_MODE>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<conv3x3_wgrad_kernel<CIN, COUT, IN_MODE>>(200 * 1024));
   if (smem > 200 * 1024) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad: tile too large");
   if (g.Q + Cfg::QC + 4 * g.PW >= (1LL << 31))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad: batch too large for 32-bit positions");
@@ -564,18 +554,11 @@ __global__ void maxpool3s2_bwd_kernel(int N, int H, int W, int C, int Ho, int Wo
   }
 }
 
-static void same_pad(int n, int k, int s, int* out, int* before) {
-  *out = (n + s - 1) / s;
-  int total = (*out - 1) * s + k - n;
-  if (total < 0) total = 0;
-  *before = total / 2;
-}
-
 int maxpool3s2_forward(int N, int H, int W, int C, const float* x, float* y, uint8_t* idx,
                        cudaStream_t st) {
   int Ho, Wo, pt, pl;
-  same_pad(H, 3, 2, &Ho, &pt);
-  same_pad(W, 3, 2, &Wo, &pl);
+  same_pad3s2(H, &Ho, &pt);
+  same_pad3s2(W, &Wo, &pl);
   const long long total = (long long)N * Ho * Wo * (C / 4);
   (void)total;
   const int per_row = Wo * (C / 4);
@@ -590,8 +573,8 @@ int maxpool3s2_forward(int N, int H, int W, int C, const float* x, float* y, uin
 int maxpool3s2_backward(int N, int H, int W, int C, const float* dy, const uint8_t* idx, float* dx,
                         cudaStream_t st) {
   int Ho, Wo, pt, pl;
-  same_pad(H, 3, 2, &Ho, &pt);
-  same_pad(W, 3, 2, &Wo, &pl);
+  same_pad3s2(H, &Ho, &pt);
+  same_pad3s2(W, &Wo, &pl);
   const long long total = (long long)N * H * W * (C / 4);
   (void)total;
   const int per_row = ((W + pl + 1) / 2) * (C / 4);

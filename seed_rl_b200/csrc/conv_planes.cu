@@ -38,7 +38,6 @@
 #include <cuda_bf16.h>
 
 #include <cstdio>
-#include <cstdlib>
 
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -57,36 +56,9 @@ size_t planes_bytes(int N, int H, int W, int C) {
   return (size_t)planes_positions(N, H, W) * 16 * 2 * (C / 8);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) == cudaSuccess &&
-        qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(q);
-    (void)cudaGetLastError();
-  }
-  return fn;
-}
-
 // Positions per TMA box row.  The TMA engine pays a fixed cost per box row, so rows are as long as
 // the 256-element box limit allows: 128 positions x 16 B = 256 x uint64.  Tiles start on multiples of it.
-static int g_chunk = 0;
-int planes_chunk() {
-  if (g_chunk == 0) {
-    const char* e = getenv("SEEDRL_PLANES_CHUNK");
-    g_chunk = e ? atoi(e) : 128;
-    if (g_chunk != 16 && g_chunk != 32 && g_chunk != 64 && g_chunk != 128) g_chunk = 128;
-  }
-  return g_chunk;
-}
+constexpr int kPlanesChunk = 128;
 
 // 3-D view of a plane tensor starting `shift` positions in: {one chunk of CH positions as 2*CH
 // uint64, chunks, planes}; box = {2*CH, box_chunks, box_planes}.  Out-of-extent chunks read as zeros.
@@ -362,7 +334,7 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
   if (Lp + MT + 4 * g.PW >= (1LL << 31))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "convp: batch too large for 32-bit positions");
   const int L = MT + 2 * g.PW + 2;
-  const int CH = planes_chunk();
+  const int CH = kPlanesChunk;
   const int nch = (L + CH - 1) / CH;
   const size_t stage = (size_t)2 * (CIN / 8) * nch * CH * 16;
   const size_t fixed = (size_t)2 * 9 * CIN * COUT * 2 + COUT * 4 + 2 * kCpMaxStages * 8;
@@ -372,12 +344,7 @@ static int launch_convp(const PlaneConv& c, cudaStream_t st) {
   const size_t smem = nb * stage + fixed;
   CUtensorMap tm;
   SEEDRL_TRY(make_plane_map(&tm, c.in, Lp, 2 * (CIN / 8), 0, CH, nch, 2 * (CIN / 8)));
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(convp_kernel<CIN, COUT, NSUB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     227 * 1024));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<convp_kernel<CIN, COUT, NSUB>>(227 * 1024));
   ConvpArgs a;
   a.g = g; a.Lp = (int)Lp; a.nch = nch; a.chunk = CH; a.nb = nb;
   a.ntiles = (int)((Lp - g.PW - 1 + MT - 1) / MT);       // every storage position >= PW + 1 is written
@@ -583,7 +550,7 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
   const ConvGeom g = make_geom(N, H, W);
   const long long Lp = planes_positions(N, H, W);
   constexpr int G = CP / 8, GO = COUT / 8;
-  const int CH = planes_chunk() < KC ? planes_chunk() : KC;    // K chunks start on multiples of KC
+  const int CH = kPlanesChunk < KC ? kPlanesChunk : KC;    // K chunks start on multiples of KC
   if (KC % CH) return kPlanesTryNext;
   const int T = (2 * g.PW + kWpHaloRow - 1) / kWpHaloRow * kWpHaloRow;
   const size_t stage = (size_t)2 * G * (KC + kWpHaloRow) * 16 + (size_t)2 * GO * (KC + T) * 16;
@@ -596,14 +563,7 @@ static int launch_wgradp(int N, int H, int W, const void* x, const void* dy, flo
   SEEDRL_TRY(make_plane_map(&tm.x_halo, x, Lp, 2 * G, g.PW, kWpHaloRow, 1, 1));
   SEEDRL_TRY(make_plane_map(&tm.dy, dy, Lp, 2 * GO, 1, CH, KC / CH, 1));
   SEEDRL_TRY(make_plane_map(&tm.dy_halo, dy, Lp, 2 * GO, 1, kWpHaloRow, T / kWpHaloRow, 1));
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(wgradp_kernel<CP, COUT, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     227 * 1024));
-    attr = true;
-  }
-  static const bool dbg = getenv("SEEDRL_DEBUG_LAUNCH") != nullptr;
-  if (dbg) fprintf(stderr, "wgradp<%d,%d,%d> CH=%d T=%d nb=%d stage=%zu smem=%zu\n", CP, COUT, KC, CH, T, nb, stage, smem);
+  SEEDRL_CUDA(allow_smem<wgradp_kernel<CP, COUT, KC>>(227 * 1024));
   constexpr int NW = 9 * CP * COUT + COUT;
   WgradpArgs a;
   a.PW = g.PW; a.T = T; a.nb = nb; a.err = err; a.chunk = CH;
@@ -804,12 +764,6 @@ __global__ void poolp_bwd_kernel(ConvGeom gf, int Lpf, ConvGeom gp, int Lpp, int
     float4* dst = reinterpret_cast<float4*>(dx_nhwc + (size_t)pix * C + gq * 8);
     dst[0] = a; dst[1] = b;
   }
-}
-
-static void same_pad3s2(int in, int* out, int* before) {
-  *out = (in + 1) / 2;
-  const int total = (*out - 1) * 2 + 3 - in;
-  *before = total > 0 ? total / 2 : 0;
 }
 
 int poolp_forward(int N, int H, int W, int C, const float* x, void* out_raw, void* out_relu, uint8_t* idx,

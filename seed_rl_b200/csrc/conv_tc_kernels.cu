@@ -20,9 +20,6 @@
 // positions per 8-channel group) -> bias / ReLU-mask / residual -> fp32 NHWC.
 #include <cuda_bf16.h>
 
-#include <cstdio>
-#include <cstdlib>
-
 #include "kernels.h"
 #include "tc_common.cuh"
 
@@ -130,7 +127,7 @@ template <int CIN, int COUT, int IN_MODE, bool SPLIT, int MT>
 __global__ void __launch_bounds__(kTcThreads, CIN >= 32 ? kTcMinBlocks - 1 : kTcMinBlocks)
 conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restrict__ wq,
                   const float* __restrict__ bias, const float* __restrict__ mask,
-                  const float* __restrict__ res, float* __restrict__ out, int variant) {
+                  const float* __restrict__ res, float* __restrict__ out) {
   constexpr int CK = CIN < 16 ? 16 : CIN;   // channels the MMAs contract over
   constexpr int G = CIN < 8 ? 1 : CIN / 8;  // staged channel-group planes
   constexpr int NS = CK / 16;               // K slabs per tap
@@ -154,11 +151,10 @@ conv3x3_tc_kernel(ConvGeom g, const void* __restrict__ in_, const uint4* __restr
   if (tid < COUT) s_bias[tid] = bias ? __ldg(bias + tid) : 0.f;
   __syncthreads();
   const uint32_t a_base = smem_u32(s_a), b_base = smem_u32(s_b);
-  const uint32_t plane_b = CIN < 16 ? 0u : (uint32_t)LPl * 16u;   // K-group stride of A
-  const uint32_t a_lbo = (variant & 1) ? 128u : plane_b;
-  const uint32_t a_sbo = (variant & 1) ? plane_b : 128u;
-  const uint32_t b_lbo = (variant & 2) ? 128u : (uint32_t)(COUT / 8) * 128u;
-  const uint32_t b_sbo = (variant & 2) ? (uint32_t)(COUT / 8) * 128u : 128u;
+  // K-major descriptors (header comment): A's LBO is the plane stride (0 for the one IN_U8 plane), B's
+  // the COUT/8 core matrices of one K-group; SBO is one 128-byte core matrix for both
+  const uint32_t a_lbo = CIN < 16 ? 0u : (uint32_t)LPl * 16u;
+  constexpr uint32_t a_sbo = 128u, b_lbo = (uint32_t)(COUT / 8) * 128u, b_sbo = 128u;
   const float oscale = IN_MODE == IN_U8 ? (1.0f / 255.0f) : 1.0f;
 
   const int nchunks = (int)((g.Q + MT - 1) / MT);
@@ -279,8 +275,7 @@ constexpr int kTcTryNext = -12346;
 
 template <int CIN, int COUT, int IN_MODE, bool SPLIT, int MT>
 static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const float* bias,
-                     const float* mask, const float* res, float* out, int variant, int* err,
-                     cudaStream_t st) {
+                     const float* mask, const float* res, float* out, int* err, cudaStream_t st) {
   const ConvGeom g = make_geom(N, H, W);
   const int L = MT + 2 * g.PW + 2;
   constexpr int CK = CIN < 16 ? 16 : CIN;
@@ -291,12 +286,7 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
     if (MT > kTcM) return kTcTryNext;
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "conv3x3_tc: image too wide");
   }
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(conv3x3_tc_kernel<CIN, COUT, IN_MODE, SPLIT, MT>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<conv3x3_tc_kernel<CIN, COUT, IN_MODE, SPLIT, MT>>(200 * 1024));
   // resident CTAs per SM: registers (64K, allocated in units of 8 per thread), shared memory
   // (228 KB, 1 KB reserved per CTA), threads
   static int regs = 0, static_smem = 0;
@@ -318,12 +308,8 @@ static int launch_tc(int N, int H, int W, const void* in, const uint4* wq, const
   const long long nchunks = (g.Q + MT - 1) / MT;
   long long grid = (long long)kNumSMs * per_sm;
   if (grid > nchunks) grid = nchunks;
-  static const bool dbg = getenv("SEEDRL_DEBUG_LAUNCH") != nullptr;
-  if (dbg)
-    fprintf(stderr, "conv3x3_tc<%d,%d,%d,%d> MT=%d per_sm=%d grid=%lld smem=%zu\n", CIN, COUT, IN_MODE,
-            (int)SPLIT, MT, per_sm, grid, smem);
   conv3x3_tc_kernel<CIN, COUT, IN_MODE, SPLIT, MT><<<(unsigned)grid, kTcThreads, smem, st>>>(
-      g, in, wq, bias, mask, res, out, variant);
+      g, in, wq, bias, mask, res, out);
   count_launch(g_conv_cat, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
@@ -625,12 +611,7 @@ static int launch_wgrad_tc(int N, int H, int W, const void* x, const float* dy, 
   if (nb < 2 || (size_t)L * (CP / 8) > (size_t)wg_ix(CP / 8, KC) * kWgProducers) return kWgTryNext;
   size_t smem = nb * buf + tail;
   if (smem < (size_t)kWgProducers * 8 * 4) smem = (size_t)kWgProducers * 8 * 4;
-  static bool attr = false;
-  if (!attr) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_tc_kernel<CIN, COUT, IN_MODE, SPLIT, KC>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget));
-    attr = true;
-  }
+  SEEDRL_CUDA(allow_smem<conv3x3_wgrad_tc_kernel<CIN, COUT, IN_MODE, SPLIT, KC>>((int)budget));
   if (g.Q + KC + 4 * g.PW >= (1LL << 31))
     return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "wgrad_tc: batch too large for 32-bit positions");
   constexpr int NW = 9 * CIN * COUT + COUT;
@@ -756,9 +737,9 @@ int conv3x3_tc_pack_weights(int cin, int cout, int flip, int split, const float*
 
 int conv3x3_tc_forward(int cin, int cout, int in_mode, int split, int N, int H, int W, const void* in,
                        const void* wq, const float* bias, const float* mask, const float* res,
-                       float* out, int variant, int* err, cudaStream_t st) {
+                       float* out, int* err, cudaStream_t st) {
   const uint4* q = reinterpret_cast<const uint4*>(wq);
-#define SEEDRL_TC_ARGS N, H, W, in, q, bias, mask, res, out, variant, err, st
+#define SEEDRL_TC_ARGS N, H, W, in, q, bias, mask, res, out, err, st
 #define SEEDRL_TC_CASE(CI, CO_, MODE)                                                               \
   if (cin == CI && cout == CO_ && in_mode == MODE) {                                                \
     int rc = kTcTryNext;                                                                            \

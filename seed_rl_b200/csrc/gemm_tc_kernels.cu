@@ -17,8 +17,6 @@
 // every operand is staged as hi and lo planes and each K-step issues hi*hi + lo*hi + hi*lo.
 // Epilogue: accumulators -> fp32 tile in shared memory -> bias / relu / mask / accumulate -> C, or
 // -> the split-K workspace, reduced in slice order by gemm_tc_reduce_kernel (deterministic).
-#include <cstdlib>
-
 #include "kernels.h"
 #include "tc_common.cuh"
 
@@ -27,8 +25,7 @@ namespace seedrl {
 constexpr int kGtThreads = 256;
 constexpr int kGtBM = 128;
 constexpr int kGtMaxBN = 128;   // tile width cap: a warpgroup holds 64 x 128 fp32 accumulators = 64 registers/thread
-// K elements per staged block = template parameter BK (64, 32 or 16): a smaller block shrinks the
-// stage so that several CTAs fit an SM and overlap each other's load / convert / MMA / epilogue phases
+constexpr int kGtBK = 32;       // K elements per staged block
 
 struct GemmTcParams {
   int M, N, K;
@@ -37,7 +34,7 @@ struct GemmTcParams {
   float* C; int ldc;            // final output (splits == 1) ...
   float* ws;                    // ... or split-K partials [splits][M][N]
   int BN;                       // tile width: multiple of 16, <= kGtMaxBN
-  int kblocks_per_split;        // K blocks (of 64) per blockIdx.z
+  int kblocks_per_split;        // K blocks (of kGtBK) per blockIdx.z
   int vecA, vecB;               // 16-byte aligned rows: float4 loads
   GemmEpi e;
   int* error_flag;
@@ -123,7 +120,7 @@ __device__ __forceinline__ void gemm_tc_mma(int bn, float* acc, uint64_t a, uint
   }
 }
 
-template <bool TA, bool TB, bool SPLIT, int kGtBK, bool GATHER>
+template <bool TA, bool TB, bool SPLIT, bool GATHER>
 __global__ void __launch_bounds__(kGtThreads)
 gemm_tc_kernel(const GemmTcParams p) {
   constexpr int S = SPLIT ? 2 : 1;
@@ -341,15 +338,11 @@ gemm_tc_reduce_wide_kernel(int M, int N, int splits, const float* __restrict__ w
   }
 }
 
-static int norm_bk(int bk) { return bk == 64 ? 64 : (bk == 16 ? 16 : 32); }
-static int g_gemm_bk = norm_bk(getenv("SEEDRL_GEMM_BK") ? atoi(getenv("SEEDRL_GEMM_BK")) : 32);
-void gemm_tc_set_bk(int bk) { g_gemm_bk = norm_bk(bk); }
-
 bool gemm_tc_supported(int M, int N, int K) { return M >= 64 && N >= 16 && K >= 32; }
 
 size_t gemm_tc_workspace_bytes() { return (size_t)48 << 20; }
 
-static int g_gemm_gather = getenv("SEEDRL_GEMM_GATHER") ? atoi(getenv("SEEDRL_GEMM_GATHER")) : 1;
+static int g_gemm_gather = 1;
 void gemm_tc_set_gather(int on) { g_gemm_gather = on; }
 bool gemm_tc_gather_enabled() { return g_gemm_gather != 0; }
 
@@ -377,12 +370,11 @@ int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, in
   p.M = M; p.N = N; p.K = K; p.A = A; p.lda = lda; p.B = B; p.ldb = ldb; p.C = C; p.ldc = ldc;
   p.e = e; p.error_flag = err;
   const int n16 = ((N + 15) / 16) * 16;
-  const int BK = g_gemm_bk;
   int bn = kGtMaxBN;
   if (bn > n16) bn = n16;
   // narrower tiles until the grid can cover the SMs (with split-K below)
-  const int nkb_all = ceil_div(K, BK);
-  const int kb256 = 256 / BK;                           // K-blocks per 256 elements of K
+  const int nkb_all = ceil_div(K, kGtBK);
+  const int kb256 = 256 / kGtBK;                        // K-blocks per 256 elements of K
   while (bn > 64 && ceil_div(M, kGtBM) * ceil_div(N, bn) * (nkb_all >= kb256 ? nkb_all / (kb256 / 2) : 1) < kNumSMs)
     bn >>= 1;
   p.BN = ((bn + 15) / 16) * 16;
@@ -390,44 +382,32 @@ int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, in
   p.vecA = al16(A) && (lda & 3) == 0;
   p.vecB = al16(B) && (ldb & 3) == 0;
   const int tiles = ceil_div(M, kGtBM) * ceil_div(N, p.BN);
-  const int nkb = ceil_div(K, BK);
+  const int nkb = ceil_div(K, kGtBK);
   // split-K until the grid covers the SMs, keeping >= 128 elements of K per slice and the
   // partials inside the workspace
   int splits = 1;
-  static const int waves = getenv("SEEDRL_GEMM_WAVES") ? atoi(getenv("SEEDRL_GEMM_WAVES")) : 1;   // tuning knob
-  while (tiles * splits < waves * kNumSMs && nkb / (splits * 2) >= 128 / BK &&
+  while (tiles * splits < kNumSMs && nkb / (splits * 2) >= 128 / kGtBK &&
          (size_t)(splits * 2) * M * N * sizeof(float) <= ws_bytes && ws)
     splits *= 2;
   p.kblocks_per_split = ceil_div(nkb, splits);
   splits = ceil_div(nkb, p.kblocks_per_split);
   p.ws = splits > 1 ? ws : nullptr;
   const int S = split ? 2 : 1;
-  const size_t a_un = ta ? (size_t)(kGtBM / 8) * (BK + 1) : (size_t)(BK / 8) * (kGtBM + 1);
-  const size_t b_un = tb ? (size_t)(BK / 8) * (p.BN + 1) : (size_t)(p.BN / 8) * (BK + 1);
+  const size_t a_un = ta ? (size_t)(kGtBM / 8) * (kGtBK + 1) : (size_t)(kGtBK / 8) * (kGtBM + 1);
+  const size_t b_un = tb ? (size_t)(kGtBK / 8) * (p.BN + 1) : (size_t)(p.BN / 8) * (kGtBK + 1);
   size_t smem = (size_t)2 * S * (a_un + b_un) * 16;
   const size_t epi = (size_t)kGtBM * (p.BN + 4) * 4;      // the epilogue's fp32 tile aliases the stages
   if (smem < epi) smem = epi;
   dim3 grid(ceil_div(N, p.BN), ceil_div(M, kGtBM), splits);
-#define SEEDRL_GT_LAUNCH2(TA_, TB_, SP_, BK_, G_)                                               \
+#define SEEDRL_GT_LAUNCH2(TA_, TB_, SP_, G_)                                                    \
   do {                                                                                          \
-    static bool attr = false;                                                                   \
-    if (!attr) {                                                                                \
-      SEEDRL_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<TA_, TB_, SP_, BK_, G_>,                  \
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-      attr = true;                                                                              \
-    }                                                                                           \
-    gemm_tc_kernel<TA_, TB_, SP_, BK_, G_><<<grid, kGtThreads, smem, st>>>(p);                  \
-  } while (0)
-#define SEEDRL_GT_LAUNCH1(TA_, TB_, SP_, BK_)                                                   \
-  do {                                                                                          \
-    if (cg && !(TB_)) SEEDRL_GT_LAUNCH2(TA_, false, SP_, BK_, true);                            \
-    else SEEDRL_GT_LAUNCH2(TA_, TB_, SP_, BK_, false);                                          \
+    SEEDRL_CUDA(allow_smem<gemm_tc_kernel<TA_, TB_, SP_, G_>>(200 * 1024));                     \
+    gemm_tc_kernel<TA_, TB_, SP_, G_><<<grid, kGtThreads, smem, st>>>(p);                       \
   } while (0)
 #define SEEDRL_GT_LAUNCH(TA_, TB_, SP_)                                                         \
   do {                                                                                          \
-    if (BK == 32) SEEDRL_GT_LAUNCH1(TA_, TB_, SP_, 32);                                         \
-    else if (BK == 16) SEEDRL_GT_LAUNCH1(TA_, TB_, SP_, 16);                                    \
-    else SEEDRL_GT_LAUNCH1(TA_, TB_, SP_, 64);                                                  \
+    if (cg && !(TB_)) SEEDRL_GT_LAUNCH2(TA_, false, SP_, true);                                 \
+    else SEEDRL_GT_LAUNCH2(TA_, TB_, SP_, false);                                               \
   } while (0)
   if (split) {
     if (!ta && !tb) SEEDRL_GT_LAUNCH(false, false, true);
@@ -441,7 +421,6 @@ int gemm_tc(bool ta, bool tb, int split, int M, int N, int K, const float* A, in
     else SEEDRL_GT_LAUNCH(true, true, false);
   }
 #undef SEEDRL_GT_LAUNCH
-#undef SEEDRL_GT_LAUNCH1
 #undef SEEDRL_GT_LAUNCH2
   count_launch(PC_GEMM, st);
   SEEDRL_CHECK_LAUNCH();

@@ -86,7 +86,7 @@ int conv3x3_tc_pack_weights_batch(const PackTable& t, int split, cudaStream_t st
 void conv3x3_tc_set_tile(int mt);           // upper bound: 512 (default), 256 or 128
 int conv3x3_tc_forward(int cin, int cout, int in_mode, int split, int N, int H, int W, const void* in,
                        const void* wq, const float* bias, const float* mask, const float* res,
-                       float* out, int variant, int* err, cudaStream_t st);
+                       float* out, int* err, cudaStream_t st);
 
 // conv_planes.cu ("planes" path: activations stored in HBM as bf16 hi/lo channel-group planes of
 // the padded tall image = the wgmma operand format; TMA-fed, warp-specialised kernels)
@@ -140,6 +140,13 @@ int wgrad_reduce(int nparts, int nw, int nb, const float* partial, float* dw, fl
 int conv3x3_wgrad(int cin, int cout, int in_mode, int N, int H, int W, const void* x,
                   const float* dy, float* dw, float* db, float* partial, size_t partial_bytes,
                   cudaStream_t st);
+// TF 'SAME' padding of the 3x3 / stride 2 max-pool along one axis: `in` pixels -> *out pooled pixels,
+// *before padding pixels ahead of the first
+inline void same_pad3s2(int in, int* out, int* before) {
+  *out = (in + 1) / 2;
+  const int total = (*out - 1) * 2 + 3 - in;
+  *before = total > 0 ? total / 2 : 0;
+}
 int maxpool3s2_forward(int N, int H, int W, int C, const float* x, float* y, uint8_t* idx,
                        cudaStream_t st);
 int maxpool3s2_backward(int N, int H, int W, int C, const float* dy, const uint8_t* idx, float* dx,
@@ -177,7 +184,6 @@ int colsum(int M, int N, const float* X, int ld, float* out, cudaStream_t st, fl
 // gemm_tc_kernels.cu (wgmma): same contract as sgemm; split = bf16x3 operands; `ws` holds
 // split-K partials (gemm_tc_workspace_bytes()); *err is set if a bounded mbarrier wait expires.
 bool gemm_tc_supported(int M, int N, int K);
-void gemm_tc_set_bk(int bk);                 // K elements per staged block: 64 or 32 (tuning knob)
 size_t gemm_tc_workspace_bytes();
 // op(A) = the im2col matrix of an NHWC tensor x[N][H][W][C] for a K x K / stride S 'valid' convolution
 // (rows = output positions (n, ho, wo), columns = (kh, kw, c)), gathered while the GEMM stages its A

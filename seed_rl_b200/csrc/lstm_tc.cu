@@ -367,11 +367,7 @@ static int launch_lstm_tc(bool bwd, LstmTcArgs a, cudaStream_t st) {
   a.nug = H / kLtNU;
   if (nbt > 64) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "lstm (tc3): batch too large");
   const void* fn = bwd ? (const void*)lstm_tc_bwd_kernel<H> : (const void*)lstm_tc_fwd_kernel<H>;
-  static bool attr[2] = {false, false};
-  if (!attr[bwd ? 1 : 0]) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[bwd ? 1 : 0] = true;
-  }
+  SEEDRL_CUDA(bwd ? allow_smem<lstm_tc_bwd_kernel<H>>((int)smem) : allow_smem<lstm_tc_fwd_kernel<H>>((int)smem));
   SEEDRL_CUDA(cudaMemsetAsync(a.counter, 0, 64 * sizeof(unsigned int), st));
   const int grid = nbt * a.nug;
   void* args[] = {&a};

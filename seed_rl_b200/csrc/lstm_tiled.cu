@@ -287,11 +287,7 @@ static int launch_lstm2(bool bwd, Lstm2Args a, cudaStream_t st) {
   a.nug = H / kTlNU;
   if (a.nbt > 64) return set_error(SEEDRL_ERR_INVALID_ARGUMENT, "lstm (tiled): batch too large");
   const void* fn = bwd ? (const void*)lstm2_bwd_kernel<H> : (const void*)lstm2_fwd_kernel<H>;
-  static bool attr[2] = {false, false};
-  if (!attr[bwd ? 1 : 0]) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    attr[bwd ? 1 : 0] = true;
-  }
+  SEEDRL_CUDA(bwd ? allow_smem<lstm2_bwd_kernel<H>>(220 * 1024) : allow_smem<lstm2_fwd_kernel<H>>(220 * 1024));
   SEEDRL_CUDA(cudaMemsetAsync(a.counter, 0, 64 * sizeof(unsigned int), st));
   const int grid = a.nbt * a.nug;
   void* args[] = {&a};

@@ -169,12 +169,11 @@ static const float* flat_features(const seedrl_net* n, const Plan& pl, void* ws)
   return W<float>(ws, n->cfg.net == SEEDRL_NET_DEEP ? pl.st.back().o1.raw : pl.sh_a2);
 }
 
-// The deep net's first layer (stack 0's conv + max-pool on the uint8 frames) runs one of four kernel paths.
+// The deep net's first layer (stack 0's conv + max-pool on the uint8 frames) runs one of three kernel paths.
 // The forward and the backward pick theirs independently: the fused kernels' limits differ (conv_first.cu).
 enum FirstPath {
   kFirstFused,     // conv0pool_forward / first_wgrad_pooled (plane tensors): no full-resolution tensor
   kFirstStaged,    // 4-channel frames: wgmma conv on staged uint8 tiles + max-pool, wgmma weight gradient
-  kFirstSimt4,     // the same on the fp32 SIMT kernels
   kFirstGeneric,   // SIMT channel-generic conv3x3_u8_* (1 to 16 channels) + max-pool
 };
 
@@ -201,7 +200,7 @@ static int first_layer(const seedrl_net* n, bool backward, FirstPath* path) {
                      g_first_dense || backward
                          ? "the dense first-layer path takes 3- or 4-channel frames; switch it off for these frames"
                          : "conv mode 3: the fused first layer takes frames up to 107 pixels wide");
-  *path = fused ? kFirstFused : generic_first(n) ? kFirstGeneric : n->conv_mode >= 1 ? kFirstStaged : kFirstSimt4;
+  *path = fused ? kFirstFused : n->conv_mode >= 1 && !generic_first(n) ? kFirstStaged : kFirstGeneric;
   return SEEDRL_OK;
 }
 
@@ -218,7 +217,7 @@ struct Call {
   GemmExec ex;
   PackTable packed;
   WgradBatch wb;
-  FirstPath first = kFirstSimt4;     // deep net: first_layer() of this call's direction
+  FirstPath first = kFirstGeneric;   // deep net: first_layer() of this call's direction
   int w0_index = -1;
   const float* w0_pad = nullptr;
   float* dw0_pad = nullptr;
@@ -322,7 +321,7 @@ static int run_conv(const Call& c, const ConvLayer& l, int H, int Wd, int in_mod
   if (c.n->conv_mode >= 1 && conv3x3_tc_supported(cin, cout, in_mode)) {
     const int split = c.n->conv_mode >= 2;
     SEEDRL_TRY(packed_weights(c, cin, cout, w, flip, split, &wq));
-    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, x, wq, bias, m, r, c.at<float>(out.raw), 0,
+    return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, Wd, x, wq, bias, m, r, c.at<float>(out.raw),
                               c.ex.err, st);
   }
   if (flip) {
@@ -415,10 +414,8 @@ static int first_forward(const Call& c, const uint8_t* obs) {
                              c.at<uint8_t>(b.idx), c.ex.err, st);
   if (c.first == kFirstStaged) {
     SEEDRL_TRY(packed_weights(c, k.cin, k.c, w, 0, split, &wq));
-    SEEDRL_TRY(conv3x3_tc_forward(k.cin, k.c, IN_U8, split, N, k.hin, k.win, obs, wq, bias, nullptr, nullptr, a0, 0,
+    SEEDRL_TRY(conv3x3_tc_forward(k.cin, k.c, IN_U8, split, N, k.hin, k.win, obs, wq, bias, nullptr, nullptr, a0,
                                   c.ex.err, st));
-  } else if (c.first == kFirstSimt4) {
-    SEEDRL_TRY(conv3x3_forward(k.cin, k.c, IN_U8, N, k.hin, k.win, obs, w, bias, nullptr, nullptr, a0, st));
   } else {
     SEEDRL_TRY(conv3x3_u8_forward(first_c(n), N, k.hin, k.win, obs, w, bias, a0, st));
   }
@@ -442,8 +439,6 @@ static int first_backward(Call& c, const uint8_t* obs) {
   if (c.first == kFirstStaged)
     return conv3x3_wgrad_tc(k.cin, k.c, IN_U8, n->conv_mode >= 2, N, k.hin, k.win, obs, gF, dw, db, partial, pbytes,
                             c.ex.err, &c.wb, st);
-  if (c.first == kFirstSimt4)
-    return conv3x3_wgrad(k.cin, k.c, IN_U8, N, k.hin, k.win, obs, gF, dw, db, partial, pbytes, st);
   return conv3x3_u8_wgrad(first_c(n), N, k.hin, k.win, obs, gF, dw, db, partial, pbytes, st);
 }
 
@@ -912,10 +907,6 @@ extern "C" int seedrl_debug_set_first_layer_dense(int on) {
   g_first_dense = on ? 1 : 0;
   return SEEDRL_OK;
 }
-extern "C" int seedrl_debug_set_gemm_bk(int bk) {
-  gemm_tc_set_bk(bk);
-  return SEEDRL_OK;
-}
 // Bench knob: output positions per tile of the tensor-core forward / data-gradient kernel
 // (the largest of 512/256/128 not above `mt` that keeps >= 2 CTAs per SM is used; default 512).
 extern "C" int seedrl_debug_set_conv_tile(int mt) {
@@ -926,17 +917,18 @@ extern "C" int seedrl_debug_set_conv_tile(int mt) {
 
 // wgmma conv test hook: packs fp32 HWIO weights (optionally flipped/transposed for the
 // data-gradient) into `wq_scratch` (>= 2*9*max(cin,16)*cout*2 bytes) and runs the tensor-core conv.
-// `variant` bit0/bit1 swap LBO/SBO of the A/B descriptors (bring-up aid); *error_flag is
-// set to 1 by the kernel if its bounded mbarrier wait expires.
+// `variant` must be 0 (the argument is kept for ABI compatibility); the kernel has no bounded waits, so
+// *error_flag is left unchanged.
 extern "C" int seedrl_debug_conv3x3_tc(int cin, int cout, int in_mode, int split, int N, int H, int W,
                                        const void* in, const float* w, const float* bias,
                                        const float* mask, const float* res, float* out, int flip,
                                        int variant, void* wq_scratch, int* error_flag,
                                        seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(variant == 0, "variant must be 0");
   SEEDRL_CHECK_ARG(conv3x3_tc_supported(cin, cout, in_mode), "unsupported (cin,cout,mode)");
   SEEDRL_TRY(conv3x3_tc_pack_weights(cin, cout, flip, split, w, wq_scratch, (cudaStream_t)stream));
   return conv3x3_tc_forward(cin, cout, in_mode, split, N, H, W, in, wq_scratch, bias, mask, res, out,
-                            variant, error_flag, (cudaStream_t)stream);
+                            error_flag, (cudaStream_t)stream);
 }
 
 // ---- plane-tensor path test hooks (conv_planes.cu) ---------------------------------------------

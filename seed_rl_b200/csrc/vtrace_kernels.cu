@@ -987,33 +987,15 @@ static int num_sms() {
   return n;
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) == cudaSuccess &&
-        qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(q);
-    (void)cudaGetLastError();
-  }
-  return fn;
-}
 // [T1, B*A] fp32 matrix, box = T rows x BB*A floats (one tile), dense in shared memory.
 static bool make_tile_map(CUtensorMap* tm, const float* base, int T1, int T, int B, int A, int BB) {
   const cuuint64_t gdim[2] = {(cuuint64_t)B * A, (cuuint64_t)T1};
   const cuuint64_t gstr[1] = {(cuuint64_t)B * A * sizeof(float)};
   const cuuint32_t box[2] = {(cuuint32_t)(BB * A), (cuuint32_t)T};
   const cuuint32_t estr[2] = {1, 1};
-  return encode_tiled()(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstr, box,
-                        estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return encode_tiled_fn()(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstr, box,
+                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // The streaming kernel applies when every tile is full, the TMA box is legal (inner extent
@@ -1023,7 +1005,7 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
   const int T = p.T, B = p.B, A = p.A;
   auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   if (!aligned16(p.ll) || !aligned16(p.bl) || !aligned16(p.dlogits)) return 0;
-  if (T > 256 || (((size_t)B * A) & 3) != 0 || !encode_tiled()) return 0;
+  if (T > 256 || (((size_t)B * A) & 3) != 0 || !encode_tiled_fn()) return 0;
   // two passes: first the largest BB that leaves room for two CTAs per SM (one CTA's
   // barriers and scan then hide behind the other's phases), else the largest that fits
   for (int pass = 0; pass < 2; ++pass)
@@ -1049,13 +1031,8 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
 template <int AS>
 static cudaError_t launch_stream(const LossParams& p, int ntiles, int threads, size_t smem, cudaStream_t stream,
                                  const CUtensorMap& tm_bl, const CUtensorMap& tm_ll, const CUtensorMap& tm_dl) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(vtrace_loss_stream_kernel<AS>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStreamSmemMax);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
+  const cudaError_t e = allow_smem<vtrace_loss_stream_kernel<AS>>((int)kStreamSmemMax);
+  if (e != cudaSuccess) return e;
   // persistent CTAs: as many per SM as shared memory and threads allow (small T: several,
   // so one CTA's barriers and scan hide behind another's copies)
   int per_sm = (int)((size_t)(228 * 1024) / (smem + 2048 + 1024));   // 228 KB/SM, 1 KB/CTA reserved
@@ -1182,12 +1159,7 @@ extern "C" int seedrl_vtrace_loss_fwd_bwd(
   p.d_ecp = d_entropy_cost_param; p.vs_out = vs_out; p.pg_out = pg_advantages_out;
   p.ticket = reinterpret_cast<unsigned int*>(scratch);
   p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
-  static bool attr_set = false;
-  if (!attr_set) {
-    SEEDRL_CUDA(cudaFuncSetAttribute(vtrace_loss_kernel,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
-  }
+  SEEDRL_CUDA(allow_smem<vtrace_loss_kernel>(200 * 1024));
   int threads = 0;
   p.BB = g_loss_stream_enabled ? pick_stream(p, g_loss_stream_enabled, &threads, &smem) : 0;
   alignas(64) CUtensorMap tm_bl, tm_ll, tm_dl;

@@ -36,6 +36,15 @@ def test_argument_errors_are_reported_not_crashed():
   assert b'null pointer' in L.seedrl_last_error()
   with pytest.raises(_lib.SeedrlError):
     _lib.check(rc)
+  # the wgmma conv takes only the documented descriptor layout: any other `variant` is refused before
+  # the weights are packed or the conv launched
+  n0 = _lib.launch_count()
+  for variant in (1, 2, 3):
+    rc = L.seedrl_debug_conv3x3_tc(16, 16, 1, 0, 1, 8, 8, None, None, None, None, None, None, 0, variant,
+                                   None, None, None)
+    assert rc == 3
+    assert b'variant' in L.seedrl_last_error()
+  assert _lib.launch_count() == n0
 
 
 def test_net_param_table_matches_reference_variable_count():

@@ -7,9 +7,6 @@ from seed_rl_b200 import _lib
 
 L = _lib.lib()
 split = int(sys.argv[1]) if len(sys.argv) > 1 else 0
-if len(sys.argv) > 2:
-  _lib.check(L.seedrl_debug_set_gemm_bk(int(sys.argv[2])))
-  print('BK =', sys.argv[2])
 R = 1344
 SHAPES = [  # name, ta, tb, M, N, K, lda, ldb
     ('dense fwd', 0, 0, R, 256, 3872, 3872, 256), ('lstm proj', 0, 0, R, 1024, 275, 275, 1024),

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Single-kernel timings of the plane-tensor conv path (csrc/conv_planes.cu) at the learner's
-layer shapes: python tools/planes_bench.py  [SEEDRL_PLANES_CHUNK=16|32|64|128 in the env].
+layer shapes: python tools/planes_bench.py
 
 Every convp_kernel configuration the default ImpalaDeep step (net.cu torso_forward /
 torso_backward in conv mode tc3p) launches is timed with its real epilogue: shape x {bias, ReLU mask,
@@ -68,8 +68,7 @@ assert sum(c[-1] for c in CONFIGS) == 28
 smi = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
                      capture_output=True, text=True).stdout.strip().splitlines()
 out = {'device': torch.cuda.get_device_name(), 'nvidia_smi': smi[torch.cuda.current_device()] if smi else None,
-       'chunk': os.environ.get('SEEDRL_PLANES_CHUNK', 'default'), 'frames': N,
-       'peak_GBps_datasheet': PEAK_GBPS, 'convp': {}}
+       'frames': N, 'peak_GBps_datasheet': PEAK_GBPS, 'convp': {}}
 err = torch.zeros(1, dtype=torch.int32, device='cuda')
 step_ms = step_bytes = 0.0
 for (name, ci, co, H, flags, count) in CONFIGS:

@@ -43,7 +43,7 @@ def one(i):
     w = (rng.normal(size=(3, 3, cin, cout)) * 0.2).astype(np.float32)
     b = rng.normal(size=(cout,)).astype(np.float32)
     want = _ref(x, w, b, mode).numpy()
-  got, err = _run(cin, cout, mode, N, H, W, x, w, b, None, None, flip, 0)
+  got, err = _run(cin, cout, mode, N, H, W, x, w, b, None, None, flip)
   print('CASE', i, CASES[i], 'relerr %.4g' % _relerr(got, want), 'timeout_flag', err, 'nan',
         int(np.isnan(got).sum()), flush=True)
 
