@@ -103,6 +103,7 @@ enum {
   SEEDRL_LT_KL = 4, SEEDRL_LT_ENTROPY_ADJ = 5, SEEDRL_LT_V_MEAN = 6,
   SEEDRL_LT_V_L2_ERROR = 7, SEEDRL_LT_MEAN_ENTROPY = 8, SEEDRL_LT_ENTROPY_COST = 9,
   SEEDRL_LT_MEAN_KL = 10, SEEDRL_LT_MAX_ACTION_ABS = 11,
+  SEEDRL_LT_POPART_MEAN = 12, SEEDRL_LT_POPART_STD = 13,   /* PopArt only (0 otherwise) */
   SEEDRL_LOSS_TERMS = 16
 };
 
@@ -129,6 +130,43 @@ int seedrl_vtrace_loss_fwd_bwd(
     float* loss_terms, float* dlogits, float* dbaseline,
     float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
     void* scratch, seedrl_stream_t stream);
+
+/* PopArt value normalisation (opt-in; reference agents/policy_gradient/modules/popart.py with
+ * running_statistics.py EMAMeanStd, composed as in generalized_onpolicy_loss.py:94-133,169-199).
+ * A learner step is
+ *   seedrl_vtrace_popart_loss_fwd -> [SUM all-reduce of moment_sums across replicas] ->
+ *   seedrl_vtrace_popart_update.
+ * State: popart_moments = (mu1, mu2), the EMA moments (not trained), and popart_compensation =
+ * (sigma, mu), trained; with m = mu1, s = clip(sqrt(mu2 - mu1^2), 1e-6, 1e6), the value of a
+ * baseline output V in return units is u = s (sigma V + mu) + m.
+ *
+ * seedrl_vtrace_popart_loss_fwd: seedrl_vtrace_loss_fwd_bwd on u (values = u[:-1], bootstrap =
+ * u[-1]), with the policy gradient taken on pg_advantages / s.  Writes every loss term but the value
+ * loss (V, V_L2_ERROR, TOTAL: written by the update), dlogits, d_entropy_cost_param, row T1-1 of
+ * dbaseline (zero), td_out [T1-1,B] = (vs - u) / s, and moment_sums[2] = (sum vs, sum vs^2) over
+ * the T1-1 x B rows.  vs_out / pg_advantages_out (optional) are in return units.  Same scratch.
+ *
+ * seedrl_vtrace_popart_update: with the moment sums of all `world` replicas (equal batches), the
+ * EMA update mu_k' = mu_k + beta (mean - mu_k), the compensation update sigma+ = (s/s') sigma,
+ * mu+ = (m - m' + s mu) / s' (written to popart_moments / popart_compensation in place), and with
+ * e = (vs - m)/s - (sigma+ V + mu+): dbaseline rows [0, T1-1) = -baseline_cost e sigma+ / N,
+ * d_popart_compensation = -baseline_cost (mean(e V), mean(e)), loss_terms V, V_L2_ERROR, TOTAL,
+ * POPART_MEAN = m', POPART_STD = s'.  `scratch` is the one seedrl_vtrace_popart_loss_fwd used. */
+int seedrl_vtrace_popart_loss_fwd(
+    int T1, int B, int A,
+    const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions,
+    const float* rewards, const uint8_t* done,
+    const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline,
+    float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
+    float* td_out, float* moment_sums, void* scratch, seedrl_stream_t stream);
+int seedrl_vtrace_popart_update(
+    int T1, int B, int world, float beta, float baseline_cost,
+    const float* learner_baseline, const float* td, const float* moment_sums,
+    float* popart_moments, float* popart_compensation, float* dbaseline,
+    float* d_popart_compensation, float* loss_terms, void* scratch, seedrl_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * (a4) Optimizer apply.  Replaces optimizer.apply_gradients

@@ -65,7 +65,7 @@ class NetConfig(ctypes.Structure):
 NET_DEEP, NET_SHALLOW = 0, 1
 LOSS_TERMS = 16
 LT = dict(total=0, policy=1, V=2, entropy=3, kl=4, entropy_adj=5, v_mean=6, v_l2_error=7,
-          mean_entropy=8, entropy_cost=9, mean_kl=10, max_action_abs=11)
+          mean_entropy=8, entropy_cost=9, mean_kl=10, max_action_abs=11, popart_mean=12, popart_std=13)
 
 # name -> (restype, argtypes); every symbol of include/seedrl_b200.h
 SIGNATURES = {
@@ -82,6 +82,11 @@ SIGNATURES = {
     'seedrl_vtrace_loss_fwd_bwd':
         (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, ctypes.POINTER(LossConfig), P,
                  P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_popart_loss_fwd':
+        (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, ctypes.POINTER(LossConfig), P, P, P,
+                 P, P, P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_popart_update':
+        (c_int, [c_int, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P, P, P, P]),
     'seedrl_adam_apply':
         (c_int, [c_size_t, P, P, P, P, c_float, c_float, c_float, c_float, c_float, c_i64,
                  c_float, c_float, P]),

@@ -52,24 +52,31 @@ common_flags.define_once(flags.DEFINE_integer, 'log_episode_frequency', 1, 'We a
 common_flags.define_once(flags.DEFINE_enum, 'grad_reduce', 'sum', ['sum', 'mean'],
                   'Cross-replica gradient reduction. The reference SUMs '
                   '(tests/utils_test.py:609-650).')
+common_flags.define_once(flags.DEFINE_bool, 'popart', False,
+                         'Normalise value targets and advantages with PopArt (popart.py, EMAMeanStd '
+                         'statistics, compensation on).')
+common_flags.define_once(flags.DEFINE_float, 'popart_beta', 1e-2,
+                         'Step size of the PopArt moment EMA (EMAMeanStd beta).')
 
 FLAGS = flags.FLAGS
 
 LossSettings = collections.namedtuple(
     'LossSettings',
     'discounting lambda_ baseline_cost entropy_cost kl_cost max_abs_reward '
-    'target_entropy entropy_cost_adjustment_speed')
+    'target_entropy entropy_cost_adjustment_speed popart popart_beta', defaults=(False, 1e-2))
 
 
 def loss_settings_from_flags():
   return LossSettings(FLAGS.discounting, FLAGS.lambda_, FLAGS.baseline_cost,
                       FLAGS.entropy_cost, FLAGS.kl_cost, FLAGS.max_abs_reward,
-                      FLAGS.target_entropy, FLAGS.entropy_cost_adjustment_speed)
+                      FLAGS.target_entropy, FLAGS.entropy_cost_adjustment_speed, FLAGS.popart,
+                      FLAGS.popart_beta)
 
 
 def default_loss_settings(**kw):
   d = dict(discounting=.99, lambda_=1., baseline_cost=.5, entropy_cost=0.00025, kl_cost=0.,
-           max_abs_reward=0., target_entropy=None, entropy_cost_adjustment_speed=10.)
+           max_abs_reward=0., target_entropy=None, entropy_cost_adjustment_speed=10., popart=False,
+           popart_beta=1e-2)
   d.update(kw)
   return LossSettings(**d)
 
@@ -89,6 +96,7 @@ _LOG_NAMES = [  # learner.py:138-157
     ('policy/max_action_abs(before_tanh)', 'max_action_abs'),
     ('policy/entropy', 'mean_entropy'), ('policy/entropy_cost', 'entropy_cost'),
     ('policy/kl(old|new)', 'mean_kl')]
+_POPART_LOG_NAMES = [('PopArt/mean', 'popart_mean'), ('PopArt/std', 'popart_std')]   # popart.py:175-176
 
 _scratch_cache = {}
 
@@ -101,11 +109,8 @@ def _loss_scratch(T1, B, A, device):
   return _scratch_cache[key]
 
 
-def vtrace_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits,
-                        actions, rewards, done, entropy_cost_param, want_vtrace=False):
-  """The fused kernel of compute_loss (learner.py:82-157) + its gradient.  All inputs
-  have T+1 rows.  Returns dict(loss_terms[16], dlogits, dbaseline, d_entropy_cost_param,
-  vs, pg_advantages)."""
+def _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions, rewards, done,
+                 entropy_cost_param):
   f32 = torch.float32
   ll = _lib.require_cuda(learner_logits, f32, 'learner_logits')
   lb = _lib.require_cuda(learner_baseline, f32, 'learner_baseline')
@@ -121,44 +126,119 @@ def vtrace_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_lo
                      (act, (T1, B), 'actions'), (rew, (T1, B), 'rewards'), (dn, (T1, B), 'done')):
     if tuple(t.shape) != shp:
       raise ValueError('%s has shape %s, expected %s' % (nm, tuple(t.shape), shp))
-  dev = ll.device
-  cfg = _lib.LossConfig(
+  return ll, lb, bl, act, rew, dn, ecp
+
+
+def _loss_config(settings):
+  return _lib.LossConfig(
       settings.discounting, settings.lambda_, settings.baseline_cost, settings.kl_cost,
       settings.max_abs_reward or 0.0, 1.0, 1.0,     # compute_loss uses vtrace's default clips
       settings.target_entropy or 0.0, 1 if settings.target_entropy else 0,
       settings.entropy_cost_adjustment_speed)
-  out = dict(
+
+
+def _loss_outputs(ll, lb, want_vtrace):
+  f32 = torch.float32
+  T1, B = int(ll.shape[0]), int(ll.shape[1])
+  dev = ll.device
+  return dict(
       loss_terms=torch.empty(_lib.LOSS_TERMS, dtype=f32, device=dev),
       dlogits=torch.empty_like(ll), dbaseline=torch.empty_like(lb),
       d_entropy_cost_param=torch.empty((), dtype=f32, device=dev),
       vs=torch.empty([T1 - 1, B], dtype=f32, device=dev) if want_vtrace else None,
       pg_advantages=torch.empty([T1 - 1, B], dtype=f32, device=dev) if want_vtrace else None)
+
+
+def vtrace_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits,
+                        actions, rewards, done, entropy_cost_param, want_vtrace=False):
+  """The fused kernel of compute_loss (learner.py:82-157) + its gradient.  All inputs
+  have T+1 rows.  Returns dict(loss_terms[16], dlogits, dbaseline, d_entropy_cost_param,
+  vs, pg_advantages)."""
+  ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
+                                               rewards, done, entropy_cost_param)
+  T1, B, A = (int(x) for x in ll.shape)
+  cfg = _loss_config(settings)
+  out = _loss_outputs(ll, lb, want_vtrace)
   import ctypes
   _lib.check(_lib.lib().seedrl_vtrace_loss_fwd_bwd(
       T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew),
       _lib.ptr(dn), ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(out['loss_terms']),
       _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
       _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']),
-      _lib.ptr(out['pg_advantages']), _lib.ptr(_loss_scratch(T1, B, A, dev)),
+      _lib.ptr(out['pg_advantages']), _lib.ptr(_loss_scratch(T1, B, A, ll.device)),
       _lib.stream_ptr()))
   return out
 
 
+def popart_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits, actions, rewards,
+                        done, entropy_cost_param, popart_moments, popart_compensation, d_popart_compensation,
+                        reduce_moment_sums=None, world=1, want_vtrace=False):
+  """compute_loss with PopArt (generalized_onpolicy_loss.py:94-133,169-199 around popart.py and
+  EMAMeanStd) + its gradient: seedrl_vtrace_popart_loss_fwd, then `reduce_moment_sums` (in-place
+  SUM of the two moment sums across the `world` replicas; None for one replica), then
+  seedrl_vtrace_popart_update.  Updates popart_moments (mu1, mu2) and popart_compensation
+  (sigma, mu) in place and writes d(loss)/d(sigma, mu) to d_popart_compensation.  Returns what
+  vtrace_loss_fwd_bwd returns; vs and pg_advantages are in return units."""
+  ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
+                                               rewards, done, entropy_cost_param)
+  T1, B, A = (int(x) for x in ll.shape)
+  f32 = torch.float32
+  for t, nm in ((popart_moments, 'popart_moments'), (popart_compensation, 'popart_compensation'),
+                (d_popart_compensation, 'd_popart_compensation')):
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == f32 and t.is_contiguous() and t.numel() == 2):
+      raise ValueError('%s must be a contiguous float32 CUDA tensor of 2 elements' % nm)
+  beta = float(settings.popart_beta)
+  if not 0.0 <= beta <= 1.0:
+    raise ValueError('popart_beta must be in [0, 1], got %r' % beta)
+  cfg = _loss_config(settings)
+  out = _loss_outputs(ll, lb, want_vtrace)
+  td = torch.empty([T1 - 1, B], dtype=f32, device=ll.device)
+  sums = torch.empty(2, dtype=f32, device=ll.device)
+  scratch = _loss_scratch(T1, B, A, ll.device)
+  import ctypes
+  L = _lib.lib()
+  _lib.check(L.seedrl_vtrace_popart_loss_fwd(
+      T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew),
+      _lib.ptr(dn), ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(popart_moments), _lib.ptr(popart_compensation),
+      _lib.ptr(out['loss_terms']), _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
+      _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']), _lib.ptr(out['pg_advantages']),
+      _lib.ptr(td), _lib.ptr(sums), _lib.ptr(scratch), _lib.stream_ptr()))
+  if reduce_moment_sums is not None:
+    reduce_moment_sums(sums)
+  _lib.check(L.seedrl_vtrace_popart_update(
+      T1, B, int(world), beta, float(settings.baseline_cost), _lib.ptr(lb), _lib.ptr(td), _lib.ptr(sums),
+      _lib.ptr(popart_moments), _lib.ptr(popart_compensation), _lib.ptr(out['dbaseline']),
+      _lib.ptr(d_popart_compensation), _lib.ptr(out['loss_terms']), _lib.ptr(scratch), _lib.stream_ptr()))
+  return out
+
+
 def compute_loss(logger, parametric_action_distribution, agent, agent_state,
-                 prev_actions, env_outputs, agent_outputs, settings=None):
+                 prev_actions, env_outputs, agent_outputs, settings=None, reduce_moment_sums=None, world=1):
   """reference learner.py:73-159.  Returns (total_loss, log session).  The gradient of
-  total_loss w.r.t. the network outputs is left on the agent for `minimize`."""
+  total_loss w.r.t. the network outputs is left on the agent for `minimize`.  With
+  settings.popart the agent must have enable_popart()'d: its PopArt state is updated here and
+  d(loss)/d(sigma, mu) written to its gradient tail; `reduce_moment_sums` and `world` are the
+  cross-replica sum of popart_loss_fwd_bwd."""
   settings = settings or loss_settings_from_flags()
   learner_outputs, _ = agent(prev_actions, env_outputs, agent_state,
                              unroll=True, is_training=True)                 # :75-79
-  r = vtrace_loss_fwd_bwd(settings, learner_outputs.policy_logits, learner_outputs.baseline,
-                          agent_outputs.policy_logits, agent_outputs.action,
-                          env_outputs[0], env_outputs[1], agent.entropy_cost_param)
+  if settings.popart:
+    if getattr(agent, 'popart_moments', None) is None:
+      raise ValueError('settings.popart needs an agent with enable_popart() called')
+    r = popart_loss_fwd_bwd(settings, learner_outputs.policy_logits, learner_outputs.baseline,
+                            agent_outputs.policy_logits, agent_outputs.action,
+                            env_outputs[0], env_outputs[1], agent.entropy_cost_param,
+                            agent.popart_moments, agent.popart_compensation, agent.popart_compensation_grad,
+                            reduce_moment_sums, world)
+  else:
+    r = vtrace_loss_fwd_bwd(settings, learner_outputs.policy_logits, learner_outputs.baseline,
+                            agent_outputs.policy_logits, agent_outputs.action,
+                            env_outputs[0], env_outputs[1], agent.entropy_cost_param)
   agent._loss_grads = r
   logger = logger or _NullLogger()
   session = logger.log_session()
   lt = r['loss_terms']
-  for name, key in _LOG_NAMES:
+  for name, key in _LOG_NAMES + (_POPART_LOG_NAMES if settings.popart else []):
     logger.log(session, name, lt[_lib.LT[key]])
   return lt[_lib.LT['total']], session
 
@@ -212,13 +292,22 @@ class LearnerStep(object):
     if not hasattr(agent, '_entropy_mul'):
       agent.init_entropy_cost(self.settings.entropy_cost,
                               self.settings.entropy_cost_adjustment_speed)       # :225-234
+    if self.settings.popart and agent.popart_moments is None:
+      if optimizer.m is not None:
+        raise ValueError('PopArt extends the parameter arena: enable it before the optimizer creates its slots')
+      agent.enable_popart()
     optimizer._create_slots(agent.params)                                        # :244-245
     self.last_loss_terms = None
+
+  def _reduce_moment_sums(self, sums):
+    import torch.distributed as td
+    td.all_reduce(sums, op=td.ReduceOp.SUM, group=self.pg)
 
   def compute_gradients(self, unroll):
     loss, logs = compute_loss(self.logger, self.dist, self.agent, unroll.agent_state,
                               unroll.prev_actions, unroll.env_outputs, unroll.agent_outputs,
-                              self.settings)
+                              self.settings, self._reduce_moment_sums if self.world > 1 else None,
+                              self.world)
     r = self.agent._loss_grads
     self._head_work = None
     if self.world > 1 and self.overlap_reduce and torch.cuda.is_available():

@@ -118,6 +118,7 @@ def save_checkpoint(path, agent, optimizer, extra=None):
 def restore_checkpoint(path, agent, optimizer):
   """ckpt.restore(...).assert_consumed() analogue: raises on a tensor-table mismatch."""
   d = torch.load(path, map_location='cpu', weights_only=False)
+  networks.check_popart_state(d['agent'], getattr(agent, 'popart_moments', None) is not None)
   info = d['agent'].get('param_info')
   if info is not None and [tuple(x) for x in info] != [tuple(x) for x in agent.param_info]:
     raise ValueError('checkpoint %s was written by a different network (tensor table mismatch)' % path)

@@ -12,6 +12,7 @@
 #include <cuda.h>
 #include <math.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "common.cuh"
@@ -174,7 +175,24 @@ struct LossParams {
   float* pg_out;
   double* partials;       // [grid][8]
   unsigned int* ticket;   // self-resetting
+  // PopArt instantiations only (phase 1 of seedrl_vtrace_popart_loss_fwd)
+  const float* pop_mom;   // [2] EMA moments mu1, mu2
+  const float* pop_comp;  // [2] compensation sigma, mu
+  float* pop_td;          // [T,B] (vs - u) / s
+  float* pop_sums;        // [2] sum vs, sum vs^2 over this replica's T x B
 };
+
+// ---- PopArt (agents/policy_gradient/modules/popart.py, running_statistics.py EMAMeanStd) ----
+// s = clip(sqrt(mu2 - mu1^2), 1e-6, 1e6) (running_statistics.py:149-153), evaluated in float64 and
+// rounded once; every kernel that needs s calls this, so the two phases agree bit for bit.
+__device__ __forceinline__ float popart_std(float mu1, float mu2) {
+  const double var = (double)mu2 - (double)mu1 * (double)mu1;
+  return (float)fmin(fmax(sqrt(var), 1e-6), 1e6);
+}
+// u = s (sigma V + mu) + m: correct_prediction, then unnormalize_prediction (popart.py)
+__device__ __forceinline__ float popart_u(float V, float s, float m, float sigma, float mu) {
+  return fmaf(s, fmaf(sigma, V, mu), m);
+}
 
 __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
   v = warp_sum(v);
@@ -393,7 +411,9 @@ __device__ __forceinline__ void row_grad(float* l, int A_rt, int a, float la, fl
 }
 
 // Last CTA to arrive (ticket) reduces the per-CTA partials in index order and writes the
-// loss terms; deterministic for a given grid.
+// loss terms; deterministic for a given grid.  POPART: partials 6 and 7 are sum vs and sum vs^2,
+// written to pop_sums; the value-loss terms are left to seedrl_vtrace_popart_update.
+template <bool POPART>
 __device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red, float ec) {
   const int tid = threadIdx.x;
   const float mul = p.cfg.entropy_cost_adjustment_speed;
@@ -420,6 +440,20 @@ __device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red,
 #pragma unroll
   for (int k = 0; k < 5; ++k) tot[k] = block_reduce_sum_d(acc5[k]);
   const float max_a = block_reduce_max(amax, s_red);
+  if (POPART) {
+    double s1 = 0.0, s2 = 0.0;
+    for (unsigned int g = tid; g < gridDim.x; g += blockDim.x) {
+      const volatile double* q = p.partials + (size_t)g * kLossPartials;
+      s1 += q[6];
+      s2 += q[7];
+    }
+    s1 = block_reduce_sum_d(s1);
+    s2 = block_reduce_sum_d(s2);
+    if (tid == 0) {
+      p.pop_sums[0] = (float)s1;
+      p.pop_sums[1] = (float)s2;
+    }
+  }
   if (tid == 0) {
     const double n = (double)p.T * (double)p.B;
     const float policy_loss = (float)(-tot[0] / n);
@@ -481,8 +515,11 @@ __device__ __forceinline__ void tile_copy(float* s_tile, typename std::condition
   }
 }
 
-__global__ void __launch_bounds__(kLossThreads)
-vtrace_loss_kernel(const LossParams p) {
+// POPART: the values V are replaced by u = s (sigma V + mu) + m before the scan, the policy gradient
+// takes pg_adv / s, and the value loss is left to seedrl_vtrace_popart_update: it gets (vs - u) / s
+// in pop_td and sum vs, sum vs^2 in pop_sums.
+template <bool POPART>
+__device__ __forceinline__ void loss_small_body(const LossParams& p) {
   extern __shared__ float smem[];
   const int T = p.T, B = p.B, A = p.A, BB = p.BB;
   const int b0 = blockIdx.x * BB;
@@ -519,12 +556,23 @@ vtrace_loss_kernel(const LossParams p) {
       s_rew[i] = 0.f; s_dis[i] = 0.f; s_act[i] = 0;
     }
   }
+  float pop_s = 1.f, pop_m = 0.f, pop_sigma = 1.f, pop_mu = 0.f;
+  if (POPART) {
+    pop_m = __ldg(p.pop_mom);
+    pop_s = popart_std(pop_m, __ldg(p.pop_mom + 1));
+    pop_sigma = __ldg(p.pop_comp);
+    pop_mu = __ldg(p.pop_comp + 1);
+  }
   for (int i = tid; i < (T + 1) * BB; i += kLossThreads) {
     const int t = i / BB, c = i - t * BB;
-    s_val[i] = c < nb ? __ldg(p.lb + (size_t)t * B + b0 + c) : 0.f;
+    if (POPART)
+      s_val[i] = c < nb ? popart_u(__ldg(p.lb + (size_t)t * B + b0 + c), pop_s, pop_m, pop_sigma, pop_mu) : 0.f;
+    else
+      s_val[i] = c < nb ? __ldg(p.lb + (size_t)t * B + b0 + c) : 0.f;
   }
 
   double sum_tp = 0.0, sum_ve2 = 0.0, sum_h = 0.0, sum_kl = 0.0, sum_v = 0.0;
+  double sum_vs = 0.0, sum_vs2 = 0.0;
 
   // ---- phase A: behaviour logits ------------------------------------------
   tile_copy<true>(s_logits, p.bl + (size_t)b0 * A, T, B, A, BB, nb, tid);
@@ -595,13 +643,22 @@ vtrace_loss_kernel(const LossParams p) {
       vs_next = vs_t;
       v_next = v;
       const float verr = vs_t - v;                         // :115
-      sum_tp += tl * pg;                                   // :111-112
-      sum_ve2 += verr * verr;                              // :116
+      if (POPART) {
+        const float pgn = __fdiv_rn(pg, pop_s);            // generalized_onpolicy_loss.py:129-132
+        sum_tp += tl * pgn;
+        sum_vs += vs_t;
+        sum_vs2 += (double)vs_t * vs_t;
+        s_tlp[i] = pgn;
+        s_blp[i] = __fdiv_rn(verr, pop_s);
+      } else {
+        sum_tp += tl * pg;                                 // :111-112
+        sum_ve2 += verr * verr;                            // :116
+        s_tlp[i] = pg;     // reuse: pg_adv
+        s_blp[i] = verr;   // reuse: v_err
+      }
       sum_h += s_ent[i];
       sum_v += v;
       max_a = fmaxf(max_a, fabsf((float)s_act[i]));
-      s_tlp[i] = pg;     // reuse: pg_adv
-      s_blp[i] = verr;   // reuse: v_err
       const size_t g = (size_t)t * B + b0 + c;
       if (p.vs_out) p.vs_out[g] = vs_t;
       if (p.pg_out) p.pg_out[g] = pg;
@@ -631,8 +688,12 @@ vtrace_loss_kernel(const LossParams p) {
   for (int i = tid; i < (T + 1) * BB; i += kLossThreads) {
     const int t = i / BB, c = i - t * BB;
     if (c < nb) {
-      // d(bc*0.5*mean((vs-V)^2))/dV = -bc*(vs-V)/N
-      p.dbaseline[(size_t)t * B + b0 + c] = t < T ? -p.cfg.baseline_cost * s_blp[i] * invN : 0.f;
+      if (POPART && t < T) {
+        p.pop_td[(size_t)t * B + b0 + c] = s_blp[i];
+      } else {
+        // d(bc*0.5*mean((vs-V)^2))/dV = -bc*(vs-V)/N
+        p.dbaseline[(size_t)t * B + b0 + c] = t < T ? -p.cfg.baseline_cost * s_blp[i] * invN : 0.f;
+      }
     }
   }
 
@@ -645,7 +706,16 @@ vtrace_loss_kernel(const LossParams p) {
   r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
   r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  loss_finalize(p, s_red, ec);
+  if (POPART) {
+    r = block_reduce_sum_d(sum_vs);  if (tid == 0) part[6] = r;
+    r = block_reduce_sum_d(sum_vs2); if (tid == 0) part[7] = r;
+  }
+  loss_finalize<POPART>(p, s_red, ec);
+}
+
+__global__ void __launch_bounds__(kLossThreads) vtrace_loss_kernel(const LossParams p) { loss_small_body<false>(p); }
+__global__ void __launch_bounds__(kLossThreads) vtrace_popart_loss_kernel(const LossParams p) {
+  loss_small_body<true>(p);
 }
 
 
@@ -695,12 +765,11 @@ struct SmallRegs {
   uint8_t done[kStreamRounds];
 };
 
-template <int AS>
-__global__ void __launch_bounds__(kStreamThreadsMax)
-vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
-                          const __grid_constant__ CUtensorMap tm_bl,
-                          const __grid_constant__ CUtensorMap tm_ll,
-                          const __grid_constant__ CUtensorMap tm_dl) {
+// POPART: as in loss_small_body.
+template <int AS, bool POPART>
+__device__ __forceinline__ void loss_stream_body(const LossParams& p, const int ntiles, const int tile_stride_f,
+                                                 const CUtensorMap& tm_bl, const CUtensorMap& tm_ll,
+                                                 const CUtensorMap& tm_dl) {
   extern __shared__ __align__(128) float smem[];
   const int T = p.T, B = p.B, A = AS ? AS : p.A, BB = p.BB;
   const int rows = T * BB;
@@ -729,8 +798,15 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   const int bb_sh = 31 - __clz(BB);                      // BB is a power of two
   int lpc = 32;                                          // lanes per column in the scan
   while (lpc > 1 && T <= lpc * 4) lpc >>= 1;
+  __shared__ float s_pop[4];                             // PopArt s, m, sigma, mu
 
   if (tid == 0) {
+    if (POPART) {
+      s_pop[0] = popart_std(__ldg(p.pop_mom), __ldg(p.pop_mom + 1));
+      s_pop[1] = __ldg(p.pop_mom);
+      s_pop[2] = __ldg(p.pop_comp);
+      s_pop[3] = __ldg(p.pop_comp + 1);
+    }
 #pragma unroll
     for (int k = 0; k < 3; ++k)
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sm_u32(s_full + k)));
@@ -744,6 +820,7 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   // per-thread sums stay fp32 (a thread adds one or a few rows per tile); the block and grid
   // reductions are float64
   float sum_tp = 0.f, sum_ve2 = 0.f, sum_h = 0.f, sum_kl = 0.f, sum_v = 0.f, max_a = 0.f;
+  float sum_vs = 0.f, sum_vs2 = 0.f;
   // one thread, one instruction per tile
   auto issue_load = [&](int k, const CUtensorMap* tm, int tile) {
     uint64_t* bar = s_full + (k % 3);
@@ -777,7 +854,7 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
     for (int k = 0; k < kStreamRounds; ++k) {
       const int i = tid + k * nthreads;
       if (i < (T + 1) * BB) {
-        s_val[i] = r.val[k];
+        s_val[i] = POPART ? popart_u(r.val[k], s_pop[0], s_pop[1], s_pop[2], s_pop[3]) : r.val[k];
         if (i < rows) {
           float rw = r.rew[k];
           if (p.cfg.max_abs_reward != 0.f)                 // :90-92
@@ -911,13 +988,22 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
       const float vs_next = t + 1 < T ? s_acc[i + BB] + s_val[i + BB] : s_val[T * BB + c];
       const float pg = s_cpg[i] * (s_rew[i] + s_dis[i] * vs_next - v);   // vtrace.py:143-144
       const float tl = s_tlp[i];
-      sum_tp += tl * pg;                                   // :111-112
-      sum_ve2 += verr * verr;                              // :116
       const size_t g = (size_t)t * B + (size_t)tile * BB + c;
       if (p.vs_out) p.vs_out[g] = verr + v;
       if (p.pg_out) p.pg_out[g] = pg;
-      p.dbaseline[g] = -p.cfg.baseline_cost * verr * invN;
-      row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_la[i], s_lb[i], s_ent[i], -(pg + kc) * invN, ec * invN);
+      if (POPART) {
+        const float s = s_pop[0], pgn = __fdiv_rn(pg, s), vs = verr + v;   // generalized_onpolicy_loss.py:129-132
+        sum_tp += tl * pgn;
+        sum_vs += vs;
+        sum_vs2 += vs * vs;
+        p.pop_td[g] = __fdiv_rn(verr, s);
+        row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_la[i], s_lb[i], s_ent[i], -(pgn + kc) * invN, ec * invN);
+      } else {
+        sum_tp += tl * pg;                                 // :111-112
+        sum_ve2 += verr * verr;                            // :116
+        p.dbaseline[g] = -p.cfg.baseline_cost * verr * invN;
+        row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_la[i], s_lb[i], s_ent[i], -(pg + kc) * invN, ec * invN);
+      }
     }
     // generic-proxy writes of the gradient tile -> visible to the TMA (async) proxy
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -948,7 +1034,124 @@ vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_s
   r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
   r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  loss_finalize(p, s_red, ec);
+  if (POPART) {
+    r = block_reduce_sum_d(sum_vs);  if (tid == 0) part[6] = r;
+    r = block_reduce_sum_d(sum_vs2); if (tid == 0) part[7] = r;
+  }
+  loss_finalize<POPART>(p, s_red, ec);
+}
+
+template <int AS>
+__global__ void __launch_bounds__(kStreamThreadsMax)
+vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
+                          const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_ll,
+                          const __grid_constant__ CUtensorMap tm_dl) {
+  loss_stream_body<AS, false>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
+}
+template <int AS>
+__global__ void __launch_bounds__(kStreamThreadsMax)
+vtrace_popart_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
+                                 const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_ll,
+                                 const __grid_constant__ CUtensorMap tm_dl) {
+  loss_stream_body<AS, true>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
+}
+
+// ---------------------------------------------------------------------------
+// (a2, PopArt phase 2)  After phase 1 (and the cross-replica sum of its two moment sums): the EMA
+// and compensation update, the value loss and its gradients (steps 5-8 of the PopArt learner step,
+// running_statistics.py:123-153, popart.py:163-183, generalized_onpolicy_loss.py:94-133).
+// Grid-stride over the T x B value rows; every CTA derives the same new state from the same inputs,
+// and the last CTA to arrive (ticket) reduces the per-CTA float64 partials in index order, writes
+// the state and the loss terms.  No floating-point atomics: deterministic for a given shape.
+//   e = n - (sigma+ V + mu+) = td + ((sigma V + mu) - (sigma+ V + mu+)),  td = (vs - u) / s
+// (n = (vs - m)/s and u = s (sigma V + mu) + m).  The residual form is the kernels' own verr / s:
+// with the state unchanged it gives phase 1's verr exactly, and it never subtracts two
+// return-sized numbers.
+constexpr int kPopThreads = 512;
+constexpr int kPopPartials = 4;
+
+struct PopArtUpdateParams {
+  int T, B;
+  float baseline_cost, beta;
+  double count;            // elements behind pop_sums: world x T x B
+  const float* lb;         // [T+1,B] learner baseline V
+  const float* td;         // [T,B]
+  const float* sums;       // [2]
+  float* mom;              // [2] mu1, mu2 (in/out)
+  float* comp;             // [2] sigma, mu (in/out)
+  float* dbaseline;        // rows [0,T)
+  float* dcomp;            // [2] d sigma, d mu
+  float* loss_terms;
+  double* partials;        // [grid][4]
+  unsigned int* ticket;
+};
+
+__global__ void __launch_bounds__(kPopThreads)
+vtrace_popart_update_kernel(const PopArtUpdateParams p) {
+  __shared__ bool s_last;
+  const int tid = threadIdx.x;
+  const float mu1 = p.mom[0], mu2 = p.mom[1], sigma = p.comp[0], mu = p.comp[1];
+  // EMAMeanStd.update (running_statistics.py:123-147), in fp32 like the reference's variables
+  const float bm1 = (float)((double)p.sums[0] / p.count), bm2 = (float)((double)p.sums[1] / p.count);
+  const float mu1n = __fadd_rn(mu1, __fmul_rn(p.beta, __fsub_rn(bm1, mu1)));
+  const float mu2n = __fadd_rn(mu2, __fmul_rn(p.beta, __fsub_rn(bm2, mu2)));
+  const float s = popart_std(mu1, mu2), sn = popart_std(mu1n, mu2n);
+  // popart.py:178-183
+  const float sigma_n = __fmul_rn(__fdiv_rn(s, sn), sigma);
+  const float mu_n = __fdiv_rn(__fadd_rn(__fsub_rn(mu1, mu1n), __fmul_rn(s, mu)), sn);
+
+  const size_t n = (size_t)p.T * p.B;
+  const float invN = 1.0f / ((float)p.T * (float)p.B);
+  double se2 = 0.0, sev = 0.0, se = 0.0;
+  for (size_t i = (size_t)blockIdx.x * kPopThreads + tid; i < n; i += (size_t)gridDim.x * kPopThreads) {
+    const float V = __ldg(p.lb + i);
+    const float e = __ldg(p.td + i) + (fmaf(sigma, V, mu) - fmaf(sigma_n, V, mu_n));
+    // d(bc * 0.5 * mean(e^2)) / dV = -bc e sigma+ / N
+    p.dbaseline[i] = (-p.baseline_cost * e * invN) * sigma_n;
+    se2 += (double)e * e;
+    sev += (double)e * V;
+    se += e;
+  }
+  double r;
+  double* part = p.partials + (size_t)blockIdx.x * kPopPartials;
+  r = block_reduce_sum_d(se2); if (tid == 0) part[0] = r;
+  r = block_reduce_sum_d(sev); if (tid == 0) part[1] = r;
+  r = block_reduce_sum_d(se);  if (tid == 0) part[2] = r;
+  if (tid == 0) {
+    __threadfence();
+    s_last = atomicAdd(p.ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  double a[3] = {0.0, 0.0, 0.0};
+  for (unsigned int g = tid; g < gridDim.x; g += blockDim.x) {
+    const volatile double* q = p.partials + (size_t)g * kPopPartials;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a[k] += q[k];
+  }
+  double tot[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) tot[k] = block_reduce_sum_d(a[k]);
+  if (tid == 0) {
+    const double nn = (double)n;
+    const float mse = (float)(tot[0] / nn);
+    const float v_loss = p.baseline_cost * 0.5f * mse;
+    float* L = p.loss_terms;
+    L[SEEDRL_LT_V] = v_loss;
+    L[SEEDRL_LT_V_L2_ERROR] = sqrtf(mse);
+    L[SEEDRL_LT_TOTAL] = L[SEEDRL_LT_POLICY] + v_loss + L[SEEDRL_LT_ENTROPY] + L[SEEDRL_LT_KL] +
+                         L[SEEDRL_LT_ENTROPY_ADJ];
+    L[SEEDRL_LT_POPART_MEAN] = mu1n;
+    L[SEEDRL_LT_POPART_STD] = sn;
+    p.dcomp[0] = (float)(-(double)p.baseline_cost * tot[1] / nn);
+    p.dcomp[1] = (float)(-(double)p.baseline_cost * tot[2] / nn);
+    p.mom[0] = mu1n;
+    p.mom[1] = mu2n;
+    p.comp[0] = sigma_n;
+    p.comp[1] = mu_n;
+    *p.ticket = 0u;
+  }
 }
 
 static size_t loss_smem_bytes(int T, int A, int BB) {
@@ -1028,10 +1231,12 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
   return 0;
 }
 
-template <int AS>
+template <int AS, bool POPART>
 static cudaError_t launch_stream(const LossParams& p, int ntiles, int threads, size_t smem, cudaStream_t stream,
                                  const CUtensorMap& tm_bl, const CUtensorMap& tm_ll, const CUtensorMap& tm_dl) {
-  const cudaError_t e = allow_smem<vtrace_loss_stream_kernel<AS>>((int)kStreamSmemMax);
+  auto kernel = POPART ? vtrace_popart_loss_stream_kernel<AS> : vtrace_loss_stream_kernel<AS>;
+  const cudaError_t e = POPART ? allow_smem<vtrace_popart_loss_stream_kernel<AS>>((int)kStreamSmemMax)
+                               : allow_smem<vtrace_loss_stream_kernel<AS>>((int)kStreamSmemMax);
   if (e != cudaSuccess) return e;
   // persistent CTAs: as many per SM as shared memory and threads allow (small T: several,
   // so one CTA's barriers and scan hide behind another's copies)
@@ -1041,7 +1246,7 @@ static cudaError_t launch_stream(const LossParams& p, int ntiles, int threads, s
   if (per_sm < 1) per_sm = 1;
   int grid = num_sms() * per_sm;
   if (grid > ntiles) grid = ntiles;
-  vtrace_loss_stream_kernel<AS><<<grid, threads, smem, stream>>>(
+  kernel<<<grid, threads, smem, stream>>>(
       p, ntiles, stream_tile_stride_f(p.T, p.A, p.BB), tm_bl, tm_ll, tm_dl);
   return cudaSuccess;
 }
@@ -1138,6 +1343,56 @@ extern "C" size_t seedrl_vtrace_loss_scratch_bytes(int T1, int B, int A) {
   return 256 + (size_t)(B > kNumSMs ? B : kNumSMs) * kLossPartials * sizeof(double);
 }
 
+// Picks the kernel form (TMA-streamed at large aligned B, else vtrace_loss_kernel) and launches it;
+// p has everything but BB.
+template <bool POPART>
+static int launch_loss(LossParams p, cudaStream_t st) {
+  const int T1 = p.T + 1, B = p.B, A = p.A;
+  size_t smem = 0;
+  auto small_kernel = POPART ? vtrace_popart_loss_kernel : vtrace_loss_kernel;
+  SEEDRL_CUDA(POPART ? allow_smem<vtrace_popart_loss_kernel>(200 * 1024) : allow_smem<vtrace_loss_kernel>(200 * 1024));
+  int threads = 0;
+  p.BB = g_loss_stream_enabled ? pick_stream(p, g_loss_stream_enabled, &threads, &smem) : 0;
+  alignas(64) CUtensorMap tm_bl, tm_ll, tm_dl;
+  if (p.BB > 0 && !(make_tile_map(&tm_bl, p.bl, T1, p.T, B, A, p.BB) &&
+                    make_tile_map(&tm_ll, p.ll, T1, p.T, B, A, p.BB) &&
+                    make_tile_map(&tm_dl, p.dlogits, T1, p.T, B, A, p.BB)))
+    p.BB = 0;
+  if (p.BB > 0) {
+    const int ntiles = B / p.BB;
+    switch (A) {   // compile-time action counts of the reference's environments
+      case 9:  SEEDRL_CUDA((launch_stream<9, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;    // DMLab
+      case 18: SEEDRL_CUDA((launch_stream<18, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // Atari
+      case 19: SEEDRL_CUDA((launch_stream<19, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // football
+      default: SEEDRL_CUDA((launch_stream<0, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;
+    }
+  } else {
+    p.BB = pick_bb(p.T, B, A, &smem);
+    SEEDRL_CHECK_ARG(p.BB > 0, "unroll_length * num_actions too large for shared memory");
+    small_kernel<<<ceil_div(B, p.BB), kLossThreads, smem, st>>>(p);
+  }
+  count_launch(PC_LOSS, st);
+  SEEDRL_CHECK_LAUNCH();
+  return SEEDRL_OK;
+}
+
+static LossParams loss_params(int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
+                              const float* behaviour_logits, const int64_t* actions, const float* rewards,
+                              const uint8_t* done, const seedrl_loss_config* cfg, const float* entropy_cost_param,
+                              float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
+                              float* vs_out, float* pg_advantages_out, void* scratch) {
+  LossParams p = {};
+  p.T = T1 - 1; p.B = B; p.A = A;
+  p.AP = A | 1;
+  p.ll = learner_logits; p.lb = learner_baseline; p.bl = behaviour_logits;
+  p.act = actions; p.rew = rewards; p.done = done; p.cfg = *cfg; p.ecp = entropy_cost_param;
+  p.loss_terms = loss_terms; p.dlogits = dlogits; p.dbaseline = dbaseline;
+  p.d_ecp = d_entropy_cost_param; p.vs_out = vs_out; p.pg_out = pg_advantages_out;
+  p.ticket = reinterpret_cast<unsigned int*>(scratch);
+  p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
+  return p;
+}
+
 extern "C" int seedrl_vtrace_loss_fwd_bwd(
     int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
     const float* behaviour_logits, const int64_t* actions, const float* rewards,
@@ -1149,38 +1404,59 @@ extern "C" int seedrl_vtrace_loss_fwd_bwd(
                        rewards && done && cfg && entropy_cost_param && loss_terms &&
                        dlogits && dbaseline && d_entropy_cost_param && scratch,
                    "null pointer");
-  LossParams p;
-  p.T = T1 - 1; p.B = B; p.A = A;
-  size_t smem = 0;
-  p.AP = A | 1;
-  p.ll = learner_logits; p.lb = learner_baseline; p.bl = behaviour_logits;
-  p.act = actions; p.rew = rewards; p.done = done; p.cfg = *cfg; p.ecp = entropy_cost_param;
-  p.loss_terms = loss_terms; p.dlogits = dlogits; p.dbaseline = dbaseline;
-  p.d_ecp = d_entropy_cost_param; p.vs_out = vs_out; p.pg_out = pg_advantages_out;
+  return launch_loss<false>(
+      loss_params(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done, cfg,
+                  entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param, vs_out,
+                  pg_advantages_out, scratch),
+      (cudaStream_t)stream);
+}
+
+extern "C" int seedrl_vtrace_popart_loss_fwd(
+    int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions, const float* rewards,
+    const uint8_t* done, const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
+    float* vs_out, float* pg_advantages_out, float* td_out, float* moment_sums,
+    void* scratch, seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(T1 >= 2 && B >= 1 && A >= 1, "need T1>=2, B>=1, A>=1");
+  SEEDRL_CHECK_ARG(learner_logits && learner_baseline && behaviour_logits && actions &&
+                       rewards && done && cfg && entropy_cost_param && popart_moments &&
+                       popart_compensation && loss_terms && dlogits && dbaseline &&
+                       d_entropy_cost_param && td_out && moment_sums && scratch,
+                   "null pointer");
+  LossParams p = loss_params(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done,
+                             cfg, entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param,
+                             vs_out, pg_advantages_out, scratch);
+  p.pop_mom = popart_moments; p.pop_comp = popart_compensation;
+  p.pop_td = td_out; p.pop_sums = moment_sums;
+  return launch_loss<true>(p, (cudaStream_t)stream);
+}
+
+extern "C" int seedrl_vtrace_popart_update(
+    int T1, int B, int world, float beta, float baseline_cost, const float* learner_baseline,
+    const float* td, const float* moment_sums, float* popart_moments, float* popart_compensation,
+    float* dbaseline, float* d_popart_compensation, float* loss_terms, void* scratch,
+    seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(T1 >= 2 && B >= 1 && world >= 1, "need T1>=2, B>=1, world>=1");
+  SEEDRL_CHECK_ARG(beta >= 0.f && beta <= 1.f, "beta must be in [0, 1]");
+  SEEDRL_CHECK_ARG(learner_baseline && td && moment_sums && popart_moments && popart_compensation &&
+                       dbaseline && d_popart_compensation && loss_terms && scratch,
+                   "null pointer");
+  PopArtUpdateParams p;
+  p.T = T1 - 1; p.B = B;
+  p.baseline_cost = baseline_cost; p.beta = beta;
+  p.count = (double)world * (double)p.T * (double)B;
+  p.lb = learner_baseline; p.td = td; p.sums = moment_sums;
+  p.mom = popart_moments; p.comp = popart_compensation;
+  p.dbaseline = dbaseline; p.dcomp = d_popart_compensation; p.loss_terms = loss_terms;
   p.ticket = reinterpret_cast<unsigned int*>(scratch);
   p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
-  SEEDRL_CUDA(allow_smem<vtrace_loss_kernel>(200 * 1024));
-  int threads = 0;
-  p.BB = g_loss_stream_enabled ? pick_stream(p, g_loss_stream_enabled, &threads, &smem) : 0;
-  alignas(64) CUtensorMap tm_bl, tm_ll, tm_dl;
-  if (p.BB > 0 && !(make_tile_map(&tm_bl, p.bl, T1, p.T, B, A, p.BB) &&
-                    make_tile_map(&tm_ll, p.ll, T1, p.T, B, A, p.BB) &&
-                    make_tile_map(&tm_dl, p.dlogits, T1, p.T, B, A, p.BB)))
-    p.BB = 0;
-  if (p.BB > 0) {
-    const int ntiles = B / p.BB;
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (A) {   // compile-time action counts of the reference's environments
-      case 9:  SEEDRL_CUDA(launch_stream<9>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl)); break;    // DMLab
-      case 18: SEEDRL_CUDA(launch_stream<18>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl)); break;   // Atari
-      case 19: SEEDRL_CUDA(launch_stream<19>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl)); break;   // football
-      default: SEEDRL_CUDA(launch_stream<0>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl)); break;
-    }
-  } else {
-    p.BB = pick_bb(p.T, B, A, &smem);
-    SEEDRL_CHECK_ARG(p.BB > 0, "unroll_length * num_actions too large for shared memory");
-    vtrace_loss_kernel<<<ceil_div(B, p.BB), kLossThreads, smem, (cudaStream_t)stream>>>(p);
-  }
+  // at most kNumSMs CTAs: their partials fit the kNumSMs x kLossPartials doubles that
+  // seedrl_vtrace_loss_scratch_bytes always provides
+  const size_t n = (size_t)p.T * B;
+  const int grid = (int)std::min<size_t>(ceil_div_sz(n, (size_t)kPopThreads * 4), (size_t)kNumSMs);
+  vtrace_popart_update_kernel<<<grid, kPopThreads, 0, (cudaStream_t)stream>>>(p);
   count_launch(PC_LOSS, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;

@@ -175,6 +175,57 @@ class _CudaAgent(CudaNet):
   def entropy_cost(self):
     return torch.exp(self._entropy_mul * self.entropy_cost_param)
 
+  # ---- PopArt (popart.py; the V-trace learner's --popart) ---------------------------
+  popart_moments = None    # [2] EMA moments (mu1, mu2): a device buffer of their own, not trained
+
+  def enable_popart(self):
+    """Appends the trained compensation (sigma, mu) = (1, 0) after entropy_cost_param, in a 64-float
+    tail of the parameter and gradient arenas (so Adam and the gradient all-reduce take them with
+    everything else), and creates the moments (0, 1).  The network's own arena, its offsets and
+    grad_split are unchanged.  Call before an optimizer creates its slots and before anything keeps
+    a pointer to `params` (inference hosts, CUDA graphs): both arenas are reallocated."""
+    if self.popart_moments is not None:
+      return
+    off = self.arena_floats
+    params = torch.zeros(off + 64, dtype=torch.float32, device=self.device)
+    params[:off].copy_(self.params)
+    params[off] = 1.0
+    self.params, self.grads = params, torch.zeros_like(params)
+    self.param_info = self.param_info + [('popart/compensation_std', (), off), ('popart/compensation_mean', (), off + 1)]
+    self.popart_moments = torch.tensor([0.0, 1.0], dtype=torch.float32, device=self.device)
+
+  @property
+  def popart_compensation(self):
+    """(sigma, mu): a view of the parameter arena."""
+    off = self.arena_floats
+    return self.params[off:off + 2]
+
+  @property
+  def popart_compensation_grad(self):
+    off = self.arena_floats
+    return self.grads[off:off + 2]
+
+  def state_dict(self):
+    d = super(_CudaAgent, self).state_dict()
+    if self.popart_moments is not None:
+      d['popart_moments'] = self.popart_moments.detach().cpu()
+    return d
+
+  def load_state_dict(self, d):
+    check_popart_state(d, self.popart_moments is not None)
+    super(_CudaAgent, self).load_state_dict(d)
+    if self.popart_moments is not None:
+      self.popart_moments.copy_(d['popart_moments'].to(self.device))
+
+
+def check_popart_state(agent_state, popart):
+  """Raises ValueError when a checkpoint's agent state and a learner disagree on PopArt."""
+  has = 'popart_moments' in agent_state
+  if has and not popart:
+    raise ValueError('the checkpoint was written with PopArt (--popart); this learner runs without it')
+  if popart and not has:
+    raise ValueError('the checkpoint was written without PopArt; this learner runs with --popart')
+
 
 class ImpalaDeep(_CudaAgent):
   """reference dmlab/networks.py:63-171."""
