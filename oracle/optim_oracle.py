@@ -35,7 +35,8 @@ def keras_adam_step(p, g, m, v, iterations, lr, beta1=0.9, beta2=0.999, eps=1e-7
   `training_ops.resource_apply_adam` update in the form its Eigen kernel uses:
       m += (g - m) * (1 - beta1);  v += (g*g - v) * (1 - beta2)
       var -= (m * lr_t) / (sqrt(v) + eps)
-  Note `1 - beta2` is an fp32 subtraction (1 - fp32(0.999) = 0.00100004673)."""
+  Note `1 - beta2` is an fp32 subtraction, exact for beta2 in [0.5, 1]: 1 - fp32(0.999) = 0.000999987125, not the
+  decimal 0.001."""
   f = np.float32
   t = f(iterations + 1)
   b1, b2 = f(beta1), f(beta2)
