@@ -130,6 +130,24 @@ int seedrl_vtrace_loss_fwd_bwd(
     float* loss_terms, float* dlogits, float* dbaseline,
     float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
     void* scratch, seedrl_stream_t stream);
+/* Abandoned episodes (reference agents/policy_gradient/modules/advantages.py vtrace): the same, with
+ * abandoned uint8 [T1,B] after done (NULL = none; seedrl_vtrace_loss_fwd_bwd passes NULL).  An
+ * abandoned row ended an episode by a time limit, not by the task: row t+1 holds the reset
+ * observation, and the caller guarantees done[t+1] = 1 there.  Transition t is masked iff
+ * abandoned[t+1]: its rho-weighted TD term and its clipped policy-gradient rho are 0, so vs_t = V_t,
+ * pg_advantages_t = 0, dbaseline row t = 0, and vs_{t-1} bootstraps from V_t, the value of the
+ * last real observation, instead of treating it as terminal.  Entropy and KL still cover every row,
+ * and every mean keeps its (T1-1) x B denominator.  With abandoned NULL or all zero every output is
+ * bit-identical to seedrl_vtrace_loss_fwd_bwd. */
+int seedrl_vtrace_loss_fwd_bwd_abandoned(
+    int T1, int B, int A,
+    const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions,
+    const float* rewards, const uint8_t* done, const uint8_t* abandoned,
+    const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    float* loss_terms, float* dlogits, float* dbaseline,
+    float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
+    void* scratch, seedrl_stream_t stream);
 
 /* PopArt value normalisation (opt-in; reference agents/policy_gradient/modules/popart.py with
  * running_statistics.py EMAMeanStd, composed as in generalized_onpolicy_loss.py:94-133,169-199).
@@ -157,6 +175,18 @@ int seedrl_vtrace_popart_loss_fwd(
     const float* learner_logits, const float* learner_baseline,
     const float* behaviour_logits, const int64_t* actions,
     const float* rewards, const uint8_t* done,
+    const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline,
+    float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
+    float* td_out, float* moment_sums, void* scratch, seedrl_stream_t stream);
+/* seedrl_vtrace_popart_loss_fwd with the abandoned mask of seedrl_vtrace_loss_fwd_bwd_abandoned:
+ * masked rows have vs_t = u_t, so they enter moment_sums as u_t and td_out there is 0. */
+int seedrl_vtrace_popart_loss_fwd_abandoned(
+    int T1, int B, int A,
+    const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions,
+    const float* rewards, const uint8_t* done, const uint8_t* abandoned,
     const seedrl_loss_config* cfg, const float* entropy_cost_param,
     const float* popart_moments, const float* popart_compensation,
     float* loss_terms, float* dlogits, float* dbaseline,
@@ -473,6 +503,28 @@ int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float* q_train, 
                                      float lambda_, float eta, float value_rescaling_eps, float* loss,
                                      float* priorities, float* dq, void* scratch,
                                      seedrl_stream_t stream);
+/* Abandoned episodes (reference agents/policy_gradient/modules/advantages.py NStep): the two losses
+ *   above with abandoned uint8 [T,B] after done (NULL = none; the entry points without the suffix
+ *   pass NULL).  Row i abandoned marks the transition into x_i as not real (a time limit ended the
+ *   episode, x_i is the reset observation, done_i = 1).  Transition t is masked iff row t+1 is
+ *   abandoned: td_t = 0 in the loss and the priorities (whose denominators stay T-1) and its dq row
+ *   is 0.  With q*_i as above, an unmasked n-step target walks i = t+1 .. t+n: an abandoned row i stops
+ *   it at G + gamma^(i-1-t) q*_{i-1}; otherwise G += gamma^(i-1-t) r_i, and a terminated row stops it
+ *   at G; past the window it bootstraps as the reference does.  Retrace: Y[i] = r_i + g_i q*_i when
+ *   row i+1 is abandoned (no trace correction).  With abandoned NULL or all zero every output is
+ *   bit-identical to the entry points without it. */
+int seedrl_r2d2_loss_fwd_bwd_abandoned(int T, int B, int A, const float* q_train, const float* q_target,
+                                       const int64_t* replay_action, const float* reward, const uint8_t* done,
+                                       const uint8_t* abandoned, const float* importance_weights, float gamma,
+                                       int n_steps, float eta, float value_rescaling_eps, float* loss,
+                                       float* priorities, float* dq, void* scratch, seedrl_stream_t stream);
+int seedrl_r2d2_retrace_loss_fwd_bwd_abandoned(int T, int B, int A, const float* q_train, const float* q_target,
+                                               const int64_t* replay_action, const float* reward,
+                                               const uint8_t* done, const uint8_t* abandoned,
+                                               const float* importance_weights, float gamma, float lambda_,
+                                               float eta, float value_rescaling_eps, float* loss,
+                                               float* priorities, float* dq, void* scratch,
+                                               seedrl_stream_t stream);
 /* <- agents/r2d2/learner.py:155-177 (apply_epsilon_greedy) on the device.  actions int32 [N]: the
  *   greedy actions on entry, the chosen ones on exit; envs_epsilon float32 [num_envs] (the table of
  *   get_envs_epsilon, :129-152), read at env_ids[n].  Row n draws

@@ -85,6 +85,12 @@ SIGNATURES = {
     'seedrl_vtrace_popart_loss_fwd':
         (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, ctypes.POINTER(LossConfig), P, P, P,
                  P, P, P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_loss_fwd_bwd_abandoned':
+        (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, ctypes.POINTER(LossConfig), P,
+                 P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_popart_loss_fwd_abandoned':
+        (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, ctypes.POINTER(LossConfig), P, P, P,
+                 P, P, P, P, P, P, P, P, P, P]),
     'seedrl_vtrace_popart_update':
         (c_int, [c_int, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P, P, P, P]),
     'seedrl_adam_apply':
@@ -153,6 +159,10 @@ SIGNATURES = {
     'seedrl_r2d2_retrace_loss_scratch_bytes': (c_size_t, [c_int, c_int]),
     'seedrl_r2d2_retrace_loss_fwd_bwd': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, c_float, c_float, c_float,
                                                  c_float, P, P, P, P, P]),
+    'seedrl_r2d2_loss_fwd_bwd_abandoned': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, c_float, c_int,
+                                                   c_float, c_float, P, P, P, P, P]),
+    'seedrl_r2d2_retrace_loss_fwd_bwd_abandoned': (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, c_float,
+                                                           c_float, c_float, c_float, P, P, P, P, P]),
     'seedrl_r2d2_epsilon_greedy': (c_int, [c_int, c_int, P, P, c_u64, P, P, P]),
     'seedrl_replay_sample': (c_int, [c_int, P, c_float, c_float, c_int, P, P, P, P, P]),
     'seedrl_clip_scratch_bytes': (c_size_t, []),

@@ -66,6 +66,10 @@ _define(flags.DEFINE_string, 'bellman_target', 'n_step',
         'Retrace(lambda) targets (Munos et al. 2016) with a target policy greedy in the online network. '
         'Retrace is not in the reference; under it --n_steps is unused.')
 _define(flags.DEFINE_float, 'retrace_lambda', 0.95, 'Trace coefficient lambda in [0, 1] of --bellman_target=retrace.')
+_define(flags.DEFINE_bool, 'bootstrap_abandoned', False,
+        'Accept abandoned episodes (EnvOutput.abandoned: a time limit, not the task, ended them) and '
+        'bootstrap from the value of their last observation instead of treating it as terminal '
+        '(advantages.py NStep).')
 _define(flags.DEFINE_float, 'eval_epsilon', 1e-3, 'Epsilon (as in epsilon-greedy) used for evaluation.')
 _define(flags.DEFINE_bool, 'inference_cuda_graph', False,
         'Replay the device side of every full inference batch as one CUDA graph, with epsilon-greedy '
@@ -88,7 +92,7 @@ R2D2Settings = collections.namedtuple(
     'batch_size replay_ratio unroll_length update_target_every_n_step replay_buffer_size '
     'replay_buffer_min_size priority_exponent burn_in importance_sampling_exponent clip_norm '
     'value_function_rescaling_epsilon n_steps discounting eval_epsilon num_training_tpus bellman_target '
-    'retrace_lambda')
+    'retrace_lambda bootstrap_abandoned', defaults=(False,))
 
 
 def default_settings(**kw):
@@ -98,7 +102,7 @@ def default_settings(**kw):
            replay_buffer_size=100, replay_buffer_min_size=10, priority_exponent=0.9, burn_in=40,
            importance_sampling_exponent=0.6, clip_norm=40., value_function_rescaling_epsilon=1e-3, n_steps=5,
            discounting=.997, eval_epsilon=1e-3, num_training_tpus=1, bellman_target='n_step',
-           retrace_lambda=RETRACE_LAMBDA)
+           retrace_lambda=RETRACE_LAMBDA, bootstrap_abandoned=False)
   d.update(kw)
   return R2D2Settings(**d)
 
@@ -164,7 +168,8 @@ def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target
                                                    agent_outputs, gamma, eta=0.9, n_steps=N_STEPS,
                                                    importance_weights=None,
                                                    value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON,
-                                                   bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA):
+                                                   bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA,
+                                                   abandoned=None):
   """reference :258-330.  Returns (loss [B], priorities [B]); the gradient of
   mean(loss * importance_weights) w.r.t. training_agent_output.q_values (reference :604) is
   returned as the third element (the reference gets it from the tape).
@@ -172,7 +177,11 @@ def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target
   bellman_target='n_step' is the reference's rule.  'retrace' (not in the reference) replaces the
   n-step targets by Retrace(retrace_lambda) targets whose target policy is greedy in the online
   network, so the trace is retrace_lambda * 1[replayed action == argmax_a Q_online]; n_steps is then
-  unused (seedrl_r2d2_retrace_loss_fwd_bwd in include/seedrl_b200.h states the targets)."""
+  unused (seedrl_r2d2_retrace_loss_fwd_bwd in include/seedrl_b200.h states the targets).
+
+  abandoned [T,B] (None = none): row i marks the transition into x_i as not real, as
+  advantages.py NStep does; targets reaching it bootstrap from x_{i-1} and transition i-1 adds
+  nothing to the loss (seedrl_r2d2_loss_fwd_bwd_abandoned)."""
   check_bellman_target(bellman_target, retrace_lambda)
   f32 = torch.float32
   q = _lib.require_cuda(training_agent_output.q_values, f32, 'training q_values')
@@ -183,22 +192,35 @@ def compute_loss_and_priorities_from_agent_outputs(training_agent_output, target
   if q.dim() != 3 or tuple(qt.shape) != tuple(q.shape):
     raise ValueError('q_values must be [time, batch, num_actions] for both agents')
   T, B, A = (int(x) for x in q.shape)
+  ab = None
+  if abandoned is not None:
+    ab = _lib.require_cuda(abandoned, torch.bool, 'abandoned')
+    if tuple(ab.shape) != (T, B):
+      raise ValueError('abandoned has shape %s, expected %s' % (tuple(ab.shape), (T, B)))
   w = None if importance_weights is None else _lib.require_cuda(importance_weights, f32, 'importance_weights')
   L = _lib.lib()
   loss = torch.empty(B, dtype=f32, device=q.device); prio = torch.empty_like(loss)
   dq = torch.empty_like(q)
   if bellman_target == 'retrace':
     scratch = torch.empty(int(L.seedrl_r2d2_retrace_loss_scratch_bytes(T, B)), dtype=torch.uint8, device=q.device)
-    _lib.check(L.seedrl_r2d2_retrace_loss_fwd_bwd(
-        T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn), _lib.ptr(w), float(gamma),
-        float(retrace_lambda), float(eta), float(value_function_rescaling_epsilon), _lib.ptr(loss), _lib.ptr(prio),
-        _lib.ptr(dq), _lib.ptr(scratch), _lib.stream_ptr()))
+    tail = (_lib.ptr(w), float(gamma), float(retrace_lambda), float(eta), float(value_function_rescaling_epsilon),
+            _lib.ptr(loss), _lib.ptr(prio), _lib.ptr(dq), _lib.ptr(scratch), _lib.stream_ptr())
+    if ab is None:
+      _lib.check(L.seedrl_r2d2_retrace_loss_fwd_bwd(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew),
+                                                    _lib.ptr(dn), *tail))
+    else:
+      _lib.check(L.seedrl_r2d2_retrace_loss_fwd_bwd_abandoned(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act),
+                                                              _lib.ptr(rew), _lib.ptr(dn), _lib.ptr(ab), *tail))
     return loss, prio, dq
   scratch = torch.empty(int(L.seedrl_r2d2_loss_scratch_bytes(T, B, n_steps)), dtype=torch.uint8, device=q.device)
-  _lib.check(L.seedrl_r2d2_loss_fwd_bwd(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn),
-                                        _lib.ptr(w), float(gamma), int(n_steps), float(eta),
-                                        float(value_function_rescaling_epsilon), _lib.ptr(loss), _lib.ptr(prio),
-                                        _lib.ptr(dq), _lib.ptr(scratch), _lib.stream_ptr()))
+  tail = (_lib.ptr(w), float(gamma), int(n_steps), float(eta), float(value_function_rescaling_epsilon),
+          _lib.ptr(loss), _lib.ptr(prio), _lib.ptr(dq), _lib.ptr(scratch), _lib.stream_ptr())
+  if ab is None:
+    _lib.check(L.seedrl_r2d2_loss_fwd_bwd(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew),
+                                          _lib.ptr(dn), *tail))
+  else:
+    _lib.check(L.seedrl_r2d2_loss_fwd_bwd_abandoned(T, B, A, _lib.ptr(q), _lib.ptr(qt), _lib.ptr(act), _lib.ptr(rew),
+                                                    _lib.ptr(dn), _lib.ptr(ab), *tail))
   return loss, prio, dq
 
 
@@ -245,11 +267,12 @@ def split_structure(structure, prefix_length):
 def compute_loss_and_priorities(training_agent, target_agent, agent_state, prev_actions, env_outputs, agent_outputs,
                                 gamma, burn_in, importance_weights=None, n_steps=N_STEPS,
                                 value_function_rescaling_epsilon=VALUE_FUNCTION_RESCALING_EPSILON,
-                                bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA):
+                                bellman_target='n_step', retrace_lambda=RETRACE_LAMBDA, abandoned=None):
   """reference :333-386.  Time-major inputs with burn_in + unroll_length + 1 rows.  Burn-in
   unrolls update the recurrent state of both networks without gradient (:365-371); the suffix is
   unrolled by the training agent (kept for `backward`) and the target agent.  Returns
-  (loss [B], priorities [B], dq [T_suffix, B, A])."""
+  (loss [B], priorities [B], dq [T_suffix, B, A]).  `abandoned` (None = none) has the rows of
+  env_outputs; its suffix goes to compute_loss_and_priorities_from_agent_outputs."""
   check_bellman_target(bellman_target, retrace_lambda)     # before any network work
   if burn_in:
     (pa_pre, env_pre), (pa_suf, env_suf) = split_structure((prev_actions, tuple(env_outputs)), burn_in)
@@ -264,7 +287,8 @@ def compute_loss_and_priorities(training_agent, target_agent, agent_state, prev_
   return compute_loss_and_priorities_from_agent_outputs(
       training_out, target_out, utils.EnvOutput(*env_suf), AgentOutput(*ao_suf), gamma, n_steps=n_steps,
       importance_weights=importance_weights, value_function_rescaling_epsilon=value_function_rescaling_epsilon,
-      bellman_target=bellman_target, retrace_lambda=retrace_lambda)
+      bellman_target=bellman_target, retrace_lambda=retrace_lambda,
+      abandoned=None if abandoned is None else abandoned[burn_in:])
 
 
 class R2D2LearnerStep(object):
@@ -293,7 +317,7 @@ class R2D2LearnerStep(object):
         self.agent, self.target_agent, u.agent_state, u.prev_actions, u.env_outputs, u.agent_outputs,
         gamma=s.discounting, burn_in=s.burn_in, importance_weights=w, n_steps=s.n_steps,
         value_function_rescaling_epsilon=s.value_function_rescaling_epsilon, bellman_target=s.bellman_target,
-        retrace_lambda=s.retrace_lambda)
+        retrace_lambda=s.retrace_lambda, abandoned=u.env_outputs[3] if s.bootstrap_abandoned else None)
     grads = self.agent.backward(dq)
     if s.clip_norm:
       norm = clip_by_global_norm(grads, s.clip_norm)                 # :606-609 (use_norm = the same norm)

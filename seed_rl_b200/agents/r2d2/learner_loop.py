@@ -61,6 +61,7 @@ class R2D2InferenceHost(inference_host.InferenceHostBase):
         agent, self.num_envs, inference_batch_size, observation_shape, 'int32', agent_state_specs,
         agent_output_specs, s.unroll_length, num_overlapping_steps=s.burn_in, id_limit=self.num_training_envs,
         num_action_repeats=num_action_repeats, device=device, use_graph=cuda_graph,
+        allow_abandoned=s.bootstrap_abandoned,
         info_queue=utils.StructuredFIFOQueue(-1, (TS([], 'int64', 'episode_num_frames'),
                                                   TS([], 'float32', 'episode_returns'),
                                                   TS([], 'float32', 'episode_raw_returns'),
@@ -102,7 +103,7 @@ class R2D2InferenceHost(inference_host.InferenceHostBase):
     _, priorities, _ = learner.compute_loss_and_priorities_from_agent_outputs(
         ao, ao, utils.EnvOutput(*env_suf), ao, s.discounting, n_steps=s.n_steps,
         value_function_rescaling_epsilon=s.value_function_rescaling_epsilon, bellman_target=s.bellman_target,
-        retrace_lambda=s.retrace_lambda)
+        retrace_lambda=s.retrace_lambda, abandoned=env_suf[3] if s.bootstrap_abandoned else None)
     return completed_ids, learner.Unroll(first, priorities, *unrolls)
 
 

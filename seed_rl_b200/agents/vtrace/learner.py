@@ -57,26 +57,31 @@ common_flags.define_once(flags.DEFINE_bool, 'popart', False,
                          'statistics, compensation on).')
 common_flags.define_once(flags.DEFINE_float, 'popart_beta', 1e-2,
                          'Step size of the PopArt moment EMA (EMAMeanStd beta).')
+common_flags.define_once(flags.DEFINE_bool, 'bootstrap_abandoned', False,
+                         'Accept abandoned episodes (EnvOutput.abandoned: a time limit, not the task, ended '
+                         'them) and bootstrap from the value of their last observation instead of '
+                         'treating it as terminal (advantages.py vtrace / NStep).')
 
 FLAGS = flags.FLAGS
 
 LossSettings = collections.namedtuple(
     'LossSettings',
     'discounting lambda_ baseline_cost entropy_cost kl_cost max_abs_reward '
-    'target_entropy entropy_cost_adjustment_speed popart popart_beta', defaults=(False, 1e-2))
+    'target_entropy entropy_cost_adjustment_speed popart popart_beta bootstrap_abandoned',
+    defaults=(False, 1e-2, False))
 
 
 def loss_settings_from_flags():
   return LossSettings(FLAGS.discounting, FLAGS.lambda_, FLAGS.baseline_cost,
                       FLAGS.entropy_cost, FLAGS.kl_cost, FLAGS.max_abs_reward,
                       FLAGS.target_entropy, FLAGS.entropy_cost_adjustment_speed, FLAGS.popart,
-                      FLAGS.popart_beta)
+                      FLAGS.popart_beta, FLAGS.bootstrap_abandoned)
 
 
 def default_loss_settings(**kw):
   d = dict(discounting=.99, lambda_=1., baseline_cost=.5, entropy_cost=0.00025, kl_cost=0.,
            max_abs_reward=0., target_entropy=None, entropy_cost_adjustment_speed=10., popart=False,
-           popart_beta=1e-2)
+           popart_beta=1e-2, bootstrap_abandoned=False)
   d.update(kw)
   return LossSettings(**d)
 
@@ -129,6 +134,16 @@ def _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions, re
   return ll, lb, bl, act, rew, dn, ecp
 
 
+def _abandoned_input(abandoned, shape):
+  """The [T+1,B] abandoned mask as a contiguous CUDA bool tensor, or None."""
+  if abandoned is None:
+    return None
+  ab = _lib.require_cuda(abandoned, torch.bool, 'abandoned')
+  if tuple(ab.shape) != tuple(shape):
+    raise ValueError('abandoned has shape %s, expected %s' % (tuple(ab.shape), tuple(shape)))
+  return ab
+
+
 def _loss_config(settings):
   return _lib.LossConfig(
       settings.discounting, settings.lambda_, settings.baseline_cost, settings.kl_cost,
@@ -150,37 +165,45 @@ def _loss_outputs(ll, lb, want_vtrace):
 
 
 def vtrace_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits,
-                        actions, rewards, done, entropy_cost_param, want_vtrace=False):
+                        actions, rewards, done, entropy_cost_param, want_vtrace=False, abandoned=None):
   """The fused kernel of compute_loss (learner.py:82-157) + its gradient.  All inputs
   have T+1 rows.  Returns dict(loss_terms[16], dlogits, dbaseline, d_entropy_cost_param,
-  vs, pg_advantages)."""
+  vs, pg_advantages).  `abandoned` [T+1,B] (None = none): transition t with abandoned[t+1]
+  bootstraps from V_t instead of being terminal (seedrl_vtrace_loss_fwd_bwd_abandoned)."""
   ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
                                                rewards, done, entropy_cost_param)
+  ab = _abandoned_input(abandoned, dn.shape)
   T1, B, A = (int(x) for x in ll.shape)
   cfg = _loss_config(settings)
   out = _loss_outputs(ll, lb, want_vtrace)
   import ctypes
-  _lib.check(_lib.lib().seedrl_vtrace_loss_fwd_bwd(
-      T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew),
-      _lib.ptr(dn), ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(out['loss_terms']),
-      _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
-      _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']),
-      _lib.ptr(out['pg_advantages']), _lib.ptr(_loss_scratch(T1, B, A, ll.device)),
-      _lib.stream_ptr()))
+  L = _lib.lib()
+  head = (T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn))
+  tail = (ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(out['loss_terms']),
+          _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
+          _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']),
+          _lib.ptr(out['pg_advantages']), _lib.ptr(_loss_scratch(T1, B, A, ll.device)),
+          _lib.stream_ptr())
+  if ab is None:
+    _lib.check(L.seedrl_vtrace_loss_fwd_bwd(*head, *tail))
+  else:
+    _lib.check(L.seedrl_vtrace_loss_fwd_bwd_abandoned(*head, _lib.ptr(ab), *tail))
   return out
 
 
 def popart_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits, actions, rewards,
                         done, entropy_cost_param, popart_moments, popart_compensation, d_popart_compensation,
-                        reduce_moment_sums=None, world=1, want_vtrace=False):
+                        reduce_moment_sums=None, world=1, want_vtrace=False, abandoned=None):
   """compute_loss with PopArt (generalized_onpolicy_loss.py:94-133,169-199 around popart.py and
   EMAMeanStd) + its gradient: seedrl_vtrace_popart_loss_fwd, then `reduce_moment_sums` (in-place
   SUM of the two moment sums across the `world` replicas; None for one replica), then
   seedrl_vtrace_popart_update.  Updates popart_moments (mu1, mu2) and popart_compensation
   (sigma, mu) in place and writes d(loss)/d(sigma, mu) to d_popart_compensation.  Returns what
-  vtrace_loss_fwd_bwd returns; vs and pg_advantages are in return units."""
+  vtrace_loss_fwd_bwd returns; vs and pg_advantages are in return units.  `abandoned` as in
+  vtrace_loss_fwd_bwd."""
   ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
                                                rewards, done, entropy_cost_param)
+  ab = _abandoned_input(abandoned, dn.shape)
   T1, B, A = (int(x) for x in ll.shape)
   f32 = torch.float32
   for t, nm in ((popart_moments, 'popart_moments'), (popart_compensation, 'popart_compensation'),
@@ -197,12 +220,15 @@ def popart_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_lo
   scratch = _loss_scratch(T1, B, A, ll.device)
   import ctypes
   L = _lib.lib()
-  _lib.check(L.seedrl_vtrace_popart_loss_fwd(
-      T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew),
-      _lib.ptr(dn), ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(popart_moments), _lib.ptr(popart_compensation),
-      _lib.ptr(out['loss_terms']), _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
-      _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']), _lib.ptr(out['pg_advantages']),
-      _lib.ptr(td), _lib.ptr(sums), _lib.ptr(scratch), _lib.stream_ptr()))
+  head = (T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn))
+  tail = (ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(popart_moments), _lib.ptr(popart_compensation),
+          _lib.ptr(out['loss_terms']), _lib.ptr(out['dlogits']), _lib.ptr(out['dbaseline']),
+          _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']), _lib.ptr(out['pg_advantages']),
+          _lib.ptr(td), _lib.ptr(sums), _lib.ptr(scratch), _lib.stream_ptr())
+  if ab is None:
+    _lib.check(L.seedrl_vtrace_popart_loss_fwd(*head, *tail))
+  else:
+    _lib.check(L.seedrl_vtrace_popart_loss_fwd_abandoned(*head, _lib.ptr(ab), *tail))
   if reduce_moment_sums is not None:
     reduce_moment_sums(sums)
   _lib.check(L.seedrl_vtrace_popart_update(
@@ -218,8 +244,10 @@ def compute_loss(logger, parametric_action_distribution, agent, agent_state,
   total_loss w.r.t. the network outputs is left on the agent for `minimize`.  With
   settings.popart the agent must have enable_popart()'d: its PopArt state is updated here and
   d(loss)/d(sigma, mu) written to its gradient tail; `reduce_moment_sums` and `world` are the
-  cross-replica sum of popart_loss_fwd_bwd."""
+  cross-replica sum of popart_loss_fwd_bwd.  With settings.bootstrap_abandoned the kernels get
+  env_outputs.abandoned; without it they get no mask."""
   settings = settings or loss_settings_from_flags()
+  ab = {'abandoned': env_outputs[3]} if settings.bootstrap_abandoned else {}   # EnvOutput.abandoned
   learner_outputs, _ = agent(prev_actions, env_outputs, agent_state,
                              unroll=True, is_training=True)                 # :75-79
   if settings.popart:
@@ -229,11 +257,11 @@ def compute_loss(logger, parametric_action_distribution, agent, agent_state,
                             agent_outputs.policy_logits, agent_outputs.action,
                             env_outputs[0], env_outputs[1], agent.entropy_cost_param,
                             agent.popart_moments, agent.popart_compensation, agent.popart_compensation_grad,
-                            reduce_moment_sums, world)
+                            reduce_moment_sums, world, **ab)
   else:
     r = vtrace_loss_fwd_bwd(settings, learner_outputs.policy_logits, learner_outputs.baseline,
                             agent_outputs.policy_logits, agent_outputs.action,
-                            env_outputs[0], env_outputs[1], agent.entropy_cost_param)
+                            env_outputs[0], env_outputs[1], agent.entropy_cost_param, **ab)
   agent._loss_grads = r
   logger = logger or _NullLogger()
   session = logger.log_session()

@@ -38,12 +38,13 @@ class InferenceHost(inference_host.InferenceHostBase):
 
   def __init__(self, agent, num_envs, unroll_length, inference_batch_size, obs_shape,
                num_action_repeats=1, device='cuda', info_queue=None, training_batch_size=None,
-               cuda_graph=None):
+               cuda_graph=None, allow_abandoned=False):
     """training_batch_size: when given, completed unrolls are gathered straight into the columns
     of preallocated time-major training batches (`self.assembler`, utils.BatchAssembler: zero-copy
     minibatch assembly); otherwise they go through the reference's capacity-1 `unroll_queue` of
     single unrolls and `dequeue_batch` stacks them.  cuda_graph: replay the device side of every
-    full batch as one CUDA graph (default: with the assembler); it needs the assembler."""
+    full batch as one CUDA graph (default: with the assembler); it needs the assembler.
+    allow_abandoned: accept abandoned episodes (--bootstrap_abandoned)."""
     TS = utils.TensorSpec
     agent_output_specs = networks.AgentOutput(
         TS([], 'int64', 'action'), TS([agent._num_actions], 'float32', 'policy_logits'),
@@ -57,7 +58,7 @@ class InferenceHost(inference_host.InferenceHostBase):
     super(InferenceHost, self).__init__(
         agent, num_envs, inference_batch_size, obs_shape, 'int64', agent_state_specs, agent_output_specs,
         unroll_length, time_major=True, num_action_repeats=num_action_repeats, device=device,
-        info_queue=info_queue, use_graph=use_graph)
+        info_queue=info_queue, use_graph=use_graph, allow_abandoned=allow_abandoned)
     self.unroll_specs = Unroll(agent_state_specs, *self.store.unroll_specs)
     self.unroll_queue = utils.StructuredFIFOQueue(1, self.unroll_specs)      # capacity 1, :336
     self.assembler = None
@@ -202,7 +203,7 @@ def learner_loop(create_env_fn, create_agent_fn, create_optimizer_fn):
   per_replica = FLAGS.batch_size // world                                   # :422
   host = InferenceHost(agent, FLAGS.num_envs, FLAGS.unroll_length, FLAGS.inference_batch_size,
                        env.observation_space.shape, FLAGS.num_action_repeats, info_queue=info_queue,
-                       training_batch_size=per_replica)
+                       training_batch_size=per_replica, allow_abandoned=FLAGS.bootstrap_abandoned)
   server = grpc.Server([rank_server_address(FLAGS.server_address, rank)])
   server.bind(host.inference)
   server.start()

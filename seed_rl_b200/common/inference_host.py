@@ -27,11 +27,14 @@ class InferenceHostBase(object):
   def __init__(self, agent, num_envs, inference_batch_size, observation_shape, action_dtype,
                agent_state_specs, agent_output_specs, unroll_length, num_overlapping_steps=0,
                time_major=False, id_limit=None, num_action_repeats=1, device='cuda', info_queue=None,
-               use_graph=False):
+               use_graph=False, allow_abandoned=False):
     """id_limit: environments with ids >= id_limit have no store rows (None: every environment has).
     use_graph: replay the device side of every batch of exactly `inference_batch_size` rows as one
-    CUDA graph; other batch sizes run it eagerly."""
+    CUDA graph; other batch sizes run it eagerly.  allow_abandoned: accept rows with
+    `abandoned` set (each must also have `done`: the reset observation after a time limit), for a
+    learner that bootstraps from them; otherwise they raise, as in the reference."""
     self.agent = agent
+    self.allow_abandoned = bool(allow_abandoned)
     self.device = torch.device(device)
     self.N = N = int(inference_batch_size)
     self.num_action_repeats = num_action_repeats
@@ -88,8 +91,13 @@ class InferenceHostBase(object):
   def _begin_batch(self, env_ids, run_ids, env_outputs, raw_rewards):
     """Validation, run-id resets and episode statistics (host tables, plus the rare device resets on
     the current stream).  Invalid batches raise before any table is touched."""
-    if np.asarray(env_outputs.abandoned).any():
-      raise ValueError('Abandoned done states are not supported in %s.' % self.algorithm)
+    abandoned = np.asarray(env_outputs.abandoned, bool)
+    if abandoned.any():
+      if not self.allow_abandoned:
+        raise ValueError('Abandoned done states are not supported in %s.' % self.algorithm)
+      if (abandoned & ~np.asarray(env_outputs.done, bool)).any():
+        raise ValueError('An abandoned step must also be done (env ids %s).' %
+                         np.asarray(env_ids)[abandoned & ~np.asarray(env_outputs.done, bool)])
     utils._check_no_duplicates(None, env_ids, 'inference batch')
     # Reset the environments that had their first run or crashed.
     previous = self.env_run_ids[env_ids]

@@ -163,11 +163,12 @@ extern "C" size_t seedrl_r2d2_loss_scratch_bytes(int T, int B, int n_steps) {
   return (size_t)B * (size_t)(T + n_steps) * sizeof(float);
 }
 
-extern "C" int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
-                                        const int64_t* replay_action, const float* reward, const uint8_t* done,
-                                        const float* importance_weights, float gamma, int n_steps, float eta,
-                                        float value_rescaling_eps, float* loss, float* priorities, float* dq,
-                                        void* scratch, seedrl_stream_t stream) {
+extern "C" int seedrl_r2d2_loss_fwd_bwd_abandoned(int T, int B, int A, const float* q_train, const float* q_target,
+                                                  const int64_t* replay_action, const float* reward,
+                                                  const uint8_t* done, const uint8_t* abandoned,
+                                                  const float* importance_weights, float gamma, int n_steps, float eta,
+                                                  float value_rescaling_eps, float* loss, float* priorities, float* dq,
+                                                  void* scratch, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(T >= 2 && B >= 1 && A >= 1, "need T>=2, B>=1, A>=1");
   SEEDRL_CHECK_ARG(n_steps >= 1 && n_steps <= 8, "n_steps must be in [1, 8]");
   SEEDRL_CHECK_ARG(q_train && q_target && replay_action && reward && done && loss && priorities && dq && scratch,
@@ -178,22 +179,34 @@ extern "C" int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_trai
   p.done = done; p.is_weights = importance_weights; p.gamma = gamma; p.eta = eta; p.eps = value_rescaling_eps;
   for (int k = 0; k < 8; ++k) p.gamma_pow[k] = (float)pow((double)gamma, (double)k);   // fp32(gamma ** k)
   p.loss = loss; p.priorities = priorities; p.dq = dq; p.scratch = reinterpret_cast<float*>(scratch);
+  p.abandoned = abandoned;
   r2d2_loss_kernel<<<ceil_div(B, 64), 64, 0, (cudaStream_t)stream>>>(p);
   count_launch(PC_LOSS, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
 }
 
+extern "C" int seedrl_r2d2_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
+                                        const int64_t* replay_action, const float* reward, const uint8_t* done,
+                                        const float* importance_weights, float gamma, int n_steps, float eta,
+                                        float value_rescaling_eps, float* loss, float* priorities, float* dq,
+                                        void* scratch, seedrl_stream_t stream) {
+  return seedrl_r2d2_loss_fwd_bwd_abandoned(T, B, A, q_train, q_target, replay_action, reward, done, nullptr,
+                                            importance_weights, gamma, n_steps, eta, value_rescaling_eps, loss,
+                                            priorities, dq, scratch, stream);
+}
+
 extern "C" size_t seedrl_r2d2_retrace_loss_scratch_bytes(int T, int B) {
   return (size_t)B * (size_t)T * sizeof(float);
 }
 
-extern "C" int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
-                                                const int64_t* replay_action, const float* reward,
-                                                const uint8_t* done, const float* importance_weights, float gamma,
-                                                float lambda_, float eta, float value_rescaling_eps, float* loss,
-                                                float* priorities, float* dq, void* scratch,
-                                                seedrl_stream_t stream) {
+extern "C" int seedrl_r2d2_retrace_loss_fwd_bwd_abandoned(int T, int B, int A, const float* q_train,
+                                                          const float* q_target, const int64_t* replay_action,
+                                                          const float* reward, const uint8_t* done,
+                                                          const uint8_t* abandoned, const float* importance_weights,
+                                                          float gamma, float lambda_, float eta,
+                                                          float value_rescaling_eps, float* loss, float* priorities,
+                                                          float* dq, void* scratch, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(T >= 2 && B >= 1 && A >= 1, "need T>=2, B>=1, A>=1");
   SEEDRL_CHECK_ARG(lambda_ >= 0.f && lambda_ <= 1.f, "lambda must be in [0, 1]");   // false for NaN
   SEEDRL_CHECK_ARG(q_train && q_target && replay_action && reward && done && loss && priorities && dq && scratch,
@@ -204,10 +217,22 @@ extern "C" int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float
   p.done = done; p.is_weights = importance_weights;
   p.gamma = gamma; p.lambda = lambda_; p.eta = eta; p.eps = value_rescaling_eps;
   p.loss = loss; p.priorities = priorities; p.dq = dq; p.scratch = reinterpret_cast<float*>(scratch);
+  p.abandoned = abandoned;
   r2d2_retrace_loss_kernel<<<ceil_div(B, 64), 64, 0, (cudaStream_t)stream>>>(p);
   count_launch(PC_LOSS, (cudaStream_t)stream);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
+}
+
+extern "C" int seedrl_r2d2_retrace_loss_fwd_bwd(int T, int B, int A, const float* q_train, const float* q_target,
+                                                const int64_t* replay_action, const float* reward,
+                                                const uint8_t* done, const float* importance_weights, float gamma,
+                                                float lambda_, float eta, float value_rescaling_eps, float* loss,
+                                                float* priorities, float* dq, void* scratch,
+                                                seedrl_stream_t stream) {
+  return seedrl_r2d2_retrace_loss_fwd_bwd_abandoned(T, B, A, q_train, q_target, replay_action, reward, done, nullptr,
+                                                    importance_weights, gamma, lambda_, eta, value_rescaling_eps,
+                                                    loss, priorities, dq, scratch, stream);
 }
 
 extern "C" int seedrl_replay_sample(int limit, const float* priorities, float priority_exp,

@@ -180,6 +180,10 @@ struct LossParams {
   const float* pop_comp;  // [2] compensation sigma, mu
   float* pop_td;          // [T,B] (vs - u) / s
   float* pop_sums;        // [2] sum vs, sum vs^2 over this replica's T x B
+  // [T+1,B] or null (= none).  Transition t is masked iff abandoned[t+1]: its delta_t and clipped pg
+  // rho are 0, so vs_t = V_t, pg_adv_t = 0 and vs_{t-1} bootstraps from V_t (done[t+1] already zeroes
+  // the discount, which cuts the trace).  Every other row's arithmetic is unchanged.
+  const uint8_t* abandoned = nullptr;
 };
 
 // ---- PopArt (agents/policy_gradient/modules/popart.py, running_statistics.py EMAMeanStd) ----
@@ -536,6 +540,7 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
   float* s_val = s_dis + rows;                 // [(T+1)*BB]
   int* s_act = reinterpret_cast<int*>(s_val + (T + 1) * BB);  // [rows]
   float* s_red = reinterpret_cast<float*>(s_act + rows);      // [32]
+  uint8_t* s_ab = reinterpret_cast<uint8_t*>(s_red + 32);     // [rows] abandoned[t+1], iff p.abandoned
   const int tid = threadIdx.x;
   const float mul = p.cfg.entropy_cost_adjustment_speed;
   const float ec = expf(mul * __ldg(p.ecp));   // agent.entropy_cost(), learner.py:234
@@ -550,10 +555,12 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
         r = fminf(fmaxf(r, -p.cfg.max_abs_reward), p.cfg.max_abs_reward);
       s_rew[i] = r;
       s_dis[i] = p.done[g1] ? 0.f : p.cfg.discounting;     // :93
+      if (p.abandoned) s_ab[i] = p.abandoned[g1];
       int64_t a = p.act[(size_t)t * B + b0 + c];           // agent_outputs[:-1], :86
       s_act[i] = (int)a;
     } else {
       s_rew[i] = 0.f; s_dis[i] = 0.f; s_act[i] = 0;
+      if (p.abandoned) s_ab[i] = 0;
     }
   }
   float pop_s = 1.f, pop_m = 0.f, pop_sigma = 1.f, pop_mu = 0.f;
@@ -626,6 +633,7 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
     const int c = tid;
     const bool hcr = !isnan(p.cfg.clip_rho_threshold);
     const bool hcp = !isnan(p.cfg.clip_pg_rho_threshold);
+    const bool has_ab = p.abandoned != nullptr;
     const float bootv = s_val[T * BB + c];                 // :82
     float acc = 0.f, vs_next = bootv, v_next = bootv;
     for (int t = T - 1; t >= 0; --t) {
@@ -635,10 +643,11 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
       const float crho = hcr ? fminf(p.cfg.clip_rho_threshold, rho) : rho;
       const float cc = fminf(1.0f, rho) * p.cfg.lambda_;
       const float v = s_val[i], d = s_dis[i], r = s_rew[i];
-      const float delta = crho * (r + d * v_next - v);
+      const bool masked = has_ab && s_ab[i];
+      const float delta = masked ? 0.f : crho * (r + d * v_next - v);
       acc = delta + d * cc * acc;
       const float vs_t = acc + v;
-      const float cpg = hcp ? fminf(p.cfg.clip_pg_rho_threshold, rho) : rho;
+      const float cpg = masked ? 0.f : (hcp ? fminf(p.cfg.clip_pg_rho_threshold, rho) : rho);
       const float pg = cpg * (r + d * vs_next - v);
       vs_next = vs_t;
       v_next = v;
@@ -714,7 +723,8 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
 }
 
 __global__ void __launch_bounds__(kLossThreads) vtrace_loss_kernel(const LossParams p) { loss_small_body<false>(p); }
-__global__ void __launch_bounds__(kLossThreads) vtrace_popart_loss_kernel(const LossParams p) {
+// min 2 CTAs/SM: without it ptxas caps this instantiation at 64 registers and spills in the scan
+__global__ void __launch_bounds__(kLossThreads, 2) vtrace_popart_loss_kernel(const LossParams p) {
   loss_small_body<true>(p);
 }
 
@@ -762,7 +772,7 @@ __device__ __forceinline__ void mbar_wait_or_trap(uint64_t* bar, uint32_t parity
 struct SmallRegs {
   float rew[kStreamRounds], val[kStreamRounds];
   int act[kStreamRounds];
-  uint8_t done[kStreamRounds];
+  uint8_t done[kStreamRounds], ab[kStreamRounds];
 };
 
 // POPART: as in loss_small_body.
@@ -788,6 +798,7 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
   int* s_act = reinterpret_cast<int*>(s_val + (T + 1) * BB);
   float* s_red = reinterpret_cast<float*>(s_act + rows);   // [32]
   uint64_t* s_full = reinterpret_cast<uint64_t*>(s_red + 32);
+  uint8_t* s_ab = reinterpret_cast<uint8_t*>(s_full + 3);   // [rows] abandoned[t+1], iff p.abandoned
   const int tid = threadIdx.x, nthreads = blockDim.x, warp = tid >> 5, lane = tid & 31;
   const float mul = p.cfg.entropy_cost_adjustment_speed;
   const float ec = expf(mul * __ldg(p.ecp));
@@ -844,6 +855,7 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
         if (t < T) {
           r.rew[k] = __ldg(p.rew + g + B);                 // env_outputs[1:], learner.py:87
           r.done[k] = p.done[g + B];
+          if (p.abandoned) r.ab[k] = p.abandoned[g + B];
           r.act[k] = (int)p.act[g];                        // agent_outputs[:-1], :86
         }
       }
@@ -861,6 +873,7 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
             rw = fminf(fmaxf(rw, -p.cfg.max_abs_reward), p.cfg.max_abs_reward);
           s_rew[i] = rw;
           s_dis[i] = r.done[k] ? 0.f : p.cfg.discounting;  // :93
+          if (p.abandoned) s_ab[i] = r.ab[k];
           const int a = r.act[k];
           max_a = fmaxf(max_a, fabsf((float)a));
           s_act[i] = a < 0 ? 0 : (a >= A ? A - 1 : a);
@@ -938,9 +951,10 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
       const float crho = hcr ? fminf(p.cfg.clip_rho_threshold, rho) : rho;
       const float cc = fminf(1.0f, rho) * p.cfg.lambda_;
       const float v = s_val[i], v_next = s_val[i + BB], d = s_dis[i];
-      s_acc[i] = crho * (s_rew[i] + d * v_next - v);       // delta_t, vtrace.py:122
+      const bool masked = p.abandoned && s_ab[i];
+      s_acc[i] = masked ? 0.f : crho * (s_rew[i] + d * v_next - v);   // delta_t, vtrace.py:122
       s_dc[i] = d * cc;
-      s_cpg[i] = hcp ? fminf(p.cfg.clip_pg_rho_threshold, rho) : rho;
+      s_cpg[i] = masked ? 0.f : (hcp ? fminf(p.cfg.clip_pg_rho_threshold, rho) : rho);
       sum_v += v;
     }
     __syncthreads();
@@ -1154,29 +1168,32 @@ vtrace_popart_update_kernel(const PopArtUpdateParams p) {
   }
 }
 
-static size_t loss_smem_bytes(int T, int A, int BB) {
+// has_ab: room for the abandoned mask, rows bytes after the rest
+static size_t loss_smem_bytes(int T, int A, int BB, bool has_ab) {
   const size_t rows = (size_t)T * BB;
-  return (((rows * A + 3) & ~(size_t)3) + rows * 7 + (size_t)(T + 1) * BB + rows + 32) * 4;
+  return (((rows * A + 3) & ~(size_t)3) + rows * 7 + (size_t)(T + 1) * BB + rows + 32) * 4 +
+         (has_ab ? (rows + 3) & ~(size_t)3 : 0);
 }
 
 // Columns per CTA for vtrace_loss_kernel: the largest power of two <= 16 whose tile fits in
 // shared memory, then halved while the grid would leave SMs idle (small B: latency matters,
 // not bandwidth) as long as rows stay float4-copyable.
-static int pick_bb(int T, int B, int A, size_t* smem_bytes) {
+static int pick_bb(int T, int B, int A, bool has_ab, size_t* smem_bytes) {
   int BB = 16;
-  while (BB >= 1 && loss_smem_bytes(T, A, BB) > 200 * 1024) BB >>= 1;
+  while (BB >= 1 && loss_smem_bytes(T, A, BB, has_ab) > 200 * 1024) BB >>= 1;
   if (BB == 0) return 0;
   while (BB > 1 && ceil_div(B, BB) < kNumSMs && (((BB / 2) * A) & 3) == 0) BB >>= 1;
-  *smem_bytes = loss_smem_bytes(T, A, BB);
+  *smem_bytes = loss_smem_bytes(T, A, BB, has_ab);
   return BB;
 }
 
 static int stream_tile_stride_f(int T, int A, int BB) {   // floats per ring buffer, 128-byte multiple
   return (T * BB * A + 31) & ~31;
 }
-static size_t stream_smem_bytes(int T, int A, int BB) {
+static size_t stream_smem_bytes(int T, int A, int BB, bool has_ab) {
   const size_t rows = (size_t)T * BB;
-  return (3 * (size_t)stream_tile_stride_f(T, A, BB) + 9 * rows + (size_t)(T + 1) * BB + rows + 32) * 4 + 3 * 8 + 128;
+  return (3 * (size_t)stream_tile_stride_f(T, A, BB) + 9 * rows + (size_t)(T + 1) * BB + rows + 32) * 4 + 3 * 8 + 128 +
+         (has_ab ? rows : 0);
 }
 
 static int num_sms() {
@@ -1216,7 +1233,7 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
     if (forced_bb > 1 && BB != forced_bb) continue;
     if (B % BB != 0 || ((BB * A) & 3) != 0 || BB * A > 256) continue;
     if (B / BB < num_sms()) continue;
-    const size_t bytes = stream_smem_bytes(T, A, BB);
+    const size_t bytes = stream_smem_bytes(T, A, BB, p.abandoned != nullptr);
     if (bytes > kStreamSmemMax) continue;
     if (pass == 0 && forced_bb <= 1 && 2 * (bytes + 2048 + 1024) > (size_t)228 * 1024) continue;
     const int rows = T * BB;
@@ -1367,7 +1384,7 @@ static int launch_loss(LossParams p, cudaStream_t st) {
       default: SEEDRL_CUDA((launch_stream<0, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;
     }
   } else {
-    p.BB = pick_bb(p.T, B, A, &smem);
+    p.BB = pick_bb(p.T, B, A, p.abandoned != nullptr, &smem);
     SEEDRL_CHECK_ARG(p.BB > 0, "unroll_length * num_actions too large for shared memory");
     small_kernel<<<ceil_div(B, p.BB), kLossThreads, smem, st>>>(p);
   }
@@ -1393,10 +1410,10 @@ static LossParams loss_params(int T1, int B, int A, const float* learner_logits,
   return p;
 }
 
-extern "C" int seedrl_vtrace_loss_fwd_bwd(
+extern "C" int seedrl_vtrace_loss_fwd_bwd_abandoned(
     int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
     const float* behaviour_logits, const int64_t* actions, const float* rewards,
-    const uint8_t* done, const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const uint8_t* done, const uint8_t* abandoned, const seedrl_loss_config* cfg, const float* entropy_cost_param,
     float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
     float* vs_out, float* pg_advantages_out, void* scratch, seedrl_stream_t stream) {
   SEEDRL_CHECK_ARG(T1 >= 2 && B >= 1 && A >= 1, "need T1>=2, B>=1, A>=1");
@@ -1404,17 +1421,29 @@ extern "C" int seedrl_vtrace_loss_fwd_bwd(
                        rewards && done && cfg && entropy_cost_param && loss_terms &&
                        dlogits && dbaseline && d_entropy_cost_param && scratch,
                    "null pointer");
-  return launch_loss<false>(
-      loss_params(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done, cfg,
-                  entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param, vs_out,
-                  pg_advantages_out, scratch),
-      (cudaStream_t)stream);
+  LossParams p = loss_params(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done,
+                             cfg, entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param,
+                             vs_out, pg_advantages_out, scratch);
+  p.abandoned = abandoned;
+  return launch_loss<false>(p, (cudaStream_t)stream);
 }
 
-extern "C" int seedrl_vtrace_popart_loss_fwd(
+extern "C" int seedrl_vtrace_loss_fwd_bwd(
     int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
     const float* behaviour_logits, const int64_t* actions, const float* rewards,
     const uint8_t* done, const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
+    float* vs_out, float* pg_advantages_out, void* scratch, seedrl_stream_t stream) {
+  return seedrl_vtrace_loss_fwd_bwd_abandoned(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions,
+                                              rewards, done, nullptr, cfg, entropy_cost_param, loss_terms, dlogits,
+                                              dbaseline, d_entropy_cost_param, vs_out, pg_advantages_out, scratch,
+                                              stream);
+}
+
+extern "C" int seedrl_vtrace_popart_loss_fwd_abandoned(
+    int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions, const float* rewards,
+    const uint8_t* done, const uint8_t* abandoned, const seedrl_loss_config* cfg, const float* entropy_cost_param,
     const float* popart_moments, const float* popart_compensation,
     float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
     float* vs_out, float* pg_advantages_out, float* td_out, float* moment_sums,
@@ -1430,7 +1459,22 @@ extern "C" int seedrl_vtrace_popart_loss_fwd(
                              vs_out, pg_advantages_out, scratch);
   p.pop_mom = popart_moments; p.pop_comp = popart_compensation;
   p.pop_td = td_out; p.pop_sums = moment_sums;
+  p.abandoned = abandoned;
   return launch_loss<true>(p, (cudaStream_t)stream);
+}
+
+extern "C" int seedrl_vtrace_popart_loss_fwd(
+    int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions, const float* rewards,
+    const uint8_t* done, const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
+    float* vs_out, float* pg_advantages_out, float* td_out, float* moment_sums,
+    void* scratch, seedrl_stream_t stream) {
+  return seedrl_vtrace_popart_loss_fwd_abandoned(
+      T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done, nullptr, cfg,
+      entropy_cost_param, popart_moments, popart_compensation, loss_terms, dlogits, dbaseline, d_entropy_cost_param,
+      vs_out, pg_advantages_out, td_out, moment_sums, scratch, stream);
 }
 
 extern "C" int seedrl_vtrace_popart_update(
