@@ -198,6 +198,47 @@ int seedrl_vtrace_popart_update(
     float* popart_moments, float* popart_compensation, float* dbaseline,
     float* d_popart_compensation, float* loss_terms, void* scratch, seedrl_stream_t stream);
 
+/* Multi-task PopArt (Hessel et al. 2019): K = num_tasks in [1, 64] tasks, each with its own moments and
+ * compensation.  Column b of the batch belongs to task task_ids[b] (int32 [B]); popart_moments and
+ * popart_compensation are [K,2] (row k: task k's (mu1, mu2) and (sigma, mu)).  A learner step is
+ *   seedrl_vtrace_popart_tasks_loss_fwd -> [SUM all-reduce of moment_sums across replicas] ->
+ *   seedrl_vtrace_popart_tasks_update,
+ * which is one seedrl_vtrace_popart_loss_fwd / _update per task on that task's columns, with the loss terms
+ * weighted by the task's share of the rows: entropy, KL and every loss mean still run over all (T1-1) x B
+ * rows, and d_popart_compensation row k = -baseline_cost (sum_k e V, sum_k e) / ((T1-1) B), the sums over
+ * task k's rows.  A task without rows in the summed batch keeps its moments and compensation bit for bit and
+ * gets a zero gradient.  The value output V stays one scalar shared by every task.
+ *
+ * seedrl_vtrace_popart_tasks_loss_fwd: seedrl_vtrace_popart_loss_fwd_abandoned (abandoned may be NULL) with
+ * each column's task state, writing moment_sums float64 [K,3] = (sum vs, sum vs^2, rows) per task.  float64
+ * keeps the row counts exact past 2^24 (8 replicas x T = 100 x B = 65 536 rows is 2^25.6) and their
+ * all-reduce exact.  An id outside [0, K) is not clamped: it sets *task_error (device int32, never cleared
+ * here: the caller zeroes it and polls it when it checks for errors), and that column's outputs are
+ * unspecified.  loss_terms POPART_MEAN and POPART_STD are 0 for K > 1.  With K = 1 every id must be 0, and
+ * the outputs are bit for bit those of seedrl_vtrace_popart_loss_fwd(_abandoned), the sums rounded to fp32
+ * as that entry point rounds them.
+ * seedrl_vtrace_popart_tasks_update: seedrl_vtrace_popart_update per task, counting each task's rows from
+ * the summed moment_sums (replicas may hold different task mixes).
+ * `scratch` holds seedrl_vtrace_popart_tasks_scratch_bytes(T1,B,A,K) bytes, zeroed once, as the loss
+ * scratch; both calls of a step take the same one. */
+size_t seedrl_vtrace_popart_tasks_scratch_bytes(int T1, int B, int A, int num_tasks);
+int seedrl_vtrace_popart_tasks_loss_fwd(
+    int T1, int B, int A,
+    const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions,
+    const float* rewards, const uint8_t* done, const uint8_t* abandoned,
+    const int32_t* task_ids, int num_tasks,
+    const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline,
+    float* d_entropy_cost_param, float* vs_out, float* pg_advantages_out,
+    float* td_out, double* moment_sums, int32_t* task_error, void* scratch, seedrl_stream_t stream);
+int seedrl_vtrace_popart_tasks_update(
+    int T1, int B, int num_tasks, float beta, float baseline_cost,
+    const float* learner_baseline, const float* td, const int32_t* task_ids, const double* moment_sums,
+    float* popart_moments, float* popart_compensation, float* dbaseline,
+    float* d_popart_compensation, float* loss_terms, void* scratch, seedrl_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * (a4) Optimizer apply.  Replaces optimizer.apply_gradients
  * (agents/vtrace/learner.py:272-273) with tf.keras Adam semantics

@@ -93,6 +93,12 @@ SIGNATURES = {
                  P, P, P, P, P, P, P, P, P, P]),
     'seedrl_vtrace_popart_update':
         (c_int, [c_int, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_popart_tasks_scratch_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'seedrl_vtrace_popart_tasks_loss_fwd':
+        (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P, c_int, ctypes.POINTER(LossConfig), P, P, P,
+                 P, P, P, P, P, P, P, P, P, P, P]),
+    'seedrl_vtrace_popart_tasks_update':
+        (c_int, [c_int, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P, P, P, P, P]),
     'seedrl_adam_apply':
         (c_int, [c_size_t, P, P, P, P, c_float, c_float, c_float, c_float, c_float, c_i64,
                  c_float, c_float, P]),

@@ -57,6 +57,10 @@ common_flags.define_once(flags.DEFINE_bool, 'popart', False,
                          'statistics, compensation on).')
 common_flags.define_once(flags.DEFINE_float, 'popart_beta', 1e-2,
                          'Step size of the PopArt moment EMA (EMAMeanStd beta).')
+common_flags.define_once(flags.DEFINE_integer, 'popart_tasks', 1,
+                         'With --popart: the number of tasks K (1 to 64), each with its own PopArt statistics and '
+                         'compensation.  Environment id i belongs to task i % K, as create_env_fn(i, ...) picks '
+                         'levels[i % K].')
 common_flags.define_once(flags.DEFINE_bool, 'bootstrap_abandoned', False,
                          'Accept abandoned episodes (EnvOutput.abandoned: a time limit, not the task, ended '
                          'them) and bootstrap from the value of their last observation instead of '
@@ -67,21 +71,32 @@ FLAGS = flags.FLAGS
 LossSettings = collections.namedtuple(
     'LossSettings',
     'discounting lambda_ baseline_cost entropy_cost kl_cost max_abs_reward '
-    'target_entropy entropy_cost_adjustment_speed popart popart_beta bootstrap_abandoned',
-    defaults=(False, 1e-2, False))
+    'target_entropy entropy_cost_adjustment_speed popart popart_beta bootstrap_abandoned popart_tasks',
+    defaults=(False, 1e-2, False, 1))
+
+MAX_POPART_TASKS = 64
+
+
+def check_loss_settings(settings):
+  """Raises ValueError for a PopArt task count outside [1, 64], or above 1 without PopArt."""
+  K = settings.popart_tasks
+  if not (isinstance(K, int) and 1 <= K <= MAX_POPART_TASKS):
+    raise ValueError('popart_tasks must be an integer in [1, %d], got %r' % (MAX_POPART_TASKS, K))
+  if K > 1 and not settings.popart:
+    raise ValueError('popart_tasks = %d needs popart' % K)
 
 
 def loss_settings_from_flags():
   return LossSettings(FLAGS.discounting, FLAGS.lambda_, FLAGS.baseline_cost,
                       FLAGS.entropy_cost, FLAGS.kl_cost, FLAGS.max_abs_reward,
                       FLAGS.target_entropy, FLAGS.entropy_cost_adjustment_speed, FLAGS.popart,
-                      FLAGS.popart_beta, FLAGS.bootstrap_abandoned)
+                      FLAGS.popart_beta, FLAGS.bootstrap_abandoned, FLAGS.popart_tasks)
 
 
 def default_loss_settings(**kw):
   d = dict(discounting=.99, lambda_=1., baseline_cost=.5, entropy_cost=0.00025, kl_cost=0.,
            max_abs_reward=0., target_entropy=None, entropy_cost_adjustment_speed=10., popart=False,
-           popart_beta=1e-2, bootstrap_abandoned=False)
+           popart_beta=1e-2, bootstrap_abandoned=False, popart_tasks=1)
   d.update(kw)
   return LossSettings(**d)
 
@@ -106,10 +121,13 @@ _POPART_LOG_NAMES = [('PopArt/mean', 'popart_mean'), ('PopArt/std', 'popart_std'
 _scratch_cache = {}
 
 
-def _loss_scratch(T1, B, A, device):
-  key = (T1, B, A, str(device))
+def _loss_scratch(T1, B, A, device, num_tasks=0):
+  """num_tasks > 0: the multi-task PopArt scratch."""
+  key = (T1, B, A, str(device), num_tasks)
   if key not in _scratch_cache:
-    n = int(_lib.lib().seedrl_vtrace_loss_scratch_bytes(T1, B, A))
+    L = _lib.lib()
+    n = int(L.seedrl_vtrace_popart_tasks_scratch_bytes(T1, B, A, num_tasks) if num_tasks
+            else L.seedrl_vtrace_loss_scratch_bytes(T1, B, A))
     _scratch_cache[key] = torch.zeros(n, dtype=torch.uint8, device=device)   # zeroed ONCE
   return _scratch_cache[key]
 
@@ -193,14 +211,24 @@ def vtrace_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_lo
 
 def popart_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits, actions, rewards,
                         done, entropy_cost_param, popart_moments, popart_compensation, d_popart_compensation,
-                        reduce_moment_sums=None, world=1, want_vtrace=False, abandoned=None):
+                        reduce_moment_sums=None, world=1, want_vtrace=False, abandoned=None, task_ids=None,
+                        task_error=None):
   """compute_loss with PopArt (generalized_onpolicy_loss.py:94-133,169-199 around popart.py and
   EMAMeanStd) + its gradient: seedrl_vtrace_popart_loss_fwd, then `reduce_moment_sums` (in-place
   SUM of the two moment sums across the `world` replicas; None for one replica), then
   seedrl_vtrace_popart_update.  Updates popart_moments (mu1, mu2) and popart_compensation
   (sigma, mu) in place and writes d(loss)/d(sigma, mu) to d_popart_compensation.  Returns what
   vtrace_loss_fwd_bwd returns; vs and pg_advantages are in return units.  `abandoned` as in
-  vtrace_loss_fwd_bwd."""
+  vtrace_loss_fwd_bwd.
+
+  With settings.popart_tasks = K > 1: task_ids (int32 CUDA [B], the task of each column) and task_error
+  (int32 CUDA [1], set for an id outside [0, K); zero it once and poll it) are required, the three state
+  tensors are [K,2], and the call is popart_tasks_loss_fwd_bwd.  With K = 1 they are ignored."""
+  if settings.popart_tasks > 1:
+    return popart_tasks_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits, actions,
+                                     rewards, done, entropy_cost_param, popart_moments, popart_compensation,
+                                     d_popart_compensation, task_ids, task_error, reduce_moment_sums,
+                                     want_vtrace, abandoned)
   ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
                                                rewards, done, entropy_cost_param)
   ab = _abandoned_input(abandoned, dn.shape)
@@ -238,14 +266,78 @@ def popart_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_lo
   return out
 
 
+def popart_tasks_loss_fwd_bwd(settings, learner_logits, learner_baseline, behaviour_logits, actions, rewards,
+                              done, entropy_cost_param, popart_moments, popart_compensation, d_popart_compensation,
+                              task_ids, task_error, reduce_moment_sums=None, want_vtrace=False, abandoned=None):
+  """popart_loss_fwd_bwd with K = settings.popart_tasks tasks: seedrl_vtrace_popart_tasks_loss_fwd, then
+  `reduce_moment_sums` (in-place SUM of the float64 [K,3] per-task sums across replicas), then
+  seedrl_vtrace_popart_tasks_update.  Column b is normalised with the state of task task_ids[b]."""
+  ll, lb, bl, act, rew, dn, ecp = _loss_inputs(learner_logits, learner_baseline, behaviour_logits, actions,
+                                               rewards, done, entropy_cost_param)
+  ab = _abandoned_input(abandoned, dn.shape)
+  T1, B, A = (int(x) for x in ll.shape)
+  K = int(settings.popart_tasks)
+  f32 = torch.float32
+  for t, nm in ((popart_moments, 'popart_moments'), (popart_compensation, 'popart_compensation'),
+                (d_popart_compensation, 'd_popart_compensation')):
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == f32 and t.is_contiguous() and
+            tuple(t.shape) == (K, 2)):
+      raise ValueError('%s must be a contiguous float32 CUDA tensor of shape (%d, 2)' % (nm, K))
+  if task_ids is None:
+    raise ValueError('popart_tasks = %d needs the task_ids of the batch columns' % K)
+  tid = _lib.require_cuda(task_ids, torch.int32, 'task_ids')
+  if tuple(tid.shape) != (B,):
+    raise ValueError('task_ids has shape %s, expected (%d,)' % (tuple(tid.shape), B))
+  if not (isinstance(task_error, torch.Tensor) and task_error.is_cuda and task_error.dtype == torch.int32):
+    raise ValueError('task_error must be an int32 CUDA tensor')
+  beta = float(settings.popart_beta)
+  if not 0.0 <= beta <= 1.0:
+    raise ValueError('popart_beta must be in [0, 1], got %r' % beta)
+  cfg = _loss_config(settings)
+  out = _loss_outputs(ll, lb, want_vtrace)
+  td = torch.empty([T1 - 1, B], dtype=f32, device=ll.device)
+  sums = torch.empty([K, 3], dtype=torch.float64, device=ll.device)
+  scratch = _loss_scratch(T1, B, A, ll.device, K)
+  import ctypes
+  L = _lib.lib()
+  _lib.check(L.seedrl_vtrace_popart_tasks_loss_fwd(
+      T1, B, A, _lib.ptr(ll), _lib.ptr(lb), _lib.ptr(bl), _lib.ptr(act), _lib.ptr(rew), _lib.ptr(dn),
+      _lib.ptr(ab), _lib.ptr(tid), K, ctypes.byref(cfg), _lib.ptr(ecp), _lib.ptr(popart_moments),
+      _lib.ptr(popart_compensation), _lib.ptr(out['loss_terms']), _lib.ptr(out['dlogits']),
+      _lib.ptr(out['dbaseline']), _lib.ptr(out['d_entropy_cost_param']), _lib.ptr(out['vs']),
+      _lib.ptr(out['pg_advantages']), _lib.ptr(td), _lib.ptr(sums), _lib.ptr(task_error), _lib.ptr(scratch),
+      _lib.stream_ptr()))
+  if reduce_moment_sums is not None:
+    reduce_moment_sums(sums)
+  _lib.check(L.seedrl_vtrace_popart_tasks_update(
+      T1, B, K, beta, float(settings.baseline_cost), _lib.ptr(lb), _lib.ptr(td), _lib.ptr(tid), _lib.ptr(sums),
+      _lib.ptr(popart_moments), _lib.ptr(popart_compensation), _lib.ptr(out['dbaseline']),
+      _lib.ptr(d_popart_compensation), _lib.ptr(out['loss_terms']), _lib.ptr(scratch), _lib.stream_ptr()))
+  out['moment_sums'] = sums
+  return out
+
+
+def popart_task_logs(popart_moments):
+  """[(name, device scalar)]: 'PopArt/mean/<k>' and 'PopArt/std/<k>' of every task, from the [K,2] moments
+  (the std as the kernels take it: clip(sqrt(mu2 - mu1^2), 1e-6, 1e6), in float64).  No host sync."""
+  m = popart_moments.double()
+  std = (m[:, 1] - m[:, 0] * m[:, 0]).sqrt().clamp(1e-6, 1e6).float()
+  logs = []
+  for k in range(int(popart_moments.shape[0])):
+    logs += [('PopArt/mean/%d' % k, popart_moments[k, 0]), ('PopArt/std/%d' % k, std[k])]
+  return logs
+
+
 def compute_loss(logger, parametric_action_distribution, agent, agent_state,
-                 prev_actions, env_outputs, agent_outputs, settings=None, reduce_moment_sums=None, world=1):
+                 prev_actions, env_outputs, agent_outputs, settings=None, reduce_moment_sums=None, world=1,
+                 task_ids=None):
   """reference learner.py:73-159.  Returns (total_loss, log session).  The gradient of
   total_loss w.r.t. the network outputs is left on the agent for `minimize`.  With
   settings.popart the agent must have enable_popart()'d: its PopArt state is updated here and
   d(loss)/d(sigma, mu) written to its gradient tail; `reduce_moment_sums` and `world` are the
   cross-replica sum of popart_loss_fwd_bwd.  With settings.bootstrap_abandoned the kernels get
-  env_outputs.abandoned; without it they get no mask."""
+  env_outputs.abandoned; without it they get no mask.  With settings.popart_tasks = K > 1, task_ids (int32
+  [B]) gives each column's task and is required; with K = 1 it is ignored."""
   settings = settings or loss_settings_from_flags()
   ab = {'abandoned': env_outputs[3]} if settings.bootstrap_abandoned else {}   # EnvOutput.abandoned
   learner_outputs, _ = agent(prev_actions, env_outputs, agent_state,
@@ -257,7 +349,8 @@ def compute_loss(logger, parametric_action_distribution, agent, agent_state,
                             agent_outputs.policy_logits, agent_outputs.action,
                             env_outputs[0], env_outputs[1], agent.entropy_cost_param,
                             agent.popart_moments, agent.popart_compensation, agent.popart_compensation_grad,
-                            reduce_moment_sums, world, **ab)
+                            reduce_moment_sums, world, task_ids=task_ids,
+                            task_error=getattr(agent, 'popart_task_error', None), **ab)
   else:
     r = vtrace_loss_fwd_bwd(settings, learner_outputs.policy_logits, learner_outputs.baseline,
                             agent_outputs.policy_logits, agent_outputs.action,
@@ -266,8 +359,12 @@ def compute_loss(logger, parametric_action_distribution, agent, agent_state,
   logger = logger or _NullLogger()
   session = logger.log_session()
   lt = r['loss_terms']
-  for name, key in _LOG_NAMES + (_POPART_LOG_NAMES if settings.popart else []):
+  tasks = settings.popart and settings.popart_tasks > 1
+  for name, key in _LOG_NAMES + (_POPART_LOG_NAMES if settings.popart and not tasks else []):
     logger.log(session, name, lt[_lib.LT[key]])
+  if tasks:
+    for name, value in popart_task_logs(agent.popart_moments):
+      logger.log(session, name, value)
   return lt[_lib.LT['total']], session
 
 
@@ -312,6 +409,7 @@ class LearnerStep(object):
     self.optimizer = optimizer
     self.dist = parametric_action_distribution
     self.settings = settings or default_loss_settings()
+    check_loss_settings(self.settings)
     self.logger = logger
     self.pg = process_group
     self.grad_reduce = grad_reduce
@@ -323,7 +421,10 @@ class LearnerStep(object):
     if self.settings.popart and agent.popart_moments is None:
       if optimizer.m is not None:
         raise ValueError('PopArt extends the parameter arena: enable it before the optimizer creates its slots')
-      agent.enable_popart()
+      agent.enable_popart(self.settings.popart_tasks)
+    elif self.settings.popart and agent.popart_tasks != self.settings.popart_tasks:
+      raise ValueError('the agent has %d PopArt tasks; the settings ask for %d'
+                       % (agent.popart_tasks, self.settings.popart_tasks))
     optimizer._create_slots(agent.params)                                        # :244-245
     self.last_loss_terms = None
 
@@ -331,11 +432,12 @@ class LearnerStep(object):
     import torch.distributed as td
     td.all_reduce(sums, op=td.ReduceOp.SUM, group=self.pg)
 
-  def compute_gradients(self, unroll):
+  def compute_gradients(self, unroll, task_ids=None):
+    """task_ids: int32 [B], the task of each column, required with settings.popart_tasks > 1."""
     loss, logs = compute_loss(self.logger, self.dist, self.agent, unroll.agent_state,
                               unroll.prev_actions, unroll.env_outputs, unroll.agent_outputs,
                               self.settings, self._reduce_moment_sums if self.world > 1 else None,
-                              self.world)
+                              self.world, task_ids=task_ids)
     r = self.agent._loss_grads
     self._head_work = None
     if self.world > 1 and self.overlap_reduce and torch.cuda.is_available():
@@ -371,8 +473,8 @@ class LearnerStep(object):
         clamp_index=self.agent.entropy_cost_param_index,
         clamp_lo=-20.0 / mul, clamp_hi=20.0 / mul)                                # :229-231
 
-  def minimize(self, unroll):
-    loss, logs = self.compute_gradients(unroll)
+  def minimize(self, unroll, task_ids=None):
+    loss, logs = self.compute_gradients(unroll, task_ids=task_ids)
     self.apply_gradients()
     self._steps += 1
     if self.check_errors_every and (self._steps == 1 or self._steps % self.check_errors_every == 0):

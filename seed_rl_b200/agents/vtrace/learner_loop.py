@@ -38,13 +38,14 @@ class InferenceHost(inference_host.InferenceHostBase):
 
   def __init__(self, agent, num_envs, unroll_length, inference_batch_size, obs_shape,
                num_action_repeats=1, device='cuda', info_queue=None, training_batch_size=None,
-               cuda_graph=None, allow_abandoned=False):
+               cuda_graph=None, allow_abandoned=False, num_tasks=1):
     """training_batch_size: when given, completed unrolls are gathered straight into the columns
     of preallocated time-major training batches (`self.assembler`, utils.BatchAssembler: zero-copy
     minibatch assembly); otherwise they go through the reference's capacity-1 `unroll_queue` of
     single unrolls and `dequeue_batch` stacks them.  cuda_graph: replay the device side of every
     full batch as one CUDA graph (default: with the assembler); it needs the assembler.
-    allow_abandoned: accept abandoned episodes (--bootstrap_abandoned)."""
+    allow_abandoned: accept abandoned episodes (--bootstrap_abandoned).  num_tasks: the assembler records
+    each column's task, env_id % num_tasks (--popart_tasks)."""
     TS = utils.TensorSpec
     agent_output_specs = networks.AgentOutput(
         TS([], 'int64', 'action'), TS([agent._num_actions], 'float32', 'policy_logits'),
@@ -64,7 +65,7 @@ class InferenceHost(inference_host.InferenceHostBase):
     self.assembler = None
     if training_batch_size:
       self.assembler = utils.BatchAssembler(self.store._specs, agent_state_specs, unroll_length + 1,
-                                            training_batch_size, slots=2, device=device)
+                                            training_batch_size, slots=2, device=device, num_tasks=num_tasks)
 
   def _policy(self, ids32, prev_actions, env_outputs, prev_states, counter):
     return self.agent(prev_actions, env_outputs, prev_states, is_training=False, rng_counter=counter)
@@ -81,6 +82,7 @@ class InferenceHost(inference_host.InferenceHostBase):
       first = self.first_agent_states.read(ids.to(torch.int64))
       for dst, src in zip(self.assembler._states[slot], first):
         dst[col0:col0 + int(ids.numel())].copy_(src)
+      self.assembler.place_task_ids(slot, col0, ids)
     completed_ids, _ = self.store.complete_into(nc, self.assembler, on_placed)
     return completed_ids, None
 
@@ -119,7 +121,8 @@ def save_checkpoint(path, agent, optimizer, extra=None):
 def restore_checkpoint(path, agent, optimizer):
   """ckpt.restore(...).assert_consumed() analogue: raises on a tensor-table mismatch."""
   d = torch.load(path, map_location='cpu', weights_only=False)
-  networks.check_popart_state(d['agent'], getattr(agent, 'popart_moments', None) is not None)
+  networks.check_popart_state(d['agent'], getattr(agent, 'popart_moments', None) is not None,
+                              getattr(agent, 'popart_tasks', 0) or None)
   info = d['agent'].get('param_info')
   if info is not None and [tuple(x) for x in info] != [tuple(x) for x in agent.param_info]:
     raise ValueError('checkpoint %s was written by a different network (tensor table mismatch)' % path)
@@ -203,7 +206,8 @@ def learner_loop(create_env_fn, create_agent_fn, create_optimizer_fn):
   per_replica = FLAGS.batch_size // world                                   # :422
   host = InferenceHost(agent, FLAGS.num_envs, FLAGS.unroll_length, FLAGS.inference_batch_size,
                        env.observation_space.shape, FLAGS.num_action_repeats, info_queue=info_queue,
-                       training_batch_size=per_replica, allow_abandoned=FLAGS.bootstrap_abandoned)
+                       training_batch_size=per_replica, allow_abandoned=FLAGS.bootstrap_abandoned,
+                       num_tasks=settings.popart_tasks if settings.popart else 1)
   server = grpc.Server([rank_server_address(FLAGS.server_address, rank)])
   server.bind(host.inference)
   server.start()
@@ -231,7 +235,7 @@ def learner_loop(create_env_fn, create_agent_fn, create_optimizer_fn):
         save()
         last_ckpt_time = now
       slot, batch = assembled_batch(host.assembler)
-      _, logs = step.minimize(batch)
+      _, logs = step.minimize(batch, task_ids=host.assembler.task_ids(slot))
       host.assembler.release(slot)
       logger.step_end(logs, None, iter_frame_ratio)                         # :280
   finally:

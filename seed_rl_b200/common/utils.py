@@ -277,9 +277,13 @@ class BatchAssembler(object):
   returns it with `release(slot)` once its step is enqueued.  Replaces the reference's
   capacity-1 queue of single unrolls + tf.stack + make_time_major (agents/vtrace/learner.py:336,
   418-432); the back-pressure is the same: with every slot full or in use, `claim` blocks the
-  inference thread."""
+  inference thread.
 
-  def __init__(self, timestep_specs, state_specs, full_length, batch_size, slots=2, device='cuda'):
+  num_tasks = K > 1 (multi-task PopArt) also keeps, per slot, the int32 [B] task of every column: the
+  filling thread records env_id % K for the columns it placed (`place_task_ids`), and `task_ids(slot)`
+  hands them to the learner next to the batch."""
+
+  def __init__(self, timestep_specs, state_specs, full_length, batch_size, slots=2, device='cuda', num_tasks=1):
     self._specs = timestep_specs
     self.batch_size = int(batch_size)
     self.full_length = int(full_length)
@@ -290,6 +294,9 @@ class BatchAssembler(object):
     self._states = [[torch.zeros([batch_size] + list(s.shape), dtype=as_torch_dtype(s.dtype), device=dev)
                      for s in flatten(state_specs)] for _ in range(slots)]
     self._state_specs = state_specs
+    self.num_tasks = int(num_tasks)
+    self._task_ids = ([torch.zeros([batch_size], dtype=torch.int32, device=dev) for _ in range(slots)]
+                      if self.num_tasks > 1 else None)
     self._fill = [0] * slots
     self._free = collections.deque(range(slots))     # slots the inference thread may fill
     self._cur = None
@@ -303,6 +310,16 @@ class BatchAssembler(object):
 
   def state(self, slot):
     return pack_sequence_as(self._state_specs, self._states[slot])
+
+  def place_task_ids(self, slot, col0, env_ids):
+    """Records env_id % num_tasks, on the device, as the task of columns col0.. of `slot`."""
+    if self._task_ids is not None:
+      n = int(env_ids.numel())
+      self._task_ids[slot][col0:col0 + n].copy_(torch.remainder(env_ids, self.num_tasks).to(torch.int32))
+
+  def task_ids(self, slot):
+    """The int32 [B] column tasks of `slot` (None with one task)."""
+    return None if self._task_ids is None else self._task_ids[slot]
 
   def claim(self, want):
     """-> (slot, first free column, columns granted <= want).  Blocks while no slot is free."""

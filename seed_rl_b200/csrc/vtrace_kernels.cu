@@ -184,7 +184,21 @@ struct LossParams {
   // rho are 0, so vs_t = V_t, pg_adv_t = 0 and vs_{t-1} bootstraps from V_t (done[t+1] already zeroes
   // the discount, which cuts the trace).  Every other row's arithmetic is unchanged.
   const uint8_t* abandoned = nullptr;
+  // Multi-task PopArt (seedrl_vtrace_popart_tasks_loss_fwd): column b is normalised with the state of task
+  // task_ids[b]; pop_mom / pop_comp are then [K,2].  An id outside [0, K) sets *task_error and the column
+  // takes the identity state (s = 1, m = 0, sigma = 1, mu = 0).  The tasks kernels write each column's
+  // (sum_t vs, sum_t vs^2) to col_sums [B,2]; vtrace_popart_task_moments_kernel reduces them by task.
+  // The single-task kernels only check the ids when task_ids is set (every id must be 0).
+  const int* task_ids = nullptr;
+  int num_tasks = 0;
+  int* task_error = nullptr;
+  double* col_sums = nullptr;
+  double* pop_sums_d = nullptr;   // single-task kernels: [3] (sum vs, sum vs^2, rows) instead of pop_sums
 };
+
+// loss kernel instantiations
+constexpr int kPlain = 0, kPopArt = 1, kPopArtTasks = 2;
+constexpr int kMaxTasks = 64;
 
 // ---- PopArt (agents/policy_gradient/modules/popart.py, running_statistics.py EMAMeanStd) ----
 // s = clip(sqrt(mu2 - mu1^2), 1e-6, 1e6) (running_statistics.py:149-153), evaluated in float64 and
@@ -196,6 +210,26 @@ __device__ __forceinline__ float popart_std(float mu1, float mu2) {
 // u = s (sigma V + mu) + m: correct_prediction, then unnormalize_prediction (popart.py)
 __device__ __forceinline__ float popart_u(float V, float s, float m, float sigma, float mu) {
   return fmaf(s, fmaf(sigma, V, mu), m);
+}
+
+// Multi-task PopArt: the task of column b, or num_tasks (the identity entry of the kernels' state tables) for
+// an id outside [0, num_tasks), which sets *task_error when `report`.
+__device__ __forceinline__ int task_slot(const int* task_ids, int num_tasks, int* task_error, int b, bool report) {
+  const int id = __ldg(task_ids + b);
+  if ((unsigned)id < (unsigned)num_tasks) return id;
+  if (report) atomicOr(task_error, 1);
+  return num_tasks;
+}
+// (s, m, sigma, mu) of task k (k = num_tasks: the identity)
+__device__ __forceinline__ void task_state(const LossParams& p, int k, float* q) {
+  if (k < p.num_tasks) {
+    q[1] = __ldg(p.pop_mom + 2 * k);
+    q[0] = popart_std(q[1], __ldg(p.pop_mom + 2 * k + 1));
+    q[2] = __ldg(p.pop_comp + 2 * k);
+    q[3] = __ldg(p.pop_comp + 2 * k + 1);
+  } else {
+    q[0] = 1.f; q[1] = 0.f; q[2] = 1.f; q[3] = 0.f;
+  }
 }
 
 __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
@@ -454,8 +488,14 @@ __device__ __forceinline__ void loss_finalize(const LossParams& p, float* s_red,
     s1 = block_reduce_sum_d(s1);
     s2 = block_reduce_sum_d(s2);
     if (tid == 0) {
-      p.pop_sums[0] = (float)s1;
-      p.pop_sums[1] = (float)s2;
+      if (p.pop_sums_d) {   // rounded as pop_sums are, so phase 2 sees the same fp32 sums
+        p.pop_sums_d[0] = (double)(float)s1;
+        p.pop_sums_d[1] = (double)(float)s2;
+        p.pop_sums_d[2] = (double)p.T * (double)p.B;
+      } else {
+        p.pop_sums[0] = (float)s1;
+        p.pop_sums[1] = (float)s2;
+      }
     }
   }
   if (tid == 0) {
@@ -521,10 +561,13 @@ __device__ __forceinline__ void tile_copy(float* s_tile, typename std::condition
 
 // POPART: the values V are replaced by u = s (sigma V + mu) + m before the scan, the policy gradient
 // takes pg_adv / s, and the value loss is left to seedrl_vtrace_popart_update: it gets (vs - u) / s
-// in pop_td and sum vs, sum vs^2 in pop_sums.
-template <bool POPART>
+// in pop_td and sum vs, sum vs^2 in pop_sums.  TASKS: (s, m, sigma, mu) are those of the column's task,
+// and the moment sums go to col_sums per column.
+template <int MODE>
 __device__ __forceinline__ void loss_small_body(const LossParams& p) {
+  constexpr bool POPART = MODE != kPlain, TASKS = MODE == kPopArtTasks;
   extern __shared__ float smem[];
+  __shared__ float s_cpop[TASKS ? 16 * 4 : 1];   // TASKS: (s, m, sigma, mu) of each column (BB <= 16)
   const int T = p.T, B = p.B, A = p.A, BB = p.BB;
   const int b0 = blockIdx.x * BB;
   const int nb = min(BB, B - b0);
@@ -564,15 +607,24 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
     }
   }
   float pop_s = 1.f, pop_m = 0.f, pop_sigma = 1.f, pop_mu = 0.f;
-  if (POPART) {
+  if (TASKS) {
+    if (tid < BB)
+      task_state(p, tid < nb ? task_slot(p.task_ids, p.num_tasks, p.task_error, b0 + tid, true) : p.num_tasks,
+                 s_cpop + tid * 4);
+    __syncthreads();
+  } else if (POPART) {
     pop_m = __ldg(p.pop_mom);
     pop_s = popart_std(pop_m, __ldg(p.pop_mom + 1));
     pop_sigma = __ldg(p.pop_comp);
     pop_mu = __ldg(p.pop_comp + 1);
+    if (p.task_ids && tid < nb && __ldg(p.task_ids + b0 + tid) != 0) atomicOr(p.task_error, 1);
   }
   for (int i = tid; i < (T + 1) * BB; i += kLossThreads) {
     const int t = i / BB, c = i - t * BB;
-    if (POPART)
+    if (TASKS) {
+      const float* q = s_cpop + c * 4;
+      s_val[i] = c < nb ? popart_u(__ldg(p.lb + (size_t)t * B + b0 + c), q[0], q[1], q[2], q[3]) : 0.f;
+    } else if (POPART)
       s_val[i] = c < nb ? popart_u(__ldg(p.lb + (size_t)t * B + b0 + c), pop_s, pop_m, pop_sigma, pop_mu) : 0.f;
     else
       s_val[i] = c < nb ? __ldg(p.lb + (size_t)t * B + b0 + c) : 0.f;
@@ -634,6 +686,7 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
     const bool hcr = !isnan(p.cfg.clip_rho_threshold);
     const bool hcp = !isnan(p.cfg.clip_pg_rho_threshold);
     const bool has_ab = p.abandoned != nullptr;
+    const float cs = TASKS ? s_cpop[c * 4] : pop_s;        // the column's PopArt s
     const float bootv = s_val[T * BB + c];                 // :82
     float acc = 0.f, vs_next = bootv, v_next = bootv;
     for (int t = T - 1; t >= 0; --t) {
@@ -653,12 +706,12 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
       v_next = v;
       const float verr = vs_t - v;                         // :115
       if (POPART) {
-        const float pgn = __fdiv_rn(pg, pop_s);            // generalized_onpolicy_loss.py:129-132
+        const float pgn = __fdiv_rn(pg, cs);               // generalized_onpolicy_loss.py:129-132
         sum_tp += tl * pgn;
         sum_vs += vs_t;
         sum_vs2 += (double)vs_t * vs_t;
         s_tlp[i] = pgn;
-        s_blp[i] = __fdiv_rn(verr, pop_s);
+        s_blp[i] = __fdiv_rn(verr, cs);
       } else {
         sum_tp += tl * pg;                                 // :111-112
         sum_ve2 += verr * verr;                            // :116
@@ -671,6 +724,10 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
       const size_t g = (size_t)t * B + b0 + c;
       if (p.vs_out) p.vs_out[g] = vs_t;
       if (p.pg_out) p.pg_out[g] = pg;
+    }
+    if (TASKS) {   // one thread per column: its sums are the column's
+      p.col_sums[2 * (size_t)(b0 + c)] = sum_vs;
+      p.col_sums[2 * (size_t)(b0 + c) + 1] = sum_vs2;
     }
   }
   __syncthreads();
@@ -715,17 +772,20 @@ __device__ __forceinline__ void loss_small_body(const LossParams& p) {
   r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
   r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  if (POPART) {
+  if (MODE == kPopArt) {
     r = block_reduce_sum_d(sum_vs);  if (tid == 0) part[6] = r;
     r = block_reduce_sum_d(sum_vs2); if (tid == 0) part[7] = r;
   }
-  loss_finalize<POPART>(p, s_red, ec);
+  loss_finalize<MODE == kPopArt>(p, s_red, ec);
 }
 
-__global__ void __launch_bounds__(kLossThreads) vtrace_loss_kernel(const LossParams p) { loss_small_body<false>(p); }
+__global__ void __launch_bounds__(kLossThreads) vtrace_loss_kernel(const LossParams p) { loss_small_body<kPlain>(p); }
 // min 2 CTAs/SM: without it ptxas caps this instantiation at 64 registers and spills in the scan
 __global__ void __launch_bounds__(kLossThreads, 2) vtrace_popart_loss_kernel(const LossParams p) {
-  loss_small_body<true>(p);
+  loss_small_body<kPopArt>(p);
+}
+__global__ void __launch_bounds__(kLossThreads, 2) vtrace_popart_tasks_loss_kernel(const LossParams p) {
+  loss_small_body<kPopArtTasks>(p);
 }
 
 
@@ -775,8 +835,9 @@ struct SmallRegs {
   uint8_t done[kStreamRounds], ab[kStreamRounds];
 };
 
-// POPART: as in loss_small_body.
-template <int AS, bool POPART>
+// POPART, TASKS: as in loss_small_body.  TASKS stages the state of every task in shared memory and
+// takes each column's sums of vs in the scan.
+template <int AS, int MODE>
 __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int ntiles, const int tile_stride_f,
                                                  const CUtensorMap& tm_bl, const CUtensorMap& tm_ll,
                                                  const CUtensorMap& tm_dl) {
@@ -809,10 +870,13 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
   const int bb_sh = 31 - __clz(BB);                      // BB is a power of two
   int lpc = 32;                                          // lanes per column in the scan
   while (lpc > 1 && T <= lpc * 4) lpc >>= 1;
+  constexpr bool POPART = MODE != kPlain, TASKS = MODE == kPopArtTasks;
   __shared__ float s_pop[4];                             // PopArt s, m, sigma, mu
+  __shared__ float s_ptab[TASKS ? (kMaxTasks + 1) * 4 : 1];   // TASKS: (s, m, sigma, mu) by task, then identity
 
+  if (TASKS && tid <= p.num_tasks) task_state(p, tid, s_ptab + tid * 4);
   if (tid == 0) {
-    if (POPART) {
+    if (MODE == kPopArt) {
       s_pop[0] = popart_std(__ldg(p.pop_mom), __ldg(p.pop_mom + 1));
       s_pop[1] = __ldg(p.pop_mom);
       s_pop[2] = __ldg(p.pop_comp);
@@ -858,15 +922,23 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
           if (p.abandoned) r.ab[k] = p.abandoned[g + B];
           r.act[k] = (int)p.act[g];                        // agent_outputs[:-1], :86
         }
+        if (MODE == kPopArt && p.task_ids && t == 0 && __ldg(p.task_ids + tile * BB + c) != 0)
+          atomicOr(p.task_error, 1);
       }
     }
   };
-  auto store_small = [&](const SmallRegs& r) {
+  auto store_small = [&](int tile, const SmallRegs& r) {
 #pragma unroll
     for (int k = 0; k < kStreamRounds; ++k) {
       const int i = tid + k * nthreads;
       if (i < (T + 1) * BB) {
-        s_val[i] = POPART ? popart_u(r.val[k], s_pop[0], s_pop[1], s_pop[2], s_pop[3]) : r.val[k];
+        if (TASKS) {
+          const int c = i & (BB - 1);
+          const float* q = s_ptab + task_slot(p.task_ids, p.num_tasks, p.task_error, tile * BB + c, i < BB) * 4;
+          s_val[i] = popart_u(r.val[k], q[0], q[1], q[2], q[3]);
+        } else {
+          s_val[i] = POPART ? popart_u(r.val[k], s_pop[0], s_pop[1], s_pop[2], s_pop[3]) : r.val[k];
+        }
         if (i < rows) {
           float rw = r.rew[k];
           if (p.cfg.max_abs_reward != 0.f)                 // :90-92
@@ -890,7 +962,7 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
       issue_load(1, &tm_ll, blockIdx.x);
     }
     load_small(blockIdx.x, sm);
-    store_small(sm);
+    store_small(blockIdx.x, sm);
   }
   __syncthreads();
 
@@ -986,11 +1058,27 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
         }
         float acc = __shfl_down_sync(0xffffffffu, Q, 1);
         if (sub == lpc - 1) acc = 0.f;
+        double cs1 = 0.0, cs2 = 0.0;                       // TASKS: this lane's sum of vs, vs^2
         if (live)
           for (int t = t_hi - 1; t >= t_lo; --t) {
             acc = fmaf(s_dc[t * BB + c], acc, s_acc[t * BB + c]);
             s_acc[t * BB + c] = acc;
+            if (TASKS) {
+              const float vs = acc + s_val[t * BB + c];      // phase D's vs, bit for bit
+              cs1 += vs;
+              cs2 += (double)vs * vs;
+            }
           }
+        if (TASKS) {   // the column's lanes, in a fixed tree
+          for (int d = lpc >> 1; d > 0; d >>= 1) {
+            cs1 += __shfl_down_sync(0xffffffffu, cs1, d);
+            cs2 += __shfl_down_sync(0xffffffffu, cs2, d);
+          }
+          if (live && sub == 0) {
+            p.col_sums[2 * ((size_t)tile * BB + c)] = cs1;
+            p.col_sums[2 * ((size_t)tile * BB + c) + 1] = cs2;
+          }
+        }
       }
     }
     __syncthreads();
@@ -1006,10 +1094,14 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
       if (p.vs_out) p.vs_out[g] = verr + v;
       if (p.pg_out) p.pg_out[g] = pg;
       if (POPART) {
-        const float s = s_pop[0], pgn = __fdiv_rn(pg, s), vs = verr + v;   // generalized_onpolicy_loss.py:129-132
+        const float s = TASKS ? s_ptab[task_slot(p.task_ids, p.num_tasks, nullptr, tile * BB + c, false) * 4]
+                              : s_pop[0];
+        const float pgn = __fdiv_rn(pg, s), vs = verr + v;   // generalized_onpolicy_loss.py:129-132
         sum_tp += tl * pgn;
-        sum_vs += vs;
-        sum_vs2 += vs * vs;
+        if (!TASKS) {
+          sum_vs += vs;
+          sum_vs2 += vs * vs;
+        }
         p.pop_td[g] = __fdiv_rn(verr, s);
         row_grad<AS>(tileB + (size_t)i * A, A, s_act[i], s_la[i], s_lb[i], s_ent[i], -(pgn + kc) * invN, ec * invN);
       } else {
@@ -1034,7 +1126,7 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
       for (int e = tid; e < BB * A; e += nthreads) dz[e] = 0.f;
       if (tid < BB) p.dbaseline[(size_t)T * B + (size_t)tile * BB + tid] = 0.f;
     }
-    if (has_next) store_small(sm);   // every read of the per-row arrays is behind the barrier above
+    if (has_next) store_small(next, sm);   // every read of the per-row arrays is behind the barrier above
     __syncthreads();
   }
   if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -1048,11 +1140,11 @@ __device__ __forceinline__ void loss_stream_body(const LossParams& p, const int 
   r = block_reduce_sum_d(sum_kl);  if (tid == 0) part[3] = r;
   r = block_reduce_sum_d(sum_v);   if (tid == 0) part[4] = r;
   r = block_reduce_max(max_a, s_red);   if (tid == 0) part[5] = r;
-  if (POPART) {
+  if (MODE == kPopArt) {
     r = block_reduce_sum_d(sum_vs);  if (tid == 0) part[6] = r;
     r = block_reduce_sum_d(sum_vs2); if (tid == 0) part[7] = r;
   }
-  loss_finalize<POPART>(p, s_red, ec);
+  loss_finalize<MODE == kPopArt>(p, s_red, ec);
 }
 
 template <int AS>
@@ -1060,14 +1152,22 @@ __global__ void __launch_bounds__(kStreamThreadsMax)
 vtrace_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
                           const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_ll,
                           const __grid_constant__ CUtensorMap tm_dl) {
-  loss_stream_body<AS, false>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
+  loss_stream_body<AS, kPlain>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
 }
 template <int AS>
 __global__ void __launch_bounds__(kStreamThreadsMax)
 vtrace_popart_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
                                  const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_ll,
                                  const __grid_constant__ CUtensorMap tm_dl) {
-  loss_stream_body<AS, true>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
+  loss_stream_body<AS, kPopArt>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
+}
+template <int AS>
+__global__ void __launch_bounds__(kStreamThreadsMax)
+vtrace_popart_tasks_loss_stream_kernel(const LossParams p, const int ntiles, const int tile_stride_f,
+                                       const __grid_constant__ CUtensorMap tm_bl,
+                                       const __grid_constant__ CUtensorMap tm_ll,
+                                       const __grid_constant__ CUtensorMap tm_dl) {
+  loss_stream_body<AS, kPopArtTasks>(p, ntiles, tile_stride_f, tm_bl, tm_ll, tm_dl);
 }
 
 // ---------------------------------------------------------------------------
@@ -1091,6 +1191,7 @@ struct PopArtUpdateParams {
   const float* lb;         // [T+1,B] learner baseline V
   const float* td;         // [T,B]
   const float* sums;       // [2]
+  const double* sums_d;    // or [3] (sum vs, sum vs^2, rows), which then give the count
   float* mom;              // [2] mu1, mu2 (in/out)
   float* comp;             // [2] sigma, mu (in/out)
   float* dbaseline;        // rows [0,T)
@@ -1106,7 +1207,9 @@ vtrace_popart_update_kernel(const PopArtUpdateParams p) {
   const int tid = threadIdx.x;
   const float mu1 = p.mom[0], mu2 = p.mom[1], sigma = p.comp[0], mu = p.comp[1];
   // EMAMeanStd.update (running_statistics.py:123-147), in fp32 like the reference's variables
-  const float bm1 = (float)((double)p.sums[0] / p.count), bm2 = (float)((double)p.sums[1] / p.count);
+  const double count = p.sums_d ? p.sums_d[2] : p.count;
+  const float sum1 = p.sums_d ? (float)p.sums_d[0] : p.sums[0], sum2 = p.sums_d ? (float)p.sums_d[1] : p.sums[1];
+  const float bm1 = (float)((double)sum1 / count), bm2 = (float)((double)sum2 / count);
   const float mu1n = __fadd_rn(mu1, __fmul_rn(p.beta, __fsub_rn(bm1, mu1)));
   const float mu2n = __fadd_rn(mu2, __fmul_rn(p.beta, __fsub_rn(bm2, mu2)));
   const float s = popart_std(mu1, mu2), sn = popart_std(mu1n, mu2n);
@@ -1164,6 +1267,212 @@ vtrace_popart_update_kernel(const PopArtUpdateParams p) {
     p.mom[1] = mu2n;
     p.comp[0] = sigma_n;
     p.comp[1] = mu_n;
+    *p.ticket = 0u;
+  }
+}
+
+// ---------------------------------------------------------------------------
+// (a2, multi-task PopArt)  Phase 1 leaves each column's (sum_t vs, sum_t vs^2) in col_sums; this kernel
+// reduces them by task into sums [K,3] = (sum vs, sum vs^2, rows), float64 throughout: the row counts
+// stay exact to 2^53 (a float32 count stops at 2^24 = 8 replicas x T = 100 x B = 20 972), and the
+// cross-replica SUM all-reduce adds them exactly.  Deterministic: a warp adds the columns of each task
+// in lane order (warp_task_sums), each warp keeps its own per-task sums in shared memory in a fixed
+// column order, a CTA adds its warps in order, and the last CTA adds the CTAs in index order.
+constexpr int kTaskThreads = 256;
+constexpr int kTaskPartials = 3 * kMaxTasks;   // doubles per CTA in the moments and update kernels
+
+// Every lane gets the sum of `NV` values over the lanes of the warp whose slot equals its own, added in
+// lane order; returns the mask of those lanes (the lowest one stores the group's sums).
+template <int NV>
+__device__ __forceinline__ unsigned warp_task_sums(int slot, const double* v, double* g) {
+#pragma unroll
+  for (int k = 0; k < NV; ++k) g[k] = 0.0;
+  for (int j = 0; j < 32; ++j) {
+    const int sj = __shfl_sync(0xffffffffu, slot, j);
+#pragma unroll
+    for (int k = 0; k < NV; ++k) {
+      const double x = __shfl_sync(0xffffffffu, v[k], j);
+      if (sj == slot) g[k] += x;
+    }
+  }
+  return __match_any_sync(0xffffffffu, slot);
+}
+
+struct TaskMomentParams {
+  int T, B, K;
+  const int* task_ids;
+  const double* col_sums;  // [B,2]
+  double* sums;            // [K,3]
+  double* partials;        // [grid][kTaskPartials]
+  unsigned int* ticket;
+};
+
+__global__ void __launch_bounds__(kTaskThreads) vtrace_popart_task_moments_kernel(const TaskMomentParams p) {
+  __shared__ double s_acc[kTaskThreads / 32][kMaxTasks][3];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  for (int j = tid; j < (kTaskThreads / 32) * kMaxTasks * 3; j += kTaskThreads) (&s_acc[0][0][0])[j] = 0.0;
+  __syncthreads();
+  for (int base = blockIdx.x * kTaskThreads + warp * 32; base < p.B; base += gridDim.x * kTaskThreads) {
+    const int b = base + lane;
+    // ids were checked (and reported) by phase 1; a column outside [0, K) is left out here
+    const int slot = b < p.B ? task_slot(p.task_ids, p.K, nullptr, b, false) : p.K;
+    double v[2] = {0.0, 0.0}, g[2];
+    if (slot < p.K) {
+      v[0] = p.col_sums[2 * (size_t)b];
+      v[1] = p.col_sums[2 * (size_t)b + 1];
+    }
+    const unsigned grp = warp_task_sums<2>(slot, v, g);
+    if (lane == __ffs(grp) - 1 && slot < p.K) {
+      s_acc[warp][slot][0] += g[0];
+      s_acc[warp][slot][1] += g[1];
+      s_acc[warp][slot][2] += (double)p.T * __popc(grp);
+    }
+  }
+  __syncthreads();
+  double* part = p.partials + (size_t)blockIdx.x * kTaskPartials;
+  for (int j = tid; j < 3 * p.K; j += kTaskThreads) {
+    double a = 0.0;
+    for (int w = 0; w < kTaskThreads / 32; ++w) a += s_acc[w][j / 3][j % 3];
+    part[j] = a;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    s_last = atomicAdd(p.ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  for (int j = tid; j < 3 * p.K; j += kTaskThreads) {
+    double a = 0.0;
+    for (unsigned int g = 0; g < gridDim.x; ++g) a += __ldcg(p.partials + (size_t)g * kTaskPartials + j);
+    p.sums[j] = a;
+  }
+  if (tid == 0) *p.ticket = 0u;
+}
+
+// Phase 2 with tasks: vtrace_popart_update_kernel with each task's own EMA and compensation update, and each
+// row's value error taken with its column's task state.  A task without rows (count 0) keeps its state bit
+// for bit and gets a zero gradient.  One thread per column (its T rows), so a thread's e V and e sums belong
+// to one task; the per-task reduction is the moments kernel's.  Loss means run over all T x B rows.
+struct PopArtTasksUpdateParams {
+  int T, B, K;
+  float baseline_cost, beta;
+  const float* lb;         // [T+1,B]
+  const float* td;         // [T,B]
+  const int* task_ids;     // [B]
+  const double* sums;      // [K,3]
+  float* mom;              // [K,2] (in/out)
+  float* comp;             // [K,2] (in/out)
+  float* dbaseline;
+  float* dcomp;            // [K,2]
+  float* loss_terms;
+  double* partials;        // [grid][kTaskPartials]
+  unsigned int* ticket;
+};
+
+// task k's state after the update: (mu1', mu2', sigma+, mu+) and its (sigma, mu) before
+__device__ __forceinline__ void task_update(const PopArtTasksUpdateParams& p, int k, float* o) {
+  const float mu1 = p.mom[2 * k], mu2 = p.mom[2 * k + 1], sigma = p.comp[2 * k], mu = p.comp[2 * k + 1];
+  const double count = p.sums[3 * k + 2];
+  o[4] = sigma; o[5] = mu;
+  if (count == 0.0) {
+    o[0] = mu1; o[1] = mu2; o[2] = sigma; o[3] = mu;
+    return;
+  }
+  const float bm1 = (float)(p.sums[3 * k] / count), bm2 = (float)(p.sums[3 * k + 1] / count);
+  const float mu1n = __fadd_rn(mu1, __fmul_rn(p.beta, __fsub_rn(bm1, mu1)));
+  const float mu2n = __fadd_rn(mu2, __fmul_rn(p.beta, __fsub_rn(bm2, mu2)));
+  const float s = popart_std(mu1, mu2), sn = popart_std(mu1n, mu2n);
+  o[0] = mu1n; o[1] = mu2n;
+  o[2] = __fmul_rn(__fdiv_rn(s, sn), sigma);
+  o[3] = __fdiv_rn(__fadd_rn(__fsub_rn(mu1, mu1n), __fmul_rn(s, mu)), sn);
+}
+
+__global__ void __launch_bounds__(kPopThreads) vtrace_popart_tasks_update_kernel(const PopArtTasksUpdateParams p) {
+  __shared__ float s_st[kMaxTasks + 1][6];   // task_update's; entry K: identity
+  __shared__ double s_acc[kPopThreads / 32][kMaxTasks][2];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid < p.K) task_update(p, tid, s_st[tid]);
+  if (tid == p.K) {
+    s_st[tid][0] = 0.f; s_st[tid][1] = 1.f;
+    s_st[tid][2] = s_st[tid][4] = 1.f;
+    s_st[tid][3] = s_st[tid][5] = 0.f;
+  }
+  for (int j = tid; j < (kPopThreads / 32) * kMaxTasks * 2; j += kPopThreads) (&s_acc[0][0][0])[j] = 0.0;
+  __syncthreads();
+  const float invN = 1.0f / ((float)p.T * (float)p.B);
+  double se2 = 0.0;
+  for (int base = blockIdx.x * kPopThreads + warp * 32; base < p.B; base += gridDim.x * kPopThreads) {
+    const int b = base + lane;
+    const int slot = b < p.B ? task_slot(p.task_ids, p.K, nullptr, b, false) : p.K;
+    double v[2] = {0.0, 0.0}, g[2];
+    if (b < p.B) {
+      const float sigma_n = s_st[slot][2], mu_n = s_st[slot][3], sigma = s_st[slot][4], mu = s_st[slot][5];
+      for (int t = 0; t < p.T; ++t) {
+        const size_t i = (size_t)t * p.B + b;
+        const float V = __ldg(p.lb + i);
+        const float e = __ldg(p.td + i) + (fmaf(sigma, V, mu) - fmaf(sigma_n, V, mu_n));
+        p.dbaseline[i] = (-p.baseline_cost * e * invN) * sigma_n;
+        se2 += (double)e * e;
+        v[0] += (double)e * V;
+        v[1] += e;
+      }
+    }
+    const unsigned grp = warp_task_sums<2>(slot, v, g);
+    if (lane == __ffs(grp) - 1 && slot < p.K) {
+      s_acc[warp][slot][0] += g[0];
+      s_acc[warp][slot][1] += g[1];
+    }
+  }
+  double* part = p.partials + (size_t)blockIdx.x * kTaskPartials;
+  const double r = block_reduce_sum_d(se2);
+  if (tid == 0) part[2 * kMaxTasks] = r;
+  __syncthreads();
+  for (int j = tid; j < 2 * p.K; j += kPopThreads) {
+    double a = 0.0;
+    for (int w = 0; w < kPopThreads / 32; ++w) a += s_acc[w][j >> 1][j & 1];
+    part[j] = a;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    s_last = atomicAdd(p.ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  const double nn = (double)p.T * (double)p.B;
+  for (int j = tid; j < 2 * p.K; j += kPopThreads) {
+    double a = 0.0;
+    for (unsigned int g = 0; g < gridDim.x; ++g) a += __ldcg(p.partials + (size_t)g * kTaskPartials + j);
+    const int k = j >> 1;
+    // d(bc * 0.5 * mean(e^2)) / d(sigma_k, mu_k) = -bc (sum_k e V, sum_k e) / N; exactly 0 without rows
+    p.dcomp[j] = p.sums[3 * k + 2] == 0.0 ? 0.f : (float)(-(double)p.baseline_cost * a / nn);
+  }
+  double a2 = 0.0;
+  for (unsigned int g = tid; g < gridDim.x; g += blockDim.x) a2 += __ldcg(p.partials + (size_t)g * kTaskPartials + 2 * kMaxTasks);
+  const double tot2 = block_reduce_sum_d(a2);
+  __syncthreads();   // every CTA read mom / comp before it took its ticket; the partial reads above are done
+  if (tid < p.K) {
+    const float* o = s_st[tid];
+    p.mom[2 * tid] = o[0];
+    p.mom[2 * tid + 1] = o[1];
+    p.comp[2 * tid] = o[2];
+    p.comp[2 * tid + 1] = o[3];
+  }
+  if (tid == 0) {
+    const float mse = (float)(tot2 / nn);
+    const float v_loss = p.baseline_cost * 0.5f * mse;
+    float* L = p.loss_terms;
+    L[SEEDRL_LT_V] = v_loss;
+    L[SEEDRL_LT_V_L2_ERROR] = sqrtf(mse);
+    L[SEEDRL_LT_TOTAL] = L[SEEDRL_LT_POLICY] + v_loss + L[SEEDRL_LT_ENTROPY] + L[SEEDRL_LT_KL] +
+                         L[SEEDRL_LT_ENTROPY_ADJ];
+    L[SEEDRL_LT_POPART_MEAN] = 0.f;   // unused with tasks: each task's state is in popart_moments
+    L[SEEDRL_LT_POPART_STD] = 0.f;
     *p.ticket = 0u;
   }
 }
@@ -1234,7 +1543,8 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
     if (B % BB != 0 || ((BB * A) & 3) != 0 || BB * A > 256) continue;
     if (B / BB < num_sms()) continue;
     const size_t bytes = stream_smem_bytes(T, A, BB, p.abandoned != nullptr);
-    if (bytes > kStreamSmemMax) continue;
+    // the tasks kernel's static state table takes from the same 227 KB
+    if (bytes > kStreamSmemMax - (p.task_ids && p.num_tasks > 0 ? (kMaxTasks + 1) * 16 : 0)) continue;
     if (pass == 0 && forced_bb <= 1 && 2 * (bytes + 2048 + 1024) > (size_t)228 * 1024) continue;
     const int rows = T * BB;
     const int rounds = ceil_div(rows, kStreamThreadsMax);
@@ -1248,12 +1558,15 @@ static int pick_stream(const LossParams& p, int forced_bb, int* threads, size_t*
   return 0;
 }
 
-template <int AS, bool POPART>
+template <int AS, int MODE>
 static cudaError_t launch_stream(const LossParams& p, int ntiles, int threads, size_t smem, cudaStream_t stream,
                                  const CUtensorMap& tm_bl, const CUtensorMap& tm_ll, const CUtensorMap& tm_dl) {
-  auto kernel = POPART ? vtrace_popart_loss_stream_kernel<AS> : vtrace_loss_stream_kernel<AS>;
-  const cudaError_t e = POPART ? allow_smem<vtrace_popart_loss_stream_kernel<AS>>((int)kStreamSmemMax)
-                               : allow_smem<vtrace_loss_stream_kernel<AS>>((int)kStreamSmemMax);
+  auto kernel = MODE == kPopArtTasks ? vtrace_popart_tasks_loss_stream_kernel<AS>
+              : MODE == kPopArt      ? vtrace_popart_loss_stream_kernel<AS>
+                                     : vtrace_loss_stream_kernel<AS>;
+  const cudaError_t e = MODE == kPopArtTasks ? allow_smem<vtrace_popart_tasks_loss_stream_kernel<AS>>((int)kStreamSmemMax)
+                      : MODE == kPopArt      ? allow_smem<vtrace_popart_loss_stream_kernel<AS>>((int)kStreamSmemMax)
+                                             : allow_smem<vtrace_loss_stream_kernel<AS>>((int)kStreamSmemMax);
   if (e != cudaSuccess) return e;
   // persistent CTAs: as many per SM as shared memory and threads allow (small T: several,
   // so one CTA's barriers and scan hide behind another's copies)
@@ -1362,12 +1675,16 @@ extern "C" size_t seedrl_vtrace_loss_scratch_bytes(int T1, int B, int A) {
 
 // Picks the kernel form (TMA-streamed at large aligned B, else vtrace_loss_kernel) and launches it;
 // p has everything but BB.
-template <bool POPART>
+template <int MODE>
 static int launch_loss(LossParams p, cudaStream_t st) {
   const int T1 = p.T + 1, B = p.B, A = p.A;
   size_t smem = 0;
-  auto small_kernel = POPART ? vtrace_popart_loss_kernel : vtrace_loss_kernel;
-  SEEDRL_CUDA(POPART ? allow_smem<vtrace_popart_loss_kernel>(200 * 1024) : allow_smem<vtrace_loss_kernel>(200 * 1024));
+  auto small_kernel = MODE == kPopArtTasks ? vtrace_popart_tasks_loss_kernel
+                    : MODE == kPopArt      ? vtrace_popart_loss_kernel
+                                           : vtrace_loss_kernel;
+  SEEDRL_CUDA(MODE == kPopArtTasks ? allow_smem<vtrace_popart_tasks_loss_kernel>(200 * 1024)
+              : MODE == kPopArt    ? allow_smem<vtrace_popart_loss_kernel>(200 * 1024)
+                                   : allow_smem<vtrace_loss_kernel>(200 * 1024));
   int threads = 0;
   p.BB = g_loss_stream_enabled ? pick_stream(p, g_loss_stream_enabled, &threads, &smem) : 0;
   alignas(64) CUtensorMap tm_bl, tm_ll, tm_dl;
@@ -1378,10 +1695,10 @@ static int launch_loss(LossParams p, cudaStream_t st) {
   if (p.BB > 0) {
     const int ntiles = B / p.BB;
     switch (A) {   // compile-time action counts of the reference's environments
-      case 9:  SEEDRL_CUDA((launch_stream<9, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;    // DMLab
-      case 18: SEEDRL_CUDA((launch_stream<18, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // Atari
-      case 19: SEEDRL_CUDA((launch_stream<19, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // football
-      default: SEEDRL_CUDA((launch_stream<0, POPART>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;
+      case 9:  SEEDRL_CUDA((launch_stream<9, MODE>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;    // DMLab
+      case 18: SEEDRL_CUDA((launch_stream<18, MODE>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // Atari
+      case 19: SEEDRL_CUDA((launch_stream<19, MODE>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;   // football
+      default: SEEDRL_CUDA((launch_stream<0, MODE>(p, ntiles, threads, smem, st, tm_bl, tm_ll, tm_dl))); break;
     }
   } else {
     p.BB = pick_bb(p.T, B, A, p.abandoned != nullptr, &smem);
@@ -1425,7 +1742,7 @@ extern "C" int seedrl_vtrace_loss_fwd_bwd_abandoned(
                              cfg, entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param,
                              vs_out, pg_advantages_out, scratch);
   p.abandoned = abandoned;
-  return launch_loss<false>(p, (cudaStream_t)stream);
+  return launch_loss<kPlain>(p, (cudaStream_t)stream);
 }
 
 extern "C" int seedrl_vtrace_loss_fwd_bwd(
@@ -1460,7 +1777,7 @@ extern "C" int seedrl_vtrace_popart_loss_fwd_abandoned(
   p.pop_mom = popart_moments; p.pop_comp = popart_compensation;
   p.pop_td = td_out; p.pop_sums = moment_sums;
   p.abandoned = abandoned;
-  return launch_loss<true>(p, (cudaStream_t)stream);
+  return launch_loss<kPopArt>(p, (cudaStream_t)stream);
 }
 
 extern "C" int seedrl_vtrace_popart_loss_fwd(
@@ -1477,6 +1794,17 @@ extern "C" int seedrl_vtrace_popart_loss_fwd(
       vs_out, pg_advantages_out, td_out, moment_sums, scratch, stream);
 }
 
+// at most kNumSMs CTAs: their partials fit the kNumSMs x kLossPartials doubles that
+// seedrl_vtrace_loss_scratch_bytes always provides
+static int launch_popart_update(const PopArtUpdateParams& p, cudaStream_t st) {
+  const size_t n = (size_t)p.T * p.B;
+  const int grid = (int)std::min<size_t>(ceil_div_sz(n, (size_t)kPopThreads * 4), (size_t)kNumSMs);
+  vtrace_popart_update_kernel<<<grid, kPopThreads, 0, st>>>(p);
+  count_launch(PC_LOSS, st);
+  SEEDRL_CHECK_LAUNCH();
+  return SEEDRL_OK;
+}
+
 extern "C" int seedrl_vtrace_popart_update(
     int T1, int B, int world, float beta, float baseline_cost, const float* learner_baseline,
     const float* td, const float* moment_sums, float* popart_moments, float* popart_compensation,
@@ -1487,7 +1815,7 @@ extern "C" int seedrl_vtrace_popart_update(
   SEEDRL_CHECK_ARG(learner_baseline && td && moment_sums && popart_moments && popart_compensation &&
                        dbaseline && d_popart_compensation && loss_terms && scratch,
                    "null pointer");
-  PopArtUpdateParams p;
+  PopArtUpdateParams p = {};
   p.T = T1 - 1; p.B = B;
   p.baseline_cost = baseline_cost; p.beta = beta;
   p.count = (double)world * (double)p.T * (double)B;
@@ -1496,12 +1824,97 @@ extern "C" int seedrl_vtrace_popart_update(
   p.dbaseline = dbaseline; p.dcomp = d_popart_compensation; p.loss_terms = loss_terms;
   p.ticket = reinterpret_cast<unsigned int*>(scratch);
   p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
-  // at most kNumSMs CTAs: their partials fit the kNumSMs x kLossPartials doubles that
-  // seedrl_vtrace_loss_scratch_bytes always provides
-  const size_t n = (size_t)p.T * B;
-  const int grid = (int)std::min<size_t>(ceil_div_sz(n, (size_t)kPopThreads * 4), (size_t)kNumSMs);
-  vtrace_popart_update_kernel<<<grid, kPopThreads, 0, (cudaStream_t)stream>>>(p);
-  count_launch(PC_LOSS, (cudaStream_t)stream);
+  return launch_popart_update(p, (cudaStream_t)stream);
+}
+
+// ---- multi-task PopArt ----------------------------------------------------------------------------------
+// Scratch: the loss scratch, then col_sums [B,2] doubles, then kNumSMs x kTaskPartials doubles for the
+// moments and update kernels (at most kNumSMs CTAs each).
+extern "C" size_t seedrl_vtrace_popart_tasks_scratch_bytes(int T1, int B, int A, int num_tasks) {
+  (void)num_tasks;
+  return seedrl_vtrace_loss_scratch_bytes(T1, B, A) + (size_t)B * 2 * sizeof(double) +
+         (size_t)kNumSMs * kTaskPartials * sizeof(double);
+}
+static double* task_col_sums(void* scratch, int B) {   // the loss scratch depends on B alone
+  return reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + seedrl_vtrace_loss_scratch_bytes(2, B, 1));
+}
+
+extern "C" int seedrl_vtrace_popart_tasks_loss_fwd(
+    int T1, int B, int A, const float* learner_logits, const float* learner_baseline,
+    const float* behaviour_logits, const int64_t* actions, const float* rewards,
+    const uint8_t* done, const uint8_t* abandoned, const int32_t* task_ids, int num_tasks,
+    const seedrl_loss_config* cfg, const float* entropy_cost_param,
+    const float* popart_moments, const float* popart_compensation,
+    float* loss_terms, float* dlogits, float* dbaseline, float* d_entropy_cost_param,
+    float* vs_out, float* pg_advantages_out, float* td_out, double* moment_sums, int32_t* task_error,
+    void* scratch, seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(T1 >= 2 && B >= 1 && A >= 1, "need T1>=2, B>=1, A>=1");
+  SEEDRL_CHECK_ARG(num_tasks >= 1 && num_tasks <= kMaxTasks, "num_tasks must be in [1, 64]");
+  SEEDRL_CHECK_ARG(learner_logits && learner_baseline && behaviour_logits && actions &&
+                       rewards && done && task_ids && cfg && entropy_cost_param && popart_moments &&
+                       popart_compensation && loss_terms && dlogits && dbaseline &&
+                       d_entropy_cost_param && td_out && moment_sums && task_error && scratch,
+                   "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  LossParams p = loss_params(T1, B, A, learner_logits, learner_baseline, behaviour_logits, actions, rewards, done,
+                             cfg, entropy_cost_param, loss_terms, dlogits, dbaseline, d_entropy_cost_param,
+                             vs_out, pg_advantages_out, scratch);
+  p.pop_mom = popart_moments; p.pop_comp = popart_compensation;
+  p.pop_td = td_out;
+  p.abandoned = abandoned;
+  p.task_ids = task_ids; p.task_error = task_error;
+  if (num_tasks == 1) {   // the single-task kernels: bit for bit seedrl_vtrace_popart_loss_fwd(_abandoned)
+    p.pop_sums_d = moment_sums;
+    return launch_loss<kPopArt>(p, st);
+  }
+  p.num_tasks = num_tasks;
+  p.col_sums = task_col_sums(scratch, B);
+  SEEDRL_TRY(launch_loss<kPopArtTasks>(p, st));
+  TaskMomentParams q;
+  q.T = p.T; q.B = B; q.K = num_tasks;
+  q.task_ids = task_ids; q.col_sums = p.col_sums; q.sums = moment_sums;
+  q.partials = p.col_sums + 2 * (size_t)B;
+  q.ticket = p.ticket;
+  vtrace_popart_task_moments_kernel<<<std::min(kNumSMs, ceil_div(B, kTaskThreads)), kTaskThreads, 0, st>>>(q);
+  count_launch(PC_LOSS, st);
+  SEEDRL_CHECK_LAUNCH();
+  return SEEDRL_OK;
+}
+
+extern "C" int seedrl_vtrace_popart_tasks_update(
+    int T1, int B, int num_tasks, float beta, float baseline_cost, const float* learner_baseline,
+    const float* td, const int32_t* task_ids, const double* moment_sums, float* popart_moments,
+    float* popart_compensation, float* dbaseline, float* d_popart_compensation, float* loss_terms,
+    void* scratch, seedrl_stream_t stream) {
+  SEEDRL_CHECK_ARG(T1 >= 2 && B >= 1, "need T1>=2, B>=1");
+  SEEDRL_CHECK_ARG(num_tasks >= 1 && num_tasks <= kMaxTasks, "num_tasks must be in [1, 64]");
+  SEEDRL_CHECK_ARG(beta >= 0.f && beta <= 1.f, "beta must be in [0, 1]");
+  SEEDRL_CHECK_ARG(learner_baseline && td && task_ids && moment_sums && popart_moments && popart_compensation &&
+                       dbaseline && d_popart_compensation && loss_terms && scratch,
+                   "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch);
+  if (num_tasks == 1) {   // vtrace_popart_update_kernel, counting the rows from moment_sums
+    PopArtUpdateParams p = {};
+    p.T = T1 - 1; p.B = B;
+    p.baseline_cost = baseline_cost; p.beta = beta;
+    p.lb = learner_baseline; p.td = td; p.sums_d = moment_sums;
+    p.mom = popart_moments; p.comp = popart_compensation;
+    p.dbaseline = dbaseline; p.dcomp = d_popart_compensation; p.loss_terms = loss_terms;
+    p.ticket = ticket;
+    p.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
+    return launch_popart_update(p, st);
+  }
+  PopArtTasksUpdateParams p;
+  p.T = T1 - 1; p.B = B; p.K = num_tasks;
+  p.baseline_cost = baseline_cost; p.beta = beta;
+  p.lb = learner_baseline; p.td = td; p.task_ids = task_ids; p.sums = moment_sums;
+  p.mom = popart_moments; p.comp = popart_compensation;
+  p.dbaseline = dbaseline; p.dcomp = d_popart_compensation; p.loss_terms = loss_terms;
+  p.partials = task_col_sums(scratch, B) + 2 * (size_t)B;
+  p.ticket = ticket;
+  vtrace_popart_tasks_update_kernel<<<std::min(kNumSMs, ceil_div(B, kPopThreads)), kPopThreads, 0, st>>>(p);
+  count_launch(PC_LOSS, st);
   SEEDRL_CHECK_LAUNCH();
   return SEEDRL_OK;
 }

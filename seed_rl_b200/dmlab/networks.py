@@ -176,34 +176,61 @@ class _CudaAgent(CudaNet):
     return torch.exp(self._entropy_mul * self.entropy_cost_param)
 
   # ---- PopArt (popart.py; the V-trace learner's --popart) ---------------------------
-  popart_moments = None    # [2] EMA moments (mu1, mu2): a device buffer of their own, not trained
+  popart_moments = None    # [2] EMA moments (mu1, mu2), [K,2] with K tasks: a device buffer of their own, not trained
+  popart_tasks = 0         # K once enable_popart() ran
+  popart_task_error = None  # K > 1: device int32 flag, set by the loss kernel for a task id outside [0, K)
 
-  def enable_popart(self):
-    """Appends the trained compensation (sigma, mu) = (1, 0) after entropy_cost_param, in a 64-float
-    tail of the parameter and gradient arenas (so Adam and the gradient all-reduce take them with
-    everything else), and creates the moments (0, 1).  The network's own arena, its offsets and
-    grad_split are unchanged.  Call before an optimizer creates its slots and before anything keeps
-    a pointer to `params` (inference hosts, CUDA graphs): both arenas are reallocated."""
+  def enable_popart(self, num_tasks=1):
+    """Appends the trained compensation (sigma, mu) = (1, 0) after entropy_cost_param, in a tail of
+    the parameter and gradient arenas (so Adam and the gradient all-reduce take them with everything
+    else), and creates the moments (0, 1).  With num_tasks = K > 1 every task has its own pair of each:
+    the compensation is a [K,2] view of the tail and the moments are [K,2].  The tail holds 2K floats
+    rounded up to 64.  The network's own arena, its offsets and grad_split are unchanged.  Call before an
+    optimizer creates its slots and before anything keeps a pointer to `params` (inference hosts, CUDA
+    graphs): both arenas are reallocated."""
+    K = int(num_tasks)
+    if not 1 <= K <= MAX_POPART_TASKS:
+      raise ValueError('num_tasks must be in [1, %d], got %r' % (MAX_POPART_TASKS, num_tasks))
     if self.popart_moments is not None:
+      if K != self.popart_tasks:
+        raise ValueError('PopArt is enabled with %d tasks, not %d' % (self.popart_tasks, K))
       return
     off = self.arena_floats
-    params = torch.zeros(off + 64, dtype=torch.float32, device=self.device)
+    params = torch.zeros(off + -(-2 * K // 64) * 64, dtype=torch.float32, device=self.device)
     params[:off].copy_(self.params)
-    params[off] = 1.0
+    params[off:off + 2 * K:2] = 1.0
     self.params, self.grads = params, torch.zeros_like(params)
-    self.param_info = self.param_info + [('popart/compensation_std', (), off), ('popart/compensation_mean', (), off + 1)]
-    self.popart_moments = torch.tensor([0.0, 1.0], dtype=torch.float32, device=self.device)
+    if K == 1:
+      self.param_info = self.param_info + [('popart/compensation_std', (), off),
+                                           ('popart/compensation_mean', (), off + 1)]
+      self.popart_moments = torch.tensor([0.0, 1.0], dtype=torch.float32, device=self.device)
+    else:
+      for k in range(K):
+        self.param_info = self.param_info + [('popart/compensation_std/%d' % k, (), off + 2 * k),
+                                             ('popart/compensation_mean/%d' % k, (), off + 2 * k + 1)]
+      self.popart_moments = torch.tensor([[0.0, 1.0]] * K, dtype=torch.float32, device=self.device)
+      self.popart_task_error = torch.zeros(1, dtype=torch.int32, device=self.device)
+    self.popart_tasks = K
 
   @property
   def popart_compensation(self):
-    """(sigma, mu): a view of the parameter arena."""
-    off = self.arena_floats
-    return self.params[off:off + 2]
+    """(sigma, mu), [K,2] with K > 1 tasks: a view of the parameter arena."""
+    return self._popart_tail(self.params)
 
   @property
   def popart_compensation_grad(self):
-    off = self.arena_floats
-    return self.grads[off:off + 2]
+    return self._popart_tail(self.grads)
+
+  def _popart_tail(self, arena):
+    off, K = self.arena_floats, self.popart_tasks
+    return arena[off:off + 2] if K == 1 else arena[off:off + 2 * K].view(K, 2)
+
+  def check_errors(self):
+    """CudaNet.check_errors, and with K > 1 PopArt tasks, whether a task id outside [0, K) reached the
+    loss since the agent was created."""
+    super(_CudaAgent, self).check_errors()
+    if self.popart_task_error is not None and int(self.popart_task_error.item()) != 0:
+      raise RuntimeError('a task id outside [0, %d) reached the multi-task PopArt loss' % self.popart_tasks)
 
   def state_dict(self):
     d = super(_CudaAgent, self).state_dict()
@@ -212,19 +239,34 @@ class _CudaAgent(CudaNet):
     return d
 
   def load_state_dict(self, d):
-    check_popart_state(d, self.popart_moments is not None)
+    check_popart_state(d, self.popart_moments is not None, self.popart_tasks)
     super(_CudaAgent, self).load_state_dict(d)
     if self.popart_moments is not None:
       self.popart_moments.copy_(d['popart_moments'].to(self.device))
 
 
-def check_popart_state(agent_state, popart):
-  """Raises ValueError when a checkpoint's agent state and a learner disagree on PopArt."""
+MAX_POPART_TASKS = 64
+
+
+def popart_tasks_of(agent_state):
+  """The PopArt task count of a checkpoint's agent state (0: written without PopArt)."""
+  m = agent_state.get('popart_moments')
+  if m is None:
+    return 0
+  return 1 if m.dim() == 1 else int(m.shape[0])
+
+
+def check_popart_state(agent_state, popart, num_tasks=None):
+  """Raises ValueError when a checkpoint's agent state and a learner disagree on PopArt, or, given the
+  learner's num_tasks, on its task count."""
   has = 'popart_moments' in agent_state
   if has and not popart:
     raise ValueError('the checkpoint was written with PopArt (--popart); this learner runs without it')
   if popart and not has:
     raise ValueError('the checkpoint was written without PopArt; this learner runs with --popart')
+  if has and num_tasks is not None and popart_tasks_of(agent_state) != num_tasks:
+    raise ValueError('the checkpoint was written with %d PopArt tasks (--popart_tasks); this learner runs with %d'
+                     % (popart_tasks_of(agent_state), num_tasks))
 
 
 class ImpalaDeep(_CudaAgent):

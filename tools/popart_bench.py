@@ -7,6 +7,10 @@
                 loss kernel (seedrl_vtrace_loss_fwd_bwd), PopArt phase 1 (seedrl_vtrace_popart_loss_fwd) and
                 phase 2 (seedrl_vtrace_popart_update), each called through ctypes on preallocated buffers and
                 timed as the mean of 20 back-to-back launches between one pair of events, after 3 warm-ups.
+  multi-task:   the same learner step with --popart_tasks 30 (column b in task b % 30) in the same alternating
+                rounds, and the multi-task phases (seedrl_vtrace_popart_tasks_loss_fwd, which includes the
+                per-task moment reduction, and seedrl_vtrace_popart_tasks_update) at K = 30 over the same sweep,
+                next to the single-task (K = 1) phases.
 The card's name, power limit and maximum SM clock are read in the same run.
 
   python tools/popart_bench.py [--steps 10] [--rounds 5]
@@ -63,25 +67,32 @@ def events_ms(fn, n):
   return e0.elapsed_time(e1) / n
 
 
+TASKS = 30
+
+
 def learner_steps(steps, rounds):
   un = unroll(64)
+  ids = (torch.arange(64, device='cuda') % TASKS).to(torch.int32)
+  arms = {'off': dict(popart=False), 'on': dict(popart=True), 'tasks': dict(popart=True, popart_tasks=TASKS)}
   runs = {}
-  for popart in (False, True):
+  for name, kw in arms.items():
     agent = networks.ImpalaDeep(A, seed=0, conv_mode='tc3p', lstm_mode='tc3')
     step = learner.LearnerStep(agent, optimizers.Adam(4.8e-4, beta_1=0.0, epsilon=3.125e-7),
-                               settings=learner.default_loss_settings(popart=popart), check_errors_every=0)
+                               settings=learner.default_loss_settings(**kw), check_errors_every=0)
     for _ in range(3):
-      step.minimize(un)
-    runs[popart] = step
-  times = {False: [], True: []}
+      step.minimize(un, task_ids=ids)
+    runs[name] = step
+  times = dict((k, []) for k in arms)
   for _ in range(rounds):
-    for popart in (False, True):
-      times[popart].append(events_ms(lambda: runs[popart].minimize(un), steps))
+    for name in arms:
+      times[name].append(events_ms(lambda: runs[name].minimize(un, task_ids=ids), steps))
   for s in runs.values():
     s.agent.check_errors()
   med = {k: float(np.median(v)) for k, v in times.items()}
-  return {'ms_per_step_off': med[False], 'ms_per_step_on': med[True], 'rounds_off': times[False],
-          'rounds_on': times[True], 'on_minus_off_ms': med[True] - med[False]}
+  return {'ms_per_step_off': med['off'], 'ms_per_step_on': med['on'], 'rounds_off': times['off'],
+          'rounds_on': times['on'], 'on_minus_off_ms': med['on'] - med['off'],
+          'ms_per_step_tasks%d' % TASKS: med['tasks'], 'rounds_tasks%d' % TASKS: times['tasks'],
+          'tasks_minus_on_ms': med['tasks'] - med['on']}
 
 
 def kernels():
@@ -122,11 +133,31 @@ def kernels():
       _lib.check(L.seedrl_vtrace_popart_update(
           T1, B, 1, 1e-2, 0.5, P(lb), P(td), P(sums), P(mom), P(comp), P(o['dbaseline']), P(dcomp),
           P(o['loss_terms']), P(scratch), _lib.stream_ptr()))
+
+    ids = (torch.arange(B, device='cuda') % TASKS).to(torch.int32)
+    kmom = torch.tensor([[0.0, 1.0]] * TASKS, device='cuda'); kcomp = torch.tensor([[1.0, 0.0]] * TASKS, device='cuda')
+    kdcomp = torch.zeros(TASKS, 2, device='cuda')
+    ksums = torch.empty(TASKS, 3, dtype=torch.float64, device='cuda')
+    kerr = torch.zeros(1, dtype=torch.int32, device='cuda')
+    kscratch = learner._loss_scratch(T1, B, A, ll.device, TASKS)
+
+    def tasks_phase1():
+      _lib.check(L.seedrl_vtrace_popart_tasks_loss_fwd(
+          T1, B, A, P(ll), P(lb), P(bl), P(act), P(rew), P(dn), None, P(ids), TASKS, ctypes.byref(cfg), P(ecp),
+          P(kmom), P(kcomp), P(o['loss_terms']), P(o['dlogits']), P(o['dbaseline']), P(o['d_entropy_cost_param']),
+          None, None, P(td), P(ksums), P(kerr), P(kscratch), _lib.stream_ptr()))
+
+    def tasks_phase2():
+      _lib.check(L.seedrl_vtrace_popart_tasks_update(
+          T1, B, TASKS, 1e-2, 0.5, P(lb), P(td), P(ids), P(ksums), P(kmom), P(kcomp), P(o['dbaseline']), P(kdcomp),
+          P(o['loss_terms']), P(kscratch), _lib.stream_ptr()))
     row = {'B': B}
-    for name, fn in (('plain_loss_ms', plain), ('popart_phase1_ms', phase1), ('popart_phase2_ms', phase2)):
+    for name, fn in (('plain_loss_ms', plain), ('popart_phase1_ms', phase1), ('popart_phase2_ms', phase2),
+                     ('tasks%d_phase1_ms' % TASKS, tasks_phase1), ('tasks%d_phase2_ms' % TASKS, tasks_phase2)):
       for _ in range(3):
         fn()
       row[name] = events_ms(fn, 20)
+    assert int(kerr.item()) == 0
     out.append(row)
   return out
 
