@@ -9,7 +9,9 @@ gradients, in a numpy dtype (float64: the yardstick of the GPU tests; float32: t
 
   1. m = mu1, s = clip(sqrt(mu2 - mu1^2), 1e-6, 1e6)
   2. u = s (sigma V + mu) + m over all T+1 rows
-  3. V-trace on values u[:-1], bootstrap u[-1] -> vs, pg_adv
+  3. V-trace on values u[:-1], bootstrap u[-1] -> vs, pg_adv; with an abandoned mask [T+1,B], the masked V-trace
+     of tests/abandoned_float64_reference.py on abandoned[1:] (transition t masked iff row t+1 is abandoned), in
+     float32 the same recursion with those transitions masked
   4. n = (vs - m) / s, a = pg_adv / s
   5. mu1' = mu1 + beta (mean vs - mu1), mu2' = mu2 + beta (mean vs^2 - mu2), over all replicas
   6. sigma+ = (s / s') sigma, mu+ = (m - m' + s mu) / s'
@@ -18,6 +20,7 @@ gradients, in a numpy dtype (float64: the yardstick of the GPU tests; float32: t
 """
 import numpy as np
 
+import abandoned_float64_reference as AR
 import vtrace_float64_reference as RF
 
 
@@ -82,8 +85,42 @@ def _log_softmax(x):
   return z - np.log(np.exp(z).sum(-1, keepdims=True))
 
 
-def moment_sums(cfg, ll, lb, bl, act, rew, done, state, FT=np.float64):
-  """Steps 1-3 on one replica's batch: -> (sum vs, sum vs^2, vs, pg_adv, u)."""
+def _masked_recursion(masked):
+  """vtrace_float64_reference's recursion in dtype FT with no delta and no policy gradient at the transitions
+  `masked` [T,B]: the rounding of the masked V-trace in float32."""
+  def f(target_action_log_probs, behaviour_action_log_probs, discounts, rewards, values, bootstrap_value, FT,
+        lambda_=1.0):
+    rhos = np.exp(np.asarray(target_action_log_probs, FT) - np.asarray(behaviour_action_log_probs, FT))
+    discounts, rewards, values = (np.asarray(a, FT) for a in (discounts, rewards, values))
+    boot = np.asarray(bootstrap_value, FT)
+    keep = (~masked).astype(FT)
+    clipped = np.minimum(FT(1.0), rhos) * keep
+    cs = np.minimum(FT(1.0), rhos) * FT(lambda_)
+    deltas = clipped * (rewards + discounts * np.concatenate([values[1:], boot[None]], 0) - values)
+    acc = np.zeros_like(boot)
+    out = [None] * len(deltas)
+    for i in range(len(deltas) - 1, -1, -1):
+      acc = deltas[i] + discounts[i] * cs[i] * acc
+      out[i] = acc
+    vs = np.stack(out, 0) + values
+    pg = clipped * (rewards + discounts * np.concatenate([vs[1:], boot[None]], 0) - values)
+    return vs.astype(FT), pg.astype(FT)
+  return f
+
+
+def _vtrace(abandoned, FT):
+  """Step 3's V-trace: vtrace_float64_reference's recursion; with a mask that has an abandoned transition, in
+  float64 the masked definition of abandoned_float64_reference, in any other dtype the recursion with those
+  transitions masked.  A mask without one is no mask, so that an all-false mask gives the unmasked composition
+  bit for bit."""
+  if abandoned is None or not np.asarray(abandoned, bool)[1:].any():
+    return RF.vtrace_from_importance_weights
+  masked = np.asarray(abandoned, bool)[1:]
+  return AR.masked_vtrace(masked) if FT == np.float64 else _masked_recursion(masked)
+
+
+def moment_sums(cfg, ll, lb, bl, act, rew, done, state, FT=np.float64, abandoned=None):
+  """Steps 1-3 on one replica's batch: -> (sum vs, sum vs^2, vs, pg_adv, u).  abandoned: bool [T+1,B] or None."""
   mu1, mu2, sigma, mu = (FT(x) for x in state)
   s = FT(np.clip(np.sqrt(FT(mu2 - mu1 * mu1)), 1e-6, 1e6))
   m = mu1
@@ -97,20 +134,22 @@ def moment_sums(cfg, ll, lb, bl, act, rew, done, state, FT=np.float64):
   disc = (~np.asarray(done, bool)[1:]).astype(FT) * FT(cfg.discounting)
   tl = np.take_along_axis(_log_softmax(ll[:-1]), a[..., None], -1)[..., 0]
   blp = np.take_along_axis(_log_softmax(bl[:-1]), a[..., None], -1)[..., 0]
-  vs, pg = RF.vtrace_from_importance_weights(tl, blp, disc, r, u[:-1], u[-1], FT, lambda_=cfg.lambda_)
+  vs, pg = _vtrace(abandoned, FT)(tl, blp, disc, r, u[:-1], u[-1], FT, lambda_=cfg.lambda_)
   return vs.sum(dtype=np.float64), (vs.astype(np.float64) ** 2).sum(), vs, pg, u
 
 
-def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, state, beta, FT=np.float64, global_means=None):
+def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, state, beta, FT=np.float64, global_means=None,
+                   abandoned=None):
   """Steps 1-9 in dtype FT.  state = (mu1, mu2, sigma, mu) before the step; global_means = (mean vs,
-  mean vs^2) over every replica's batch (default: this batch alone).  Returns a dict: loss terms by
-  their learner names, dlogits, dbaseline, dcomp = (d sigma, d mu), state (after the step), vs, pg_adv."""
+  mean vs^2) over every replica's batch (default: this batch alone); abandoned = bool [T+1,B] or None.
+  Returns a dict: loss terms by their learner names, dlogits, dbaseline, dcomp = (d sigma, d mu), state
+  (after the step), vs, pg_adv, and sums = (sum vs, sum vs^2, rows) of this batch."""
   mu1, mu2, sigma, mu = (FT(x) for x in state)
   ll, lb = np.asarray(ll, FT), np.asarray(lb, FT)
   T1, B, A = ll.shape
   T = T1 - 1
   N = T * B
-  s1, s2, vs, pg, u = moment_sums(cfg, ll, lb, bl, act, rew, done, state, FT)
+  s1, s2, vs, pg, u = moment_sums(cfg, ll, lb, bl, act, rew, done, state, FT, abandoned)
   if global_means is None:
     global_means = (s1 / N, s2 / N)
   s = FT(np.clip(np.sqrt(FT(mu2 - mu1 * mu1)), 1e-6, 1e6))
@@ -159,4 +198,4 @@ def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, state, beta, FT=np.floa
            'max_action_abs': float(np.abs(a).max()), 'popart_mean': mu1n, 'popart_std': sn}
   return dict(terms=terms, dlogits=dl, dbaseline=db, dcomp=dcomp, d_entropy_cost_param=dep,
               state=np.array([mu1n, mu2n, sigma_n, mu_n], FT), vs=vs, pg_adv=pg, td=(vs - u[:-1]) / s,
-              u=u, n=n, adv=adv, e=e)
+              u=u, n=n, adv=adv, e=e, sums=np.array([s1, s2, N], np.float64))

@@ -19,15 +19,17 @@ def _columns(arrays, cols):
   return [np.ascontiguousarray(np.asarray(x)[:, cols]) for x in arrays]
 
 
-def task_sums(cfg, ll, lb, bl, act, rew, done, states, task_ids, FT=np.float64):
-  """[K,3] float64 (sum vs, sum vs^2, rows) of one replica's batch, each task over its own columns."""
+def task_sums(cfg, ll, lb, bl, act, rew, done, states, task_ids, FT=np.float64, abandoned=None):
+  """[K,3] float64 (sum vs, sum vs^2, rows) of one replica's batch, each task over its own columns (and its
+  columns of the abandoned mask [T+1,B], if any)."""
   states = np.asarray(states)
   out = np.zeros((len(states), 3))
   T = np.asarray(ll).shape[0] - 1
   for k in range(len(states)):
     cols = np.nonzero(np.asarray(task_ids) == k)[0]
     if cols.size:
-      s1, s2 = PR.moment_sums(cfg, *_columns((ll, lb, bl, act, rew, done), cols), states[k], FT)[:2]
+      sub = _columns((ll, lb, bl, act, rew, done) + (() if abandoned is None else (abandoned,)), cols)
+      s1, s2 = PR.moment_sums(cfg, *sub[:6], states[k], FT, *sub[6:])[:2]
       out[k] = (s1, s2, T * cols.size)
   return out
 
@@ -39,17 +41,18 @@ def _updated(state, means, beta, FT):
   return pa.state
 
 
-def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, states, task_ids, beta, FT=np.float64, global_sums=None):
+def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, states, task_ids, beta, FT=np.float64, global_sums=None,
+                   abandoned=None):
   """states [K,4] = (mu1, mu2, sigma, mu) per task before the step; task_ids [B]; global_sums [K,3] over every
-  replica (default: this batch's task_sums).  Returns what popart_reference.loss_and_grads returns, with
-  dcomp [K,2], state [K,4] and sums [K,3] (this batch's)."""
+  replica (default: this batch's task_sums); abandoned = bool [T+1,B] or None.  Returns what
+  popart_reference.loss_and_grads returns, with dcomp [K,2], state [K,4] and sums [K,3] (this batch's)."""
   states = np.asarray(states, FT)
   K = len(states)
   task_ids = np.asarray(task_ids)
   ll = np.asarray(ll, FT)
   T1, B, A = ll.shape
   N = (T1 - 1) * B
-  sums = task_sums(cfg, ll, lb, bl, act, rew, done, states, task_ids, FT)
+  sums = task_sums(cfg, ll, lb, bl, act, rew, done, states, task_ids, FT, abandoned)
   if global_sums is None:
     global_sums = sums
   dl, db = np.zeros_like(ll), np.zeros((T1, B), FT)
@@ -68,8 +71,9 @@ def loss_and_grads(cfg, ll, lb, bl, act, rew, done, ecp, states, task_ids, beta,
       if means is not None:
         new[k] = _updated(states[k], means, beta, FT)
       continue
-    sub = _columns((ll, lb, bl, act, rew, done), cols)
-    r = PR.loss_and_grads(cfg, *sub, ecp, states[k], beta, FT, global_means=means)
+    sub = _columns((ll, lb, bl, act, rew, done) + (() if abandoned is None else (abandoned,)), cols)
+    r = PR.loss_and_grads(cfg, *sub[:6], ecp, states[k], beta, FT, global_means=means,
+                          abandoned=sub[6] if abandoned is not None else None)
     w = FT(cols.size * (T1 - 1)) / FT(N)       # the task's share of the rows
     dl[:, cols] = r['dlogits'] * w
     db[:, cols] = r['dbaseline'] * w

@@ -1,12 +1,14 @@
 """CPU: the PopArt restatement of tests/popart_reference.py against the reference's popart_test.py cases, the
-float64 composition's own consistency (autograd, and the plain loss at beta = 0), the flags and their defaults,
-and the checkpoint check that keeps PopArt and non-PopArt learner states apart."""
+float64 composition's own consistency (autograd, and the plain loss at beta = 0, with and without an abandoned
+mask), the flags and their defaults, and the checkpoint check that keeps PopArt and non-PopArt learner states
+apart."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
+import abandoned_float64_reference as AR
 import popart_reference as PR
 import vtrace_float64_reference as RF
 from seed_rl_b200.agents.vtrace import learner
@@ -181,6 +183,75 @@ def test_composition_at_beta0_is_the_plain_loss():
   np.testing.assert_allclose(r['dbaseline'], db, rtol=1e-12, atol=1e-18)
   np.testing.assert_allclose(r['terms']['total'], total, rtol=1e-12)
   np.testing.assert_array_equal(r['state'], [0, 1, 1, 0])
+
+
+def _masked_batch(seed, T1=9, B=6):
+  ll, lb, bl, act, rew, done = _batch(T1=T1, B=B, seed=seed)
+  done_m, ab = AR.masks(T1, B, seed + 1, p_done=0.0)
+  return (ll, lb, bl, act, rew, done | done_m), ab
+
+
+@pytest.mark.parametrize('FT', [np.float32, np.float64])
+def test_composition_without_abandonment_ignores_the_mask(FT):
+  """abandoned=None and an all-false mask: the composition is the same bit for bit."""
+  b, _ = _masked_batch(seed=4)
+  cfg = learner.default_loss_settings(popart=True, lambda_=0.95)
+  state = np.array([40.0, 5000.0, 0.7, 0.2], np.float32)
+  r0 = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3, FT=FT)
+  r1 = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3, FT=FT, abandoned=np.zeros(b[5].shape, bool))
+  for key in ('dlogits', 'dbaseline', 'dcomp', 'state', 'vs', 'pg_adv', 'u', 'e', 'sums'):
+    np.testing.assert_array_equal(r1[key], r0[key], err_msg=key)
+  for name in r0['terms']:
+    assert r1['terms'][name] == r0['terms'][name], name
+
+
+def test_masked_composition_takes_the_masked_vtrace():
+  """With abandoned transitions: vs = u and pg_adv = 0 exactly on the masked ones, every other output moves,
+  and the moment sums are those of the masked vs."""
+  b, ab = _masked_batch(seed=5)
+  cfg = learner.default_loss_settings(popart=True, lambda_=0.95)
+  state = np.array([40.0, 5000.0, 0.7, 0.2], np.float32)
+  r = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3, abandoned=ab)
+  plain = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3)
+  m = ab[1:]
+  assert m[0, 0] and m[-1, 1 % 6] and m.sum() >= 3
+  np.testing.assert_array_equal(r['vs'][m], r['u'][:-1][m])
+  assert np.all(r['pg_adv'][m] == 0) and not np.all(plain['pg_adv'][m] == 0)
+  assert not np.array_equal(r['dbaseline'], plain['dbaseline']) and not np.array_equal(r['state'], plain['state'])
+  np.testing.assert_allclose(r['sums'], [r['vs'].sum(), (r['vs'] ** 2).sum(), r['vs'].size], rtol=1e-12)
+
+
+def test_masked_float32_composition_is_the_float64_one_rounded():
+  """The float32 composition's masked recursion against the float64 definition: the same targets to float32
+  rounding, masked transitions included."""
+  b, ab = _masked_batch(seed=7)
+  cfg = learner.default_loss_settings(popart=True, lambda_=0.95)
+  state = np.array([40.0, 5000.0, 0.7, 0.2], np.float32)
+  r32 = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3, FT=np.float32, abandoned=ab)
+  r64 = PR.loss_and_grads(cfg, *b, -1.0, state, 0.3, abandoned=ab)
+  for key in ('vs', 'pg_adv', 'dbaseline', 'state'):
+    _close(key, r32[key], r64[key], 1e-5)
+  assert np.all(r32['pg_adv'][ab[1:]] == 0)
+
+
+def test_masked_composition_at_beta0_is_the_masked_plain_loss(monkeypatch):
+  """beta = 0 from the initial state, with an abandoned mask: the plain loss of tests/test_gpu_abandoned.py (the
+  float64 loss with its V-trace replaced by the masked one)."""
+  b, ab = _masked_batch(seed=6)
+  kw = dict(discounting=0.97, lambda_=0.95, kl_cost=0.01)
+  r = PR.loss_and_grads(learner.default_loss_settings(popart=True, **kw), *b, -0.8,
+                        np.array([0, 1, 1, 0], np.float32), 0.0, abandoned=ab)
+  monkeypatch.setattr(RF, 'vtrace_from_importance_weights', AR.masked_vtrace(ab[1:]))
+  total, logs, dl, db, dep, vs, pg = RF.loss_and_grads(learner.default_loss_settings(**kw), *b, -0.8, torch.float64)
+  np.testing.assert_allclose(r['vs'], vs, rtol=1e-12, atol=1e-15)
+  np.testing.assert_allclose(r['pg_adv'], pg, rtol=1e-12, atol=1e-15)
+  np.testing.assert_allclose(r['dlogits'], dl, rtol=1e-12, atol=1e-18)
+  np.testing.assert_allclose(r['dbaseline'], db, rtol=1e-12, atol=1e-18)
+  np.testing.assert_allclose(r['terms']['total'], total, rtol=1e-12)
+  for name, key in learner._LOG_NAMES:
+    np.testing.assert_allclose(r['terms'][key], logs[name], rtol=1e-12, atol=1e-15, err_msg=name)
+  np.testing.assert_array_equal(r['state'], [0, 1, 1, 0])
+  assert np.all(db[:-1][ab[1:]] == 0)
 
 
 # ---- flags and settings -----------------------------------------------------------------------------------------

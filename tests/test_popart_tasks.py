@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import abandoned_float64_reference as AR
 import popart_reference as PR
 import popart_tasks_reference as PT
 from seed_rl_b200.agents.vtrace import learner
@@ -82,6 +83,51 @@ def test_one_task_is_the_single_task_composition(FT):
   np.testing.assert_array_equal(r['state'][0], ref['state'])
   for name in ('total', 'policy', 'V', 'entropy', 'kl', 'v_l2_error', 'v_mean', 'mean_entropy', 'mean_kl'):
     assert r['terms'][name] == ref['terms'][name], name
+
+
+@pytest.mark.parametrize('FT', [np.float32, np.float64])
+def test_one_task_with_a_mask_is_the_single_task_composition(FT):
+  rng = np.random.default_rng(6)
+  batch = _batch(rng)
+  done, ab = AR.masks(9, 10, 7, p_done=0.0)
+  batch = batch[:5] + (batch[5] | done,)
+  cfg = learner.default_loss_settings(popart=True, lambda_=0.95)
+  state = np.array([3.0, 40.0, 1.2, -0.1], FT)
+  ref = PR.loss_and_grads(cfg, *batch, -7.0, state, 0.05, FT, abandoned=ab)
+  r = PT.loss_and_grads(cfg, *batch, -7.0, state[None], np.zeros(10, np.int32), 0.05, FT, abandoned=ab)
+  assert not np.array_equal(ref['vs'], PR.loss_and_grads(cfg, *batch, -7.0, state, 0.05, FT)['vs'])
+  for key in ('dlogits', 'dbaseline', 'vs', 'pg_adv', 'td'):
+    np.testing.assert_array_equal(r[key], ref[key])
+  np.testing.assert_array_equal(r['dcomp'][0], ref['dcomp'])
+  np.testing.assert_array_equal(r['state'][0], ref['state'])
+  np.testing.assert_array_equal(r['sums'][0], ref['sums'])
+  for name in ('total', 'policy', 'V', 'entropy', 'kl', 'v_l2_error', 'v_mean', 'mean_entropy', 'mean_kl'):
+    assert r['terms'][name] == ref['terms'][name], name
+
+
+def test_each_task_sees_its_own_columns_of_the_mask():
+  """Two tasks with a mask: each task's outputs are the single-task composition on its columns of every input,
+  the mask included; a task whose columns hold no abandoned transition is its unmasked composition."""
+  rng = np.random.default_rng(8)
+  batch = _batch(rng)
+  ids = np.array([0, 0, 0, 1, 0, 1, 1, 1, 1, 1], np.int32)
+  done, ab = AR.masks(9, 10, 9, p_done=0.0)
+  ab[:, ids == 1] = False
+  batch = batch[:5] + (batch[5] | done,)
+  states = np.array([[3.0, 40.0, 1.2, -0.1], [30.0, 1000.0, 0.9, 0.2]])
+  cfg = learner.default_loss_settings(popart=True, lambda_=0.95)
+  r = PT.loss_and_grads(cfg, *batch, -7.0, states, ids, 0.05, abandoned=ab)
+  for k, has_ab in ((0, True), (1, False)):
+    cols = np.nonzero(ids == k)[0]
+    sub = [np.ascontiguousarray(x[:, cols]) for x in batch + (ab,)]
+    one = PR.loss_and_grads(cfg, *sub[:6], -7.0, states[k], 0.05, abandoned=sub[6] if has_ab else None)
+    assert sub[6][1:].any() == has_ab
+    for key in ('vs', 'pg_adv', 'td', 'e'):
+      np.testing.assert_array_equal(r[key][:, cols], one[key], err_msg='%s %d' % (key, k))
+    np.testing.assert_array_equal(r['state'][k], one['state'])
+  masked = ab[1:]
+  assert np.all(r['pg_adv'][masked] == 0)
+  np.testing.assert_array_equal(r['vs'][masked], r['u'][:-1][masked])
 
 
 def test_flag_and_settings_defaults():
